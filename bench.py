@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """bench.py -- voxels/s of full-texture-suite voxel-based extraction (BASELINE.json metric, config 3).
 
-A "step" is one pass of the hot path over the whole synthetic 512^3 volume: GLCM + GLRLM + GLSZM + GLDM + NGTDM fused
-kernels -> 75 float64 feature maps (reference dtypes), kernelRadius 1, Ng 32.
+A "step" is one pass of the hot path over the whole synthetic 256^3 volume (the size of a 1 mm isotropic brain MRI): GLCM +
+GLRLM + GLSZM + GLDM + NGTDM fused kernels -> 75 float64 feature maps (reference dtypes), kernelRadius 1, Ng 32.  At 256^3
+the maps are 10 GB on the device and, through the plugin call, 10 GB of page-locked host memory.
   value  : device-resident (levels in HBM -> maps in HBM), CUDA events, max over ranks
   e2e    : the same through the reference-facing PLUGIN call with HOST buffers: raw int16 image + mask ->
            Radiomics{GLCM,GLRLM,GLSZM,GLDM,NGTDM}(image, mask, voxelBased=True, binWidth=25).execute() -> 75 float64
@@ -15,9 +16,11 @@ kernels -> 75 float64 feature maps (reference dtypes), kernelRadius 1, Ng 32.
            the numpy feature restatement) at the north-star tolerance 1e-5; `deterministic`: the step is run twice more
            and every map compared bit for bit
   secondary : the smooth volume (same metric), config 2 (GLCM-only 256^3), config 4 (wavelet + LoG -> bin -> suite,
-           12 images at 512^3) and config 5(ii) (batch of 64 independent 256^3 cases, segment-based suite, sharded by case)
+           12 images at --size^3) and config 5(ii) (batch of 64 independent 256^3 cases, segment-based suite, sharded by case)
   --impl reference : the reference's own CPU path (compiled `_cmatrices` from oracle/_ref for the matrices + the numpy
            feature restatement) on the host cores, bounded voxel sample per step.
+  --dump-outputs DIR : after the timed steps, the maps of the last step at a fixed seeded sample of DUMP_VOXELS centre
+           voxels, one float64 array [features, voxels] per class -> DIR/<class>.npy (feature order: rb_feature_name)
 """
 from __future__ import annotations
 
@@ -42,6 +45,7 @@ ALG_BYTES = {"glcm": 5 + 8 * 24, "glrlm": 5 + 8 * 16, "glszm": 5 + 8 * 16, "gldm
 CLASSES = ("glcm", "glrlm", "glszm", "gldm", "ngtdm")
 METRIC = "voxels/s full-texture voxel-based"
 RTOL, ATOL = 1e-5, 1e-9
+DUMP_VOXELS = 1 << 16          # 75 maps x 65536 voxels x 8 B = 39 MB
 
 
 def synth_volume(n, kind):
@@ -75,7 +79,7 @@ def sample_voxels(n, count, seed):
 _CPU = {}
 # the CPU arm is the reference's compiled C for the matrices but the numpy RESTATEMENT for the features (the reference's
 # Python feature classes need SimpleITK / pywt, absent here and on the GPU box): labelled "port", the weaker claim
-CPU_ARM_DETAIL = {"reference": "matrices: the unmodified reference _cmatrices compiled from /root/reference (oracle/_ref); "
+CPU_ARM_DETAIL = {"reference": "matrices: the unmodified reference _cmatrices compiled by oracle/build_ref.py (oracle/_ref); "
                                "features: numpy restatement oracle/features_np.py",
                   "port": "matrices: C restatement oracle/cmatrices_port.c; features: numpy restatement oracle/features_np.py"}
 
@@ -176,7 +180,7 @@ def workload_config(args):
     return {"workload": f"full suite GLCM+GLRLM+GLSZM+GLDM+NGTDM voxel-based, synthetic {args.size}^3 Ng=32 "
                         f"kernelRadius=1 ({args.kind} levels), 75 float64 maps",
             "size": args.size, "Ng": 32, "kernelRadius": 1, "levels": args.kind,
-            "l2": "inputs+outputs (>=25 GB per class) far exceed the 126 MB L2; no flush needed",
+            "l2": "inputs+outputs (>= 0.67 GB per class at 256^3) far exceed the 50 MB L2; no flush needed",
             "parallelism": f"z-slabs x{args.gpus}" if args.gpus > 1 else "single GPU"}
 
 
@@ -215,6 +219,19 @@ class ClockSampler:
         mx = max((float(r[2]) for r in self.rows if len(r) >= 8 and r[2].replace(".", "").isdigit()), default=None)
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons),
                 "samples": len(sm)}
+
+
+def gpu_info(gpu_index):
+    """the card a number was measured on: name and the power limit it ran under"""
+    import torch
+    info = {"name": torch.cuda.get_device_name(gpu_index), "power_limit_w": None}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_w"] = float(q.stdout.strip())
+    except (OSError, ValueError, subprocess.SubprocessError):
+        pass
+    return info
 
 
 # ----------------------------------------------------------------------------------- GPU arm
@@ -282,7 +299,28 @@ def parity_of(outs, z0, vox, feats):
             "oracle": "oracle/_ref compiled reference _cmatrices + oracle/features_np.py"}
 
 
-def measure_suite(ctx, vol, steps, warmup, classes=CLASSES, oracle=None, check_determinism=True, sample_clocks=False):
+def dump_sample(outs, z0, n, vol_shape):
+    """{class: float64 [F, DUMP_VOXELS]}: the maps at a fixed seeded sample of centre voxels (every voxel when the volume has
+    fewer), gathered from the ranks' z-slabs"""
+    import torch
+    import torch.distributed as dist
+    Z, Y, X = vol_shape
+    idx = np.sort(np.random.default_rng(1234).choice(Z * Y * X, size=min(DUMP_VOXELS, Z * Y * X), replace=False))
+    z, y, x = np.unravel_index(idx, vol_shape)
+    dev = next(iter(outs.values())).device
+    own = torch.from_numpy((z >= z0) & (z < z0 + n)).to(dev)
+    zi, yi, xi = (torch.from_numpy(a.astype(np.int64)).to(dev) for a in (np.clip(z - z0, 0, n - 1), y, x))
+    res = {}
+    for c, t in outs.items():
+        v = torch.where(own, t[:, zi, yi, xi], torch.zeros((), dtype=t.dtype, device=dev))
+        if dist.is_initialized():
+            dist.all_reduce(v)             # each voxel is owned by one rank, the others add zeros
+        res[c] = v.cpu().numpy().astype(np.float64)
+    return res
+
+
+def measure_suite(ctx, vol, steps, warmup, classes=CLASSES, oracle=None, check_determinism=True, sample_clocks=False,
+                  dump=False):
     """device-resident timing of the fused kernels over `vol` (levels), z-slabs over the ranks"""
     import torch
     from pyradiomics_b200 import _lib, distributed as D, voxel
@@ -341,6 +379,8 @@ def measure_suite(ctx, vol, steps, warmup, classes=CLASSES, oracle=None, check_d
     per_class_ms = {c: float(np.mean([a.elapsed_time(b) for a, b in ev[c]])) for c in classes}
     res = {"value": float(np.prod(vol.shape)) * steps / (ms * 1e-3), "ms_per_step": ms / steps, "per_class_ms": per_class_ms,
            "launches": launches[0], "clocks": clocks, "nz": nz}
+    if dump:
+        res["dump"] = dump_sample(outs, z0, nz, vol.shape)
     # ---- outside the timed region: bit-reproducibility and the sampled oracle comparison
     if check_determinism:
         same = True
@@ -541,7 +581,11 @@ def run_b200(args):
             oracle_s = (vox_s, feats_s)
 
     ctx = Ctx(args)
-    main = measure_suite(ctx, vol, args.steps, args.warmup, oracle=oracle, sample_clocks=True)
+    main = measure_suite(ctx, vol, args.steps, args.warmup, oracle=oracle, sample_clocks=True, dump=bool(args.dump_outputs))
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for c, a in main.pop("dump").items():
+            np.save(os.path.join(args.dump_outputs, f"{c}.npy"), a)
     value, per_class_ms, nz = main["value"], main["per_class_ms"], main["nz"]
     Z = args.size
 
@@ -552,7 +596,7 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     achieved = ALG_BYTES[dom] * (nz * Z * Z) / (per_class_ms[dom] * 1e-3) / 1e9
     traffic, traffic_src = None, None
     try:
@@ -565,7 +609,7 @@ def run_b200(args):
         pass
     roofline = {"bound": "hbm", "kernel": f"{dom} fused voxel kernels", "achieved": achieved, "peak": peak,
                 "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src,
-                "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "fallback 3350 GB/s (H100 SXM data sheet)",
                 "ms_per_launch": per_class_ms[dom], "per_class_ms": per_class_ms,
                 "suite_frac": 625.0 * value / ctx.world / 1e9 / peak,
                 "note": "issue-bound integer / fp64 kernels, not HBM-bound: see DESIGN.md section 4"}
@@ -590,7 +634,7 @@ def run_b200(args):
         secondary["config5ii_segment_batch"] = secondary_config5ii(ctx)
     if rank == 0:
         line = {
-            "metric": METRIC, "value": value, "unit": "voxels/s", "n_gpus": world, "steps": args.steps,
+            "metric": METRIC, "value": value, "unit": "voxels/s", "n_gpus": world, "gpu": gpu_info(local), "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": main["ms_per_step"], "higher_is_better": True, "scaling": "strong",
             "vs_baseline": None, "dtype": "f64", "data": "synthetic", "config": workload_config(args),
             "clocks": main["clocks"], "e2e": e2e, "gpu_launches": main["launches"], "roofline": roofline,
@@ -608,7 +652,7 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--size", type=int, default=512)
+    ap.add_argument("--size", type=int, default=256)
     ap.add_argument("--kind", default="uniform", choices=["uniform", "smooth"])
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--e2e-steps", type=int, default=2)
@@ -618,6 +662,7 @@ def main():
     ap.add_argument("--cpu-workers", type=int, default=64)
     ap.add_argument("--cpu-voxels-per-worker", type=int, default=96)
     ap.add_argument("--parity-voxels", type=int, default=20480)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

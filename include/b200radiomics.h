@@ -1,4 +1,4 @@
-/* b200radiomics -- C ABI of the B200-native texture-matrix engine (libb200radiomics.so).
+/* b200radiomics -- C ABI of the H100-native (sm_90a) texture-matrix engine (libb200radiomics.so).
  *
  * Drop-in boundary for the hot path of AIM-Harvard/pyradiomics (SURVEY.md section 8b): the C
  * functions of reference radiomics/src/cmatrices.h:1-8 and the per-voxel driver loops of

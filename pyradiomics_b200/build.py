@@ -1,4 +1,4 @@
-"""Builds libb200radiomics.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with
+"""Builds libb200radiomics.so in-tree with nvcc for sm_90a (no JIT cache: the .so travels with
 the repository snapshot to the GPU box)."""
 from __future__ import annotations
 
@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200radiomics.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-diag-suppress", "128",
 ]
 
@@ -51,7 +51,7 @@ def _compile_and_link(out: str, extra: list[str], objdir: str, verbose: bool = F
         for rc in ex.map(lambda j: subprocess.call(j[2], cwd=CSRC), jobs):
             if rc:
                 raise RuntimeError("nvcc failed")
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", out, *[j[1] for j in jobs]], cwd=CSRC)
+    subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", out, *[j[1] for j in jobs]], cwd=CSRC)
 
 
 def build(force: bool = False, verbose: bool = False) -> str:

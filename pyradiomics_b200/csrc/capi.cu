@@ -129,7 +129,7 @@ using namespace rb;
 extern "C" {
 
 const char* rb_last_error(void) { return last_error_ref().c_str(); }
-const char* rb_version(void) { return "b200radiomics 0.1 (sm_100a)"; }
+const char* rb_version(void) { return "b200radiomics 0.1 (sm_90a)"; }
 
 int rb_device_count(void) {
   int n = 0;
@@ -209,7 +209,10 @@ int rb_maps_to_f32_dev(const double* src_dev, long long src_pitch, float* dst_de
   if (width <= 0 || height <= 0) return RB_OK;
   const long long total = width * height;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (blocks > sms * 16LL) blocks = sms * 16LL;
   maps_to_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(src_dev, src_pitch, dst_dev, dst_pitch, width, height);
   RB_LAUNCH_CHECK();
   return RB_OK;

@@ -298,7 +298,7 @@ recursive_gauss_x_kernel(const TIn* __restrict__ in, long long nlines, int X, co
 }
 
 static int grid_n(long long n, int block, int per_sm) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long need = (n + block - 1) / block, cap = (long long)sms * per_sm;

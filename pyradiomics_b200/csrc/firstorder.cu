@@ -64,7 +64,7 @@ int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uin
   FoParams P{Z, Y, X, rz, ry, rx, z0, z1, out_z0, dtype, level_bytes, shift, voxel_volume, init_value};
   const long long total = (long long)(z1 - z0) * Y * X;
   if (total <= 0) return RB_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long need = (total + 127) / 128, cap = (long long)sms * 32;

@@ -359,7 +359,7 @@ RB_HD double glcm_fast_solve(const uint8_t* w, int ws, const TT& T, int s, int c
 }
 
 // size class of an eigen-task (number of level nodes) -- tasks of one class share a warp
-// (16 keys: n - 2, clamped; ncu showed 11 of 32 lanes active with 8 coarser classes because the loop
+// (16 keys: n - 2, clamped; with 8 coarser classes a third of the lanes stay active because the loop
 // lengths of the sparse solver follow n)
 constexpr int GF_NCLS = 16, GF_CLS_BITS = 4;
 RB_HD int glcm_task_class(int n) { return n <= 2 ? 0 : n >= 17 ? 15 : n - 2; }
@@ -406,7 +406,7 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
   // R(level) = number of matrix entries in its row = popcount(class & EA) + popcount(class & EB);
   // sum_levels R log2 R = sum over the 2n pair ends of log2 R(their level).
   // (Straight-line per-pair code on purpose: a loop over the classes with its shared-memory load in the carried
-  // dependence measured 25 % slower for the whole kernel -- 8 to 16 warps per SM cannot hide a 30-cycle chain per class.)
+  // dependence is slower -- 8 to 16 warps per SM cannot hide a 30-cycle chain per class.)
   double rl = 0;
   uint32_t reps = 0, all = 0, comp = 0;
   uint32_t em[NP];
@@ -469,7 +469,11 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
   // scan the sorted keys: runs of equal key1 = merged matrix entries (length nn), runs of equal
   // a+b = p_{x+y} bins, runs of equal key2 = p_{x-y} bins (the |i-j| table features are taken per run)
   double cs = 0, cp = 0, idm = 0, idmn = 0, id = 0, idn = 0, inv = 0, lgE = 0, lgD = 0, lgS = 0;
-  int E2 = 0, cmax = 0, runK = 0, runS = 0, runD = 0;
+  // a run's length is its end minus its start index.  (The same sums written with three counters incremented per element
+  // and reset at run ends gave wrong DifferenceEntropy and SumEntropy maps on an H100 when built for sm_90a with
+  // -Xptxas -O2 or -O3 -- tests/test_voxel_gpu.py::test_glcm_fast_path_equals_generic_kernel failed -- and the right ones
+  // with -Xptxas -O1.)
+  int E2 = 0, cmax = 0, startK = 0, startS = 0, startD = 0;
 #pragma unroll
   for (int i = 0; i < NP; i++) {
     if (i < n) {
@@ -479,20 +483,25 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
       const int nx1 = (i + 1 < NP) ? key1[i + 1 < NP ? i + 1 : i] : -1;
       const int nx2 = (i + 1 < NP) ? key2[i + 1 < NP ? i + 1 : i] : -1;
       const bool last = (i + 1 == n);
-      runK++; runS++; runD++;
       if (last || nx1 != k1) {                 // end of a merged-entry run
+        const int runK = i + 1 - startK;
         const int c = kd ? runK : 2 * runK;    // count of the matrix entry (both orders when i != j)
         E2 += kd ? 2 * runK * runK : 4 * runK * runK;
         if (c > cmax) cmax = c;
         lgE += runK * T.log2t[c];
-        runK = 0;
+        startK = i + 1;
       }
-      if (last || (nx1 >> 8) != ks) { lgS += runS * T.log2t[2 * runS]; runS = 0; }
+      if (last || (nx1 >> 8) != ks) {
+        const int runS = i + 1 - startS;
+        lgS += runS * T.log2t[2 * runS];
+        startS = i + 1;
+      }
       if (last || nx2 != k2) {                 // end of a |i-j| bin
+        const int runD = i + 1 - startD;
         const double r = (double)runD;
         lgD += r * T.log2t[2 * runD];
         idm += r * T.idm[k2]; idmn += r * T.idmn[k2]; id += r * T.id[k2]; idn += r * T.idn[k2]; inv += r * T.inv[k2];
-        runD = 0;
+        startD = i + 1;
       }
     }
   }
@@ -545,7 +554,7 @@ RB_HD uint32_t glcm_fast_voxel_phaseA(const uint8_t* w, int ws, uint32_t* eq, in
   acc.n_ok = 0; acc.n_imc2 = 0; acc.ja_nan = false; acc.tasks = 0; acc.tcls = 0;
   // RB_ANGLE_SYNC: on the device the block re-converges before every angle so that its warps walk
   // the (large, fully unrolled) angle bodies together and share instruction-cache lines -- without
-  // it the kernel is instruction-fetch bound (ncu: 15 "no_instruction" stall cycles per issue).
+  // it the kernel is instruction-fetch bound.
   for (int s = 0; s < 3; s++) { RB_ANGLE_SYNC(); glcm_fast_angle<18>(w, ws, eq, es, T, s, P, acc); }
   for (int s = 3; s < 9; s++) { RB_ANGLE_SYNC(); glcm_fast_angle<12>(w, ws, eq, es, T, s, P, acc); }
   for (int s = 9; s < 13; s++) { RB_ANGLE_SYNC(); glcm_fast_angle<8>(w, ws, eq, es, T, s, P, acc); }

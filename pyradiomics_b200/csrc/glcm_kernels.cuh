@@ -45,8 +45,7 @@ struct GlcmTask {
 #endif
 #ifndef GF_LZ_TOPUP
 #define GF_LZ_TOPUP 0              // 1: a size group's last batch is topped up with tasks of the next smaller group (needs
-                                   // LZ_EIG_EXACT_STATIC = 0 for reproducible bits).  Measured on B200, 256^3 GLCM: top-up + task-sized
-                                   // search 48.5 / 96.5 ms (uniform / smooth), no top-up + static search 46.3 / 93.0 ms
+                                   // LZ_EIG_EXACT_STATIC = 0 for reproducible bits)
 #endif
 static_assert(!(GF_LZ_TOPUP && LZ_EIG_EXACT_STATIC), "topped-up batches need the task-sized eigenvalue search (LZ_EIG_EXACT_STATIC=0): "
                                                       "otherwise a task's bits depend on the template that happens to solve it");
@@ -122,14 +121,13 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
                        const GlcmFastTables* __restrict__ Tg, const GlcmTask* __restrict__ queue,
                        const unsigned* __restrict__ qcount, double* __restrict__ res, int only) {
   // only = 0: every size group of this kind; else just the group of that template size (one launch per group keeps ONE
-  // solver body in the instruction cache at a time: ncu showed 7 no_instruction stall cycles per issue on smooth volumes,
-  // where the blocks of an SM sit in different groups)
+  // solver body in the instruction cache at a time: on smooth volumes the blocks of an SM sit in different groups)
   __shared__ GlcmSolveTables T;
   if (threadIdx.x == 0) glcm_solve_tables_from(*Tg, T);
   __syncthreads();
   const unsigned n = *qcount;
   // Tiles of GF_SOLVE_TILE (4096) consecutive tasks are counting-sorted by size class in shared memory, so the
-  // lanes of a warp run solves of the same size (ncu: 11-14 of 32 lanes active otherwise).  The sort is STABLE and
+  // lanes of a warp run solves of the same size (otherwise a third of the lanes stay active).  The sort is STABLE and
   // atomic-free (per-thread counts, one serial scan per class), so the position of a task -- and with it the batch and,
   // for topped-up Lanczos batches, the size template that solves it -- is the same in every run: bit-reproducible maps.
   constexpr int TILE = GF_SOLVE_TILE;
@@ -193,8 +191,8 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
       if (!only || only == 14) lanczos_group<14>(lev, P, T, queue, res, order, base, 0, e14b, lz_scratch);
     } else {
       // dense solves: one template size at a time, block-uniform (idle threads run on an empty window), so the
-      // barriers inside glcm_small_solve keep the warps on the same code (ncu: 8-10 no_instruction stall cycles
-      // per issue with free-running warps -- these bodies are 2-10 k straight-line instructions)
+      // barriers inside glcm_small_solve keep the warps on the same code (free-running warps stall on instruction
+      // fetch -- these bodies are 2-10 k straight-line instructions)
       if (KIND == 0) {
         if (!only || only == 4) solve_group<4>(lev, P, T, queue, res, order, base, 0, bucket[2]);
         if (!only || only == 6) solve_group<6>(lev, P, T, queue, res, order, base, bucket[2], bucket[4]);

@@ -3,8 +3,8 @@
 // level graph is connected and not bipartite (phase A filters those), D = diag(row sums R).
 //
 // Replaces round 1's glcm_fast_solve_task for these tasks.  That solver kept ~0.7 KB of float Lanczos
-// scratch per thread in local memory with dynamic indexing everywhere: ncu showed 12.4 long-scoreboard
-// stall cycles per issue, 18 of 32 lanes active and 510 B/voxel of scratch write-back to DRAM.  Here:
+// scratch per thread in local memory with dynamic indexing everywhere: long-scoreboard stalls, divergent
+// lanes and the scratch written back to DRAM.  Here:
 //   * the window is loaded PERMUTED so that the angle axis is the fastest window coordinate: the 18 pairs
 //     are the static position pairs (p, p+1), p % 3 < 2 -- no per-slot tables, all pair code is unrolled;
 //   * level classes are 27-bit position masks (__vcmpeq4 on the packed window), node i = i-th class in
@@ -39,8 +39,8 @@ constexpr uint32_t LZ_LOW = 0x36DB6DBu;       // window positions p (a*9 + b*3 +
 #endif
 #ifndef LZ_SEGSUM
 #define LZ_SEGSUM 0                // 1: neighbour sums by a segmented scan over node-sorted endpoint lists (no smem read-modify-write
-                                   // chain; bit-identical).  Measured SLOWER on B200 (256^3 uniform GLCM 51.6 vs 47.9 ms): the unrolled
-                                   // 36-entry scan pushes the kernel out of the instruction cache (no_instruction stalls 0.3 -> 2.3 per issue)
+                                   // chain; bit-identical).  Slower: the unrolled 36-entry scan pushes the kernel out of the
+                                   // instruction cache
 #endif
 constexpr int LZ_ACC = LZ_ACC_N;               // interleaved partial sums per reduction
 constexpr int LZ_NARR = 5;                    // per-thread shared arrays: U, S, IR, D, E (N doubles each)

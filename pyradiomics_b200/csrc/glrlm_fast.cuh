@@ -53,7 +53,7 @@ inline void glrlm_fast_build_tables(GlrlmFastTables& T) {
 // three more logic ops -- for all 27 voxels at once.  Everything else is popcounts per class.
 // (Round 2 tried a class-free formulation -- every quantity as a sum over the 27 run-end positions, no dynamically
 // indexed arrays: 511 instead of 645 warp instructions per voxel, but 4 fp64 accumulations per position and angle and
-// more shared-memory table lookups; measured 13.2 ms per 256^3 against 11.4 ms for this one, so it was dropped.)
+// more shared-memory table lookups; it was slower than this one and was dropped.)
 RB_HD void glrlm_fast_voxel(const int* wl, const GlrlmFastTables& T, double* out) {
   uint32_t e[27];
   RB_EQMASKS_27(wl, e);
@@ -61,7 +61,7 @@ RB_HD void glrlm_fast_voxel(const int* wl, const GlrlmFastTables& T, double* out
   // compact the level classes (data-dependent count): mask + level of each distinct level that occurs at least TWICE.
   // A level that occurs once is a run of length 1 along every angle: its share of every sum below is the same for the
   // 13 angles and is added once (S_*).  27 i.i.d. levels out of 32 have ~12 such singletons and ~7 repeated levels, so
-  // the per-angle class loops run ~7 instead of ~18 times (ncu: those loops were 62 % of the kernel's instructions).
+  // the per-angle class loops run ~7 instead of ~18 times (those loops are most of the kernel's instructions).
   uint32_t cls[13];                                       // at most 13 levels can occur twice among 27 voxels
   int clg[13];
   int nl = 0;

@@ -28,7 +28,7 @@ struct Vol {
 };
 
 static int grid_of(long long n, int block, int per_sm) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long need = (n + block - 1) / block, cap = (long long)sms * per_sm;

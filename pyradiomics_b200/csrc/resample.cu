@@ -172,7 +172,7 @@ resample_kernel(const void* __restrict__ src, int src_dt, const __grid_constant_
 }
 
 static int grid_rs(long long n, int block, int per_sm) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long need = (n + block - 1) / block, cap = (long long)sms * per_sm;

@@ -10,7 +10,7 @@
 //                     once per CTA with coalesced atomics.
 //   seg_glrlm_kernel  every voxel that ENDS a run (successor outside / unmasked / another level) walks back to the run's
 //                     start: all voxels work, loads coalesce along x (round 1: one thread per LINE start walked the
-//                     whole line -- 14 ms per 256^3, most of the volume's threads idle).  The reference's "angle without
+//                     whole line -- most of the volume's threads idle).  The reference's "angle without
 //                     a line of two voxels loses its length-1 column" rule (cmatrices.c:524-534) comes from a
 //                     pigeonhole count: some line holds two masked voxels <=> #masked voxels > #lines that hold any.
 //   ccl_*             GLSZM zones: union-find with the tile's equal-level neighbours merged in shared memory first.
@@ -35,8 +35,7 @@ struct SegVol {
 
 constexpr int ST_TX = 64, ST_THREADS = 256;
 // The staged box starts ST_XOFF columns left of the tile: TMA wants the innermost start coordinate 16-byte aligned (a box
-// at x0-1 faults with "illegal instruction", at x0-16 it loads and zero-fills: scripts/probes/tma_probe.cu,
-// profiles/r02_tma_probe.txt), and tiles start at multiples of 64.
+// at x0-1 faults with "illegal instruction", at x0-16 it loads and zero-fills), and tiles start at multiples of 64.
 constexpr int ST_XOFF = 16, ST_BX = ST_XOFF + ST_TX + 16;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -255,7 +254,7 @@ __global__ void ngtdm_seg_finish_kernel(const unsigned long long* __restrict__ a
 }
 
 static int sm_count() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;

@@ -187,7 +187,7 @@ shape_moments_kernel(const uint8_t* __restrict__ mask, int Z, int Y, int X, unsi
 }
 
 static int grid_for(long long work, int threads, int per_sm) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long need = (work + threads - 1) / threads, cap = (long long)sms * per_sm;
@@ -221,7 +221,7 @@ int shape_coefficients_dev(const uint8_t* mask_dev, int Z, int Y, int X, long lo
     if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_NOMEM, "shape: %llu mesh vertices do not fit", h.acc.nverts); }
     shape_mesh_kernel<<<grid, 256, 0, st>>>(mask_dev, Z, Y, X, sz, sy, sx, spacing[0], spacing[1], spacing[2], &d->acc, verts, &d->cursor);
     const long long nt = ((long long)h.acc.nverts + DT - 1) / DT;
-    shape_diameter_kernel<<<(int)(nt < 148 * 8 ? nt : 148 * 8), DT, 0, st>>>(verts, (long long)h.acc.nverts, spacing[0], spacing[1], spacing[2], d->dia);
+    shape_diameter_kernel<<<grid_for(nt, 1, 8), DT, 0, st>>>(verts, (long long)h.acc.nverts, spacing[0], spacing[1], spacing[2], d->dia);
     e = cudaMemcpyAsync(&h, d, sizeof(Dev), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     cudaFree(verts);
@@ -357,7 +357,7 @@ int shape2d_coefficients_dev(const uint8_t* mask_dev, int Y, int X, long long sy
     if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_NOMEM, "shape2D: %llu vertices do not fit", h.acc.nverts); }
     shape2d_kernel<<<grid, 256, 0, st>>>(mask_dev, Y, X, sy, sx, spacing[0], spacing[1], &d->acc, verts, &d->cursor);
     const long long nt = ((long long)h.acc.nverts + 255) / 256;
-    shape2d_diameter_kernel<<<(int)(nt < 148 * 8 ? nt : 148 * 8), 256, 0, st>>>(verts, (long long)h.acc.nverts, spacing[0], spacing[1], &d->best);
+    shape2d_diameter_kernel<<<grid_for(nt, 1, 8), 256, 0, st>>>(verts, (long long)h.acc.nverts, spacing[0], spacing[1], &d->best);
     e = cudaMemcpyAsync(&h, d, sizeof(Dev), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     cudaFree(verts);

@@ -94,7 +94,7 @@ int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P
   const long long plane = (long long)P.Y * P.X;
   if ((long long)(z1 - z0) * plane <= 0) return RB_OK;
   if (P.sy != P.X || P.sz != plane) return fail(RB_ERR_ARG, "GLCM fast path expects a contiguous level volume");
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   // chunk of planes whose worst-case queue (13 eigen-tasks per voxel) stays <= 48 Mi entries
@@ -110,10 +110,8 @@ int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P
     const long long total = (long long)(zb - za) * plane;
     RB_CUDA(cudaMemsetAsync(Q->count, 0, sizeof(unsigned), st));
     // phase A: one CTA per SM (register-bound).  512 threads at 128 registers (a hundred spilled words per thread, L1-
-    // resident) put 16 warps on an SM instead of the 8 of the 256-thread / 236-register build: measured 50.6 vs 62.5 ms
-    // per 256^3 (uniform), 104.7 vs 117.5 (smooth); 384 threads / 168 registers sit in between; 640 / 768 threads at 96 / 80
-    // registers (344 / 408 B of spills per thread) measured the same as 512 and were dropped again.  B200_GLCM_NT selects
-    // the variant for A/B runs.
+    // resident) put 16 warps on an SM instead of the 8 of the 256-thread / 236-register build, which hides more of the
+    // latency of this issue-bound kernel; 384 threads sit in between.  B200_GLCM_NT selects the variant for A/B runs.
     static const int nt = getenv("B200_GLCM_NT") ? atoi(getenv("B200_GLCM_NT")) : GF_PHASEA_NT;
     const uint8_t* l8 = (const uint8_t*)lev;
     const long long need = (total + nt - 1) / nt, cap = (long long)sms * 8;
@@ -131,9 +129,8 @@ int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P
     RB_LAUNCH_CHECK();
     static const int solve_bps = getenv("B200_GLCM_SOLVE_BPS") ? atoi(getenv("B200_GLCM_SOLVE_BPS")) : 8;
     // One launch per size group keeps ONE solver body in the instruction cache (the three Lanczos templates together are
-    // 18.5 k SASS instructions, 296 KB; ncu: 7.2 no_instruction stall cycles per issue on a smooth volume, whose blocks sit
-    // in different groups).  256^3 smooth, ncu launch list: Lanczos 30.1 -> 20.5 ms, dense n <= 12 16.9 -> 15.3 ms, dense
-    // n <= 8 11.9 -> 12.4 ms (so that one stays a single launch); uniform volume: +0.2 ms of repeated tile sorts.
+    // 18.5 k SASS instructions, 296 KB, and on a smooth volume the blocks of an SM otherwise sit in different groups); the
+    // dense n <= 8 solves stay a single launch, where the repeated tile sorts would cost more than they save.
     // B200_GLCM_SPLIT: bit 0 Lanczos, bit 1 dense <= 12, bit 2 dense <= 8 (A/B switch).
     static const int split = getenv("B200_GLCM_SPLIT") ? atoi(getenv("B200_GLCM_SPLIT")) : GF_SOLVE_SPLIT;
     if (split & 4) {
@@ -239,7 +236,7 @@ int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& 
   if (!T) return fail(RB_ERR_CUDA, "could not build the GLRLM table block on the device");
   const long long total = (long long)(z1 - z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long need = (total + 127) / 128, cap = (long long)sms * 32;
@@ -250,8 +247,8 @@ int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& 
 
 // ------------------------------------------------------------------ GLSZM / GLDM / NGTDM fast paths
 // SYNC: block-uniform tiles with a barrier per tile, so the block's warps stream the (large,
-// straight-line) GLDM / NGTDM bodies together and share instruction-cache lines (ncu showed 2.3
-// "no_instruction" stall cycles per issue for NGTDM with free-running warps).
+// straight-line) GLDM / NGTDM bodies together and share instruction-cache lines (free-running warps stall
+// on instruction fetch).
 template <int CLS, int NT, bool SYNC>
 __global__ void __launch_bounds__(NT)
 small_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
@@ -339,7 +336,7 @@ int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const Vo
   if (!T) return fail(RB_ERR_CUDA, "could not build the table block on the device");
   const long long total = (long long)(z1 - z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const uint8_t* l8 = (const uint8_t*)lev;

@@ -98,7 +98,7 @@ pack_levels_kernel(const int32_t* __restrict__ image, const uint8_t* __restrict_
 }
 
 static int grid_for(long long n, int block, int per_sm) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long need = (n + block - 1) / block;

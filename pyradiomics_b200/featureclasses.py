@@ -1,4 +1,4 @@
-"""B200 feature-class plugins: the same contract as the reference's ``Radiomics<Class>`` classes
+"""CUDA feature-class plugins: the same contract as the reference's ``Radiomics<Class>`` classes
 (reference radiomics/base.py:60-273 and docs/developers.rst:16-64) -- constructor
 ``(inputImage, inputMask, **settings)``, ``enableFeatureByName`` / ``enableAllFeatures`` /
 ``disableAllFeatures``, ``getFeatureNames``, ``execute()`` returning ``{feature: float}``
@@ -163,7 +163,7 @@ _DEVICE_IMAGES_MAX = 2
 
 def device_image(imageArray, maskRaw, label, masked, settings):
     """the device-resident discretised image of (image, mask, label, binning): built on first sight, shared afterwards.
-    The cache key is the CONTENT of image and mask (_fingerprint: ~25 ms for a 512^3 case) unless the caller passes
+    The cache key is the CONTENT of image and mask (_fingerprint: a hash over the whole buffers) unless the caller passes
     ``b200_image_key=<hashable>`` -- its promise that image and mask are the ones it used with that key before (a
     pyradiomics extraction already has such a key: the sha1 of the image in its diagnostics, generalinfo.py)."""
     ident = settings.get("b200_image_key")
@@ -829,7 +829,7 @@ NEXT_CLASSES = {"firstorder": RadiomicsFirstOrder, "shape": RadiomicsShape, "sha
 
 
 def install(radiomics_module=None):
-    """Drop the B200 engine under an importable pyradiomics: the feature classes replace the
+    """Drop the CUDA engine under an importable pyradiomics: the feature classes replace the
     reference's in ``radiomics.getFeatureClasses()`` and ``cMatrices`` is rebound in every module
     that captured it at import time (SURVEY.md section 8b)."""
     import importlib

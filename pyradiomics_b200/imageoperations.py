@@ -49,8 +49,7 @@ _STAGE_MIN = 64 << 20
 def _upload_staged(a):
     """pageable NumPy array -> CUDA tensor through two page-locked 32 MB staging blocks: a few threads copy chunk k+1 into
     one block (NumPy releases the GIL) while the DMA engine drains chunk k from the other.  A plain ``tensor.to(device)`` of
-    pageable memory lets the driver stage single-threaded (~10 GB/s: 40 ms for the 0.4 GB of a 512^3 image + mask, which
-    is a quarter of a rank's step when eight GPUs share one image)."""
+    pageable memory lets the driver stage it single-threaded, at a fraction of the link's rate."""
     import concurrent.futures as cf
     flat = a.reshape(-1).view(np.uint8)
     n = flat.size

@@ -424,10 +424,10 @@ def resample_goldens():
                         names=np.array(sorted(exp)), values=np.array([exp[k] for k in sorted(exp)]))
     print("resample golden", img.shape, sp, len(exp), "values")
     # the other four bundled cases, cropped: ROI box + the pad distance + 16 voxels (the cubic B-spline decomposition forgets
-    # a mirrored edge after ~16 samples), with the index the crop started at and the full size -- the output grid is
-    # anchored at the full image's index 0.  The crop resamples to exactly the arrays of the whole image (checked here).
+    # a mirrored edge after ~16 samples; lung2 takes 10 so that its file stays under 1 MB), with the index the crop started
+    # at and the full size -- the output grid is anchored at the full image's index 0.  The crop resamples to exactly the
+    # arrays of the whole image (checked here).  One file per case: resample_case_<case>.npz.
     import resample_np as RS
-    out = {}
     for case in ("brain1", "brain2", "lung1", "lung2"):
         img, sp = rh.read_nrrd(os.path.join(rh.REF_ROOT, "data", f"{case}_image.nrrd"))
         msk, _ = rh.read_nrrd(os.path.join(rh.REF_ROOT, "data", f"{case}_label.nrrd"))
@@ -440,7 +440,7 @@ def resample_goldens():
                 if r[0].startswith("original_"):
                     exp[r[0]] = float(r[i])
         idx = np.array(np.where(msk == 1))
-        marg = np.ceil((5 * 2.0 + 2.0) / np.array(sp)[::-1]).astype(int) + 16
+        marg = np.ceil((5 * 2.0 + 2.0) / np.array(sp)[::-1]).astype(int) + (10 if case == "lung2" else 16)
         a = np.maximum(idx.min(1) - marg, 0)
         b = np.minimum(idx.max(1) + marg + 1, np.array(img.shape))
         sl = tuple(slice(x, y) for x, y in zip(a, b))
@@ -449,14 +449,84 @@ def resample_goldens():
         whole = RS.resample(img, msk, sp, (2, 2, 2))
         crop = RS.resample(ci, cm, sp, (2, 2, 2), offset_xyz=off, full_size_xyz=full)
         assert np.array_equal(whole[0], crop[0]) and np.array_equal(whole[1], crop[1]), case
-        out.update({f"{case}_image": ci, f"{case}_mask": cm, f"{case}_spacing": np.array(sp), f"{case}_offset_xyz": np.array(off),
+        out = {f"{case}_image": ci, f"{case}_mask": cm, f"{case}_spacing": np.array(sp), f"{case}_offset_xyz": np.array(off),
                     f"{case}_full_size_xyz": np.array(full), f"{case}_names": np.array(sorted(exp)),
-                    f"{case}_values": np.array([exp[k] for k in sorted(exp)])})
+                    f"{case}_values": np.array([exp[k] for k in sorted(exp)])}
+        fn = os.path.join(HERE, f"resample_case_{case}.npz")
+        np.savez_compressed(fn, **out)
+        assert os.path.getsize(fn) < 1_000_000, case
         print("resample golden", case, ci.shape, "of", img.shape, len(exp), "values")
-    np.savez_compressed(os.path.join(HERE, "resample_cases.npz"), **out)
+
+
+def cmatrices_goldens():
+    """the compiled reference `_cmatrices` on the seeded random cases of tests/test_oracle.py::port_cases (every matrix,
+    segment and voxel mode; integer-valued ones stored as int32) -> cmatrices_random.npz, and the exception type it raises
+    for each malformed call of tests/test_plugin_host_logic_cpu.py::BAD_CALLS -> cmatrices_errors.json"""
+    import build_ref
+    sys.path[:0] = [os.path.join(HERE, ".."), os.path.join(HERE, "..", "..")]
+    from test_oracle import port_cases, port_outputs
+    from test_plugin_host_logic_cpu import BAD_CALLS
+    R = build_ref.load()
+
+    def raises(trial, img, msk, dist, Ng, f2, f2d):
+        try:
+            R.calculate_glcm(img, msk, dist, Ng, f2, f2d)
+            R.calculate_glrlm(img, msk, Ng, max(img.shape), f2, f2d)
+        except RuntimeError:
+            rejected.append(trial)
+            return True
+        return False
+
+    rejected, out = [], {}
+    for trial, args in port_cases(raises):
+        for k, v in port_outputs(R, *args).items():
+            v = np.asarray(v)
+            out[f"{trial}_{k}"] = v.astype(np.int32) if np.array_equal(v, v.astype(np.int32)) else v
+    np.savez_compressed(os.path.join(HERE, "cmatrices_random.npz"), rejected_trials=np.array(rejected, np.int32), **out)
+    print("cmatrices random", len(out), "matrices,", len(rejected), "rejected cases")
+    errors = {}
+    img, msk = np.ones((4, 5, 6), np.int32), np.ones((4, 5, 6), bool)
+    for what, call in BAD_CALLS.items():
+        try:
+            call(R, img, msk)
+        except Exception as e:          # noqa: BLE001 -- the type is what is recorded
+            errors[what] = type(e).__name__
+    assert len(errors) == len(BAD_CALLS)
+    json.dump(errors, open(os.path.join(HERE, "cmatrices_errors.json"), "w"), indent=0, sort_keys=True)
+
+
+def names_golden():
+    """getFeatureNames() of the reference's feature classes -> reference_feature_names.json"""
+    import importlib
+    out = {}
+    for name, cls in (("glcm", "RadiomicsGLCM"), ("glrlm", "RadiomicsGLRLM"), ("glszm", "RadiomicsGLSZM"), ("gldm", "RadiomicsGLDM"),
+                      ("ngtdm", "RadiomicsNGTDM"), ("firstorder", "RadiomicsFirstOrder"), ("shape", "RadiomicsShape"),
+                      ("shape2D", "RadiomicsShape2D")):
+        out[name] = getattr(importlib.import_module(f"radiomics.{name}"), cls).getFeatureNames()
+    json.dump(out, open(os.path.join(HERE, "reference_feature_names.json"), "w"), indent=0, sort_keys=True)
+
+
+def shape_large_roi_golden():
+    """the compiled reference `_cshape` on tests/test_shape_gpu.py::large_roi -> shape_large_roi.json"""
+    import build_ref
+    sys.path.insert(0, os.path.join(HERE, ".."))
+    from test_shape_gpu import large_roi
+    m, sp = large_roi()
+    sa, vol, dia = build_ref.load("_cshape").calculate_coefficients(m, sp)
+    json.dump({"surface_area": sa, "volume": vol, "diameters": list(dia)},
+              open(os.path.join(HERE, "shape_large_roi.json"), "w"), indent=0)
 
 
 if __name__ == "__main__":
+    if "--cmatrices-only" in sys.argv:
+        cmatrices_goldens()
+        sys.exit(0)
+    if "--names-only" in sys.argv:
+        names_golden()
+        sys.exit(0)
+    if "--shape-large-roi-only" in sys.argv:
+        shape_large_roi_golden()
+        sys.exit(0)
     if "--segment-variants-only" in sys.argv:
         segment_goldens_variants()
         sys.exit(0)

@@ -1,5 +1,5 @@
-"""The committed bench line of the round (profiles/) keeps the driver's JSON contract: a change to bench.py that drops a
-key shows here without a GPU."""
+"""The committed bench line (profiles/) keeps bench.py's JSON contract: a change to bench.py that drops a key shows here
+without a GPU."""
 import glob
 import json
 import os
@@ -7,15 +7,15 @@ import os
 import pytest
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-LINES = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_bench_n*_512_*.json")))
+LINES = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_bench_n*_*_*.json")))
 
 
 @pytest.mark.parametrize("path", LINES, ids=[os.path.basename(p) for p in LINES])
 def test_bench_line_contract(path):
     d = json.loads(open(path).read().strip().splitlines()[-1])
     base = json.load(open(os.path.join(ROOT, "BASELINE.json")))
-    # BASELINE.json: "voxels/s full-texture voxel-based on 512^3 @1/2/4/8 B200; %HBM roofline" -- the line carries the
-    # quantity, the "@N B200" part is n_gpus and the roofline part is the `roofline` object
+    # BASELINE.json: "voxels/s full-texture voxel-based on 256^3 @1/2/4/8 H100; %HBM roofline" -- the line carries the
+    # quantity, the "@N H100" part is n_gpus and the roofline part is the `roofline` object
     assert base["metric"].startswith(d["metric"])
     assert d["unit"] == "voxels/s" and d["higher_is_better"] is True and d["data"] == "synthetic"
     assert d["value"] > 0 and d["ms_per_step"] > 0 and d["steps"] >= 1 and d["warmup"] >= 3

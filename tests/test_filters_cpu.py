@@ -1,5 +1,5 @@
 """CPU checks of the two third-party pre-filter restatements (oracle/filters_np.py; PARITY UNPINNED: PyWavelets / SimpleITK
-are absent here and on the GPU box -- probed, profiles/r02_sanitizer/probe_libs.txt): the documented phase / alignment of
+are not dependencies of the project): the documented phase / alignment of
 the stationary wavelet transform, perfect reconstruction with the matching synthesis bank, Parseval, and the level loop of
 the reference's _swt3."""
 import numpy as np

@@ -3,19 +3,21 @@ it lies, with stand-ins for SimpleITK / pywt / pykwalify: oracle/ref_harness.py)
 per-module `cMatrices` rebinding (SURVEY.md 8b) and `cShape` keeping `calculate_coefficients2D` reachable for
 radiomics.shape2D (reference radiomics/shape2D.py:99).  No CUDA call is made."""
 import importlib
+import json
 import os
 import sys
 
 import pytest
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "radiomics")), reason="the reference tree is not on this box")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 @pytest.fixture(scope="module")
 def rad():
     import types
     import ref_harness
+    if not os.path.isdir(os.path.join(ref_harness.REF_ROOT, "radiomics")):
+        pytest.skip("the reference pyradiomics source tree is not available")
     # radiomics.getFeatureClasses() imports EVERY module of the package, radiomics.scripts (the CLI) among them: stand-ins
     # for what the CLI imports and this image lacks
     if "ruamel" not in sys.modules:
@@ -52,15 +54,14 @@ def test_install_registers_classes_and_rebinds_cmatrices(rad):
         cshape.no_such_function
 
 
-def test_feature_names_and_docstrings_match_the_reference_classes(rad):
-    """reference tests/test_docstrings.py: every get<Name>FeatureValue has a docstring; names equal the reference's"""
+def test_feature_names_and_docstrings_match_the_reference_classes():
+    """reference tests/test_docstrings.py: every get<Name>FeatureValue has a docstring; names (and deprecation flags) equal
+    the reference classes' getFeatureNames() (tests/golden/reference_feature_names.json, make_golden.py --names-only)"""
     from pyradiomics_b200 import featureclasses as FC
+    ref = json.load(open(os.path.join(GOLDEN, "reference_feature_names.json")))
     for name in ("glcm", "glrlm", "glszm", "gldm", "ngtdm", "firstorder", "shape", "shape2D"):
-        ref_cls = getattr(importlib.import_module(f"{rad.__name__}.{name}"), {"glcm": "RadiomicsGLCM", "glrlm": "RadiomicsGLRLM",
-                          "glszm": "RadiomicsGLSZM", "gldm": "RadiomicsGLDM", "ngtdm": "RadiomicsNGTDM",
-                          "firstorder": "RadiomicsFirstOrder", "shape": "RadiomicsShape", "shape2D": "RadiomicsShape2D"}[name])
         ours = {**FC.FEATURE_CLASSES, **FC.NEXT_CLASSES}[name]
-        assert ours.getFeatureNames() == ref_cls.getFeatureNames()
+        assert ours.getFeatureNames() == ref[name]
         for f in ours.getFeatureNames():
             assert getattr(ours, f"get{f}FeatureValue").__doc__
 

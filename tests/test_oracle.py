@@ -18,22 +18,11 @@ def seg():
     return np.load(os.path.join(GOLDEN, "segment_cases.npz")), json.load(open(os.path.join(GOLDEN, "segment_expect.json")))
 
 
-def _ref_module():
-    import build_ref
-    try:
-        return build_ref.load()
-    except ImportError:
-        return None
-
-
-def test_port_equals_compiled_reference():
-    """bit-exact agreement of oracle/cmatrices_port.c with the gcc-built reference _cmatrices on
-    random 2-D/3-D inputs, segment and voxel mode, several distances / force2D."""
-    R = _ref_module()
-    if R is None:
-        pytest.skip("oracle/_ref not built and /root/reference absent")
+def port_cases(raises):
+    """the 40 seeded random 2-D/3-D cases (several distances / force2D) of test_port_equals_compiled_reference.
+    `raises(trial, img, msk, dist, Ng, f2, f2d)` tells whether the reference rejects a case (it is then skipped); yields
+    (trial, args) with args = (img, msk, dist, Ng, f2, f2d, r, vox), r = None when fewer than two voxels are in the mask"""
     rng = np.random.default_rng(3)
-    n = 0
     for trial in range(40):
         nd = int(rng.choice([2, 3]))
         shp = tuple(int(s) for s in (rng.integers(1, 9, nd) if trial % 3 else rng.integers(3, 8, nd)))
@@ -45,29 +34,45 @@ def test_port_equals_compiled_reference():
         dist = np.array([[1], [1, 2], [2], [1, 3]][trial % 4])
         f2 = int(trial % 5 == 0 and nd == 3)
         f2d = int(rng.integers(0, nd))
-        try:
-            ra = R.calculate_glcm(img, msk, dist, Ng, f2, f2d)
-            rr = R.calculate_glrlm(img, msk, Ng, max(shp), f2, f2d)
-        except RuntimeError:
+        if raises(trial, img, msk, dist, Ng, f2, f2d):
             continue
-        pa = O.calculate_glcm(img, msk, dist, Ng, f2, f2d)
-        assert np.array_equal(ra[0], pa[0]) and np.array_equal(ra[1], pa[1])
-        pr = O.calculate_glrlm(img, msk, Ng, max(shp), f2, f2d)
-        assert np.array_equal(rr[0], pr[0]) and np.array_equal(rr[1], pr[1])
-        Ns = int(msk.sum())
-        assert np.array_equal(R.calculate_glszm(img, msk, Ng, Ns, f2, f2d), O.calculate_glszm(img, msk, Ng, Ns, f2, f2d))
-        assert np.array_equal(R.calculate_ngtdm(img, msk, dist, Ng, f2, f2d), O.calculate_ngtdm(img, msk, dist, Ng, f2, f2d))
-        assert np.array_equal(R.calculate_gldm(img, msk, dist, Ng, 1, f2, f2d), O.calculate_gldm(img, msk, dist, Ng, 1, f2, f2d))
         vox = np.array(np.where(msk)).astype(np.int32)
-        if vox.shape[1] < 2:
-            continue
-        r = int(rng.integers(1, 3))
-        assert np.array_equal(R.calculate_glcm(img, msk, dist, Ng, f2, f2d, r, vox)[0], O.calculate_glcm(img, msk, dist, Ng, f2, f2d, r, vox)[0])
-        assert np.array_equal(R.calculate_glrlm(img, msk, Ng, max(shp), f2, f2d, r, vox)[0], O.calculate_glrlm(img, msk, Ng, max(shp), f2, f2d, r, vox)[0])
-        assert np.array_equal(R.calculate_glszm(img, msk, Ng, Ns, f2, f2d, r, vox), O.calculate_glszm(img, msk, Ng, Ns, f2, f2d, r, vox))
-        assert np.array_equal(R.calculate_ngtdm(img, msk, dist, Ng, f2, f2d, r, vox), O.calculate_ngtdm(img, msk, dist, Ng, f2, f2d, r, vox))
-        assert np.array_equal(R.calculate_gldm(img, msk, dist, Ng, 0, f2, f2d, r, vox), O.calculate_gldm(img, msk, dist, Ng, 0, f2, f2d, r, vox))
-        n += 1
+        r = int(rng.integers(1, 3)) if vox.shape[1] >= 2 else None
+        yield trial, (img, msk, dist, Ng, f2, f2d, r, vox)
+
+
+def port_outputs(M, img, msk, dist, Ng, f2, f2d, r, vox):
+    """every matrix the module M (the compiled reference or the port) returns for one case, segment and voxel mode"""
+    shp, Ns = img.shape, int(msk.sum())
+    out = {}
+    out["glcm"], out["glcm_angles"] = M.calculate_glcm(img, msk, dist, Ng, f2, f2d)
+    out["glrlm"], out["glrlm_angles"] = M.calculate_glrlm(img, msk, Ng, max(shp), f2, f2d)
+    out["glszm"] = M.calculate_glszm(img, msk, Ng, Ns, f2, f2d)
+    out["ngtdm"] = M.calculate_ngtdm(img, msk, dist, Ng, f2, f2d)
+    out["gldm"] = M.calculate_gldm(img, msk, dist, Ng, 1, f2, f2d)
+    if r is not None:
+        out["voxel_glcm"] = M.calculate_glcm(img, msk, dist, Ng, f2, f2d, r, vox)[0]
+        out["voxel_glrlm"] = M.calculate_glrlm(img, msk, Ng, max(shp), f2, f2d, r, vox)[0]
+        out["voxel_glszm"] = M.calculate_glszm(img, msk, Ng, Ns, f2, f2d, r, vox)
+        out["voxel_ngtdm"] = M.calculate_ngtdm(img, msk, dist, Ng, f2, f2d, r, vox)
+        out["voxel_gldm"] = M.calculate_gldm(img, msk, dist, Ng, 0, f2, f2d, r, vox)
+    return out
+
+
+def test_port_equals_compiled_reference():
+    """bit-exact agreement of oracle/cmatrices_port.c with the gcc-built reference _cmatrices on
+    random 2-D/3-D inputs, segment and voxel mode, several distances / force2D.  The reference's
+    matrices are tests/golden/cmatrices_random.npz (make_golden.py --cmatrices-only)."""
+    z = np.load(os.path.join(GOLDEN, "cmatrices_random.npz"))
+    rejected = set(z["rejected_trials"].tolist())
+    n, seen = 0, {"rejected_trials"}
+    for trial, args in port_cases(lambda trial, *_: trial in rejected):
+        got = port_outputs(O, *args)
+        for k, v in got.items():
+            assert np.array_equal(z[f"{trial}_{k}"], v), (trial, k)
+            seen.add(f"{trial}_{k}")
+        n += "voxel_glcm" in got
+    assert seen == set(z.files)
     assert n > 20
 
 

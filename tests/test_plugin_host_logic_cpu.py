@@ -380,19 +380,8 @@ def test_bin_edges_from_min_max_equal_the_reference_arithmetic_for_every_dtype()
 
 
 # ---- cmatrices: argument errors are raised on the host, before anything touches the device, with the reference's exception
-# types (SURVEY.md 8b "Error conventions") -- checked against the compiled reference extension itself
-def _ref_cmatrices():
-    import importlib.util
-    import glob as _glob
-    so = _glob.glob(os.path.join(os.path.dirname(GOLDEN), "..", "oracle", "_ref", "_cmatrices*.so"))
-    if not so:
-        pytest.skip("oracle/_ref is not built (needs /root/reference)")
-    spec = importlib.util.spec_from_file_location("_cmatrices", so[0])
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
+# types (SURVEY.md 8b "Error conventions") -- checked against the exception types the compiled reference extension raises
+# for the same calls (tests/golden/cmatrices_errors.json, make_golden.py --cmatrices-only)
 BAD_CALLS = {
     "ndim mismatch": lambda cm, i, m: cm.calculate_glcm(i, m[0], np.array([1]), 8, False, -1),
     "shape mismatch": lambda cm, i, m: cm.calculate_glcm(i, m[:, :4], np.array([1]), 8, False, -1),
@@ -407,14 +396,12 @@ BAD_CALLS = {
 
 @pytest.mark.parametrize("what", list(BAD_CALLS))
 def test_cmatrices_argument_errors_have_the_reference_exception_types(what):
-    ref = _ref_cmatrices()
+    want = json.load(open(os.path.join(GOLDEN, "cmatrices_errors.json")))[what]
     img = np.ones((4, 5, 6), np.int32)
     msk = np.ones((4, 5, 6), bool)
-    with pytest.raises(Exception) as want:
-        BAD_CALLS[what](ref, img, msk)
     with pytest.raises(Exception) as got:
         BAD_CALLS[what](cmatrices, img, msk)
-    assert type(got.value) is type(want.value), (what, repr(got.value), repr(want.value))
+    assert type(got.value).__name__ == want, (what, repr(got.value), want)
     assert type(got.value) in (ValueError, RuntimeError)
 
 

@@ -42,9 +42,10 @@ def test_oracle_resampling_reproduces_the_reference_baseline_column():
 
 @pytest.mark.parametrize("case", ["brain1", "brain2", "lung1", "lung2"])
 def test_oracle_resampling_reproduces_the_other_four_baseline_columns(case):
-    """`<case>_resampling` of the seven baseline CSVs for the other bundled cases (tests/golden/resample_cases.npz: the ROI
-    box + pad + 16 voxels of each image, with the index the crop started at -- it resamples to exactly the whole image's arrays)"""
-    z = np.load(os.path.join(G, "resample_cases.npz"))
+    """`<case>_resampling` of the seven baseline CSVs for the other bundled cases (tests/golden/resample_case_<case>.npz: the
+    ROI box + pad + a 10-16 voxel margin of each image, with the index the crop started at -- it resamples to exactly the
+    whole image's arrays)"""
+    z = np.load(os.path.join(G, f"resample_case_{case}.npz"))
     exp = dict(zip(z[case + "_names"], z[case + "_values"]))
     img, msk, new = RS.resample(z[case + "_image"], z[case + "_mask"], z[case + "_spacing"], (2, 2, 2),
                                 offset_xyz=tuple(z[case + "_offset_xyz"]), full_size_xyz=tuple(z[case + "_full_size_xyz"]))
