@@ -233,6 +233,21 @@ int rb_resample_dev(const void *src_dev, int src_dtype, const int *in_size_zyx, 
                     const int *out_size_zyx, const double *start_zyx, const double *step_zyx, int interpolator,
                     double default_value, void *stream);
 
+/* ---- 3-D local binary pattern image type (reference radiomics/imageoperations.py:1169-1314, getLBP3DImage).
+ * For every voxel with roi_u8_dev != 0: the cubic B-spline samples of the image at the Nv sphere vertices
+ *   (scipy.ndimage.map_coordinates(order=3): SciPy's exact mirror prefilter, 0 where a coordinate leaves [0, n-1]), cast
+ *   to `sample_dtype`; their Fisher kurtosis; the sign bits sample >= centre; the spherical-harmonic level maps
+ *   Re(sqrt(sum_v (sum_m c_nm Y_nm(v))^2)) with c_nm = sum_v bit_v Y_nm(v), n < levels.
+ * img_dtype: dtype code (as rb_minmax_dev) of the data at img_dev; sample_dtype: the dtype the samples are cast to, the
+ *   image's original one (a uint16 image stored as int32 passes 1 and 5).
+ * vertices_host: [nv][3] (z, y, x) offsets in voxels; harmonics_host: [nv][levels (levels + 1) / 2][re, im], entry
+ *   n (n + 1) / 2 + m = Y_n^m(vertex) for 0 <= m <= n (negative m follow from Y_n^-m = (-1)^m conj(Y_n^m)).
+ * coeff_scratch_dev: Z*Y*X float64; out_dev: float64 [levels + 1][Z][Y][X], the level maps then the kurtosis, 0 outside
+ *   the ROI.  nv <= 162 and levels <= 4, else RB_ERR_UNSUPPORTED. */
+int rb_lbp3d_dev(const void *img_dev, int img_dtype, int sample_dtype, const uint8_t *roi_u8_dev, int Z, int Y, int X,
+                 const double *vertices_host, int nv, const double *harmonics_host, int levels,
+                 double *coeff_scratch_dev, double *out_dev, void *stream);
+
 /* ---- segment-mode shape coefficients (SURVEY.md section 8f rank 4) ------------------------------
  * rb_calculate_coefficients replaces calculate_coefficients (radiomics/src/cshape.h:1-2, binding
  *   radiomics/src/_cshape.c:75-113): HOST mask (non-zero = ROI) of `size` = {Z, Y, X} with element

@@ -76,9 +76,12 @@ int recursive_gauss_launch(const void* in, int in_is_f32, int Z, int Y, int X, i
                            double* scratch, double scale, int accumulate, cudaStream_t st);
 int swt3d_launch(const double* in, int Z, int Y, int X, const double* lo, const double* hi, int F, double* out,
                  long long band_stride, int z_begin, int z_end, cudaStream_t st);
-int bspline_prefilter_launch(double* coeffs, int Z, int Y, int X, cudaStream_t st);
+int bspline_prefilter_launch(double* coeffs, int Z, int Y, int X, cudaStream_t st, bool exact_init);
 int resample_launch(const void* src, int src_dt, const int* in_size, void* dst, int dst_dt, const int* out_size, const double* start,
                     const double* step, int interp, double default_value, cudaStream_t st);
+
+int lbp3d_launch(const void* img, int img_dt, int sample_dt, const uint8_t* roi, int Z, int Y, int X, const double* vertices,
+                 int nv, const double* harmonics, int levels, double* coeff_scratch, double* out, cudaStream_t st);
 
 int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
                       int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
@@ -343,13 +346,20 @@ int rb_swt_axis_dev(const double* in_dev, int Z, int Y, int X, int axis, const d
   return swt_axis_launch(in_dev, Z, Y, X, axis, dec_lo, dec_hi, flen, out_lo_dev, out_hi_dev, (cudaStream_t)stream);
 }
 int rb_bspline_prefilter_dev(double* coeffs_dev, int Z, int Y, int X, void* stream) {
-  return bspline_prefilter_launch(coeffs_dev, Z, Y, X, (cudaStream_t)stream);
+  return bspline_prefilter_launch(coeffs_dev, Z, Y, X, (cudaStream_t)stream, false);
 }
 int rb_resample_dev(const void* src_dev, int src_dtype, const int* in_size_zyx, void* dst_dev, int dst_dtype, const int* out_size_zyx,
                     const double* start_zyx, const double* step_zyx, int interpolator, double default_value, void* stream) {
   if (!src_dev || !dst_dev || !in_size_zyx || !out_size_zyx || !start_zyx || !step_zyx) return fail(RB_ERR_ARG, "null argument");
   return resample_launch(src_dev, src_dtype, in_size_zyx, dst_dev, dst_dtype, out_size_zyx, start_zyx, step_zyx, interpolator,
                          default_value, (cudaStream_t)stream);
+}
+
+int rb_lbp3d_dev(const void* img_dev, int img_dtype, int sample_dtype, const uint8_t* roi_u8_dev, int Z, int Y, int X,
+                 const double* vertices_host, int nv, const double* harmonics_host, int levels, double* coeff_scratch_dev,
+                 double* out_dev, void* stream) {
+  return lbp3d_launch(img_dev, img_dtype, sample_dtype, roi_u8_dev, Z, Y, X, vertices_host, nv, harmonics_host, levels,
+                      coeff_scratch_dev, out_dev, (cudaStream_t)stream);
 }
 
 int rb_swt3d_dev(const double* in_dev, int Z, int Y, int X, const double* dec_lo, const double* dec_hi, int flen,

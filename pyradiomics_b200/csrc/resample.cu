@@ -15,12 +15,16 @@ namespace rb {
 
 constexpr double BSPLINE_POLE = -0.26794919243112270647;      // sqrt(3) - 2
 
+// EXACT = false: ITK's causal initialisation (truncated after 18 samples once the line is longer);
+// EXACT = true: the closed-form mirror sum for every length, as scipy.ndimage.spline_filter does (getLBP3DImage's
+// map_coordinates; the truncation alone differs from SciPy by ~4e-11 relative on a 64-sample line)
+template <bool EXACT>
 __device__ __forceinline__ void bspline_line(double* c, long long stride, int N) {
   if (N == 1) return;
   const double z = BSPLINE_POLE;
   for (int n = 0; n < N; n++) c[n * stride] *= 6.0;            // (1 - z)(1 - 1/z)
   const int horizon = 18;                                        // ceil(log(1e-10) / log|z|)
-  if (horizon < N) {
+  if (!EXACT && horizon < N) {
     double zn = z, sum = c[0];
     for (int n = 1; n < horizon; n++) { sum += zn * c[n * stride]; zn *= z; }
     c[0] = sum;
@@ -37,6 +41,7 @@ __device__ __forceinline__ void bspline_line(double* c, long long stride, int N)
   for (int n = N - 2; n >= 0; n--) c[n * stride] = z * (c[(n + 1) * stride] - c[n * stride]);
 }
 
+template <bool EXACT>
 __global__ void __launch_bounds__(128)
 bspline_prefilter_kernel(double* __restrict__ c, int Z, int Y, int X, int axis) {
   const int N = axis == 0 ? Z : axis == 1 ? Y : X;
@@ -48,12 +53,13 @@ bspline_prefilter_kernel(double* __restrict__ c, int Z, int Y, int X, int axis) 
     if (axis == 2) base = l * X;
     else if (axis == 1) { const long long z = l / X, x = l % X; base = z * plane + x; }
     else base = l;
-    bspline_line(c + base, stride, N);
+    bspline_line<EXACT>(c + base, stride, N);
   }
 }
 
 // x axis: a warp owns 32 consecutive lines and stages them through shared memory (the whole line: X <= 2048), so global
 // accesses are coalesced rows instead of 32 lanes X elements apart
+template <bool EXACT>
 __global__ void __launch_bounds__(128)
 bspline_prefilter_x_kernel(double* __restrict__ c, long long nlines, int X) {
   extern __shared__ double sm_lines[];             // [4 warps][32 lines][X + 1]
@@ -64,7 +70,7 @@ bspline_prefilter_x_kernel(double* __restrict__ c, long long nlines, int X) {
       if (l0 + r < nlines)
         for (int x = lane; x < X; x += 32) mine[r * (X + 1) + x] = c[(l0 + r) * X + x];
     __syncwarp();
-    if (l0 + lane < nlines) bspline_line(mine + lane * (X + 1), 1, X);
+    if (l0 + lane < nlines) bspline_line<EXACT>(mine + lane * (X + 1), 1, X);
     __syncwarp();
     for (int r = 0; r < 32; r++)
       if (l0 + r < nlines)
@@ -179,23 +185,28 @@ static int grid_rs(long long n, int block, int per_sm) {
   return (int)(need < cap ? (need < 1 ? 1 : need) : cap);
 }
 
-int bspline_prefilter_launch(double* coeffs, int Z, int Y, int X, cudaStream_t st) {
+template <bool EXACT>
+static int bspline_prefilter_run(double* coeffs, int Z, int Y, int X, cudaStream_t st) {
   if (Z < 1 || Y < 1 || X < 1) return fail(RB_ERR_ARG, "empty volume");
   const long long n = (long long)Z * Y * X;
   // ITK's BSplineDecompositionImageFilter filters dimension 0 (x) first, then y, then z
   if (X > 1) {
     const size_t sh = (size_t)4 * 32 * (X + 1) * sizeof(double);
     if (sh <= 200 * 1024) {
-      cudaFuncSetAttribute(bspline_prefilter_x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh);
-      bspline_prefilter_x_kernel<<<grid_rs((n / X + 31) / 32, 4, 4), 128, sh, st>>>(coeffs, n / X, X);
+      cudaFuncSetAttribute(bspline_prefilter_x_kernel<EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh);
+      bspline_prefilter_x_kernel<EXACT><<<grid_rs((n / X + 31) / 32, 4, 4), 128, sh, st>>>(coeffs, n / X, X);
     } else {
-      bspline_prefilter_kernel<<<grid_rs(n / X, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 2);
+      bspline_prefilter_kernel<EXACT><<<grid_rs(n / X, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 2);
     }
   }
-  if (Y > 1) bspline_prefilter_kernel<<<grid_rs(n / Y, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 1);
-  if (Z > 1) bspline_prefilter_kernel<<<grid_rs(n / Z, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 0);
+  if (Y > 1) bspline_prefilter_kernel<EXACT><<<grid_rs(n / Y, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 1);
+  if (Z > 1) bspline_prefilter_kernel<EXACT><<<grid_rs(n / Z, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 0);
   RB_LAUNCH_CHECK();
   return RB_OK;
+}
+
+int bspline_prefilter_launch(double* coeffs, int Z, int Y, int X, cudaStream_t st, bool exact_init) {
+  return exact_init ? bspline_prefilter_run<true>(coeffs, Z, Y, X, st) : bspline_prefilter_run<false>(coeffs, Z, Y, X, st);
 }
 
 int resample_launch(const void* src, int src_dt, const int* in_size, void* dst, int dst_dt, const int* out_size, const double* start,

@@ -1,7 +1,7 @@
 """GPU versions of the pyradiomics image operations that sit on the texture hot path
 (reference radiomics/imageoperations.py): gray-level discretisation (getBinEdges / binImage,
-:67-174), the level-1 stationary wavelet decomposition (getWaveletImage / _swt3, :839-970) and the
-Laplacian-of-Gaussian filter (getLoGImage, :756-836).  Same function names, arguments and yielded
+:67-174), the level-1 stationary wavelet decomposition (getWaveletImage / _swt3, :839-970), the
+Laplacian-of-Gaussian filter (getLoGImage, :756-836) and the 3-D local binary pattern (getLBP3DImage, :1169-1314).  Same function names, arguments and yielded
 tuples as the reference so they can be dropped into ``radiomics.imageoperations``.
 
 Parity status (DESIGN.md): binning is bit-identical to NumPy; wavelet and LoG restate PyWavelets'
@@ -512,3 +512,129 @@ def getLoGImage(inputImage, _inputMask, **kwargs):
                                sigma, spacing, size)
         else:
             logger.warning("applyLoG: sigma must be greater than 0.0: %s", sigma)
+
+
+# ------------------------------------------------------------------------------------ LBP 3-D
+_ICOSAHEDRON_T = (1.0 + 5.0 ** 0.5) / 2.0
+_ICOSAHEDRON_V = [[-1, _ICOSAHEDRON_T, 0], [1, _ICOSAHEDRON_T, 0], [-1, -_ICOSAHEDRON_T, 0], [1, -_ICOSAHEDRON_T, 0],
+                  [0, -1, _ICOSAHEDRON_T], [0, 1, _ICOSAHEDRON_T], [0, -1, -_ICOSAHEDRON_T], [0, 1, -_ICOSAHEDRON_T],
+                  [_ICOSAHEDRON_T, 0, -1], [_ICOSAHEDRON_T, 0, 1], [-_ICOSAHEDRON_T, 0, -1], [-_ICOSAHEDRON_T, 0, 1]]
+_ICOSAHEDRON_F = [[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2], [10, 7, 6],
+                  [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11], [6, 2, 10],
+                  [8, 6, 7], [9, 8, 1]]
+
+
+def _icosphere(subdivision=1, radius=1.0):
+    """vertices (Nv, 3) of the icosphere getLBP3DImage samples on (trimesh.creation.icosphere's construction, restated):
+    the 12 normalised icosahedron vertices, then per subdivision the midpoints of every edge, all projected back onto the
+    unit sphere; finally scaled to `radius`.  12 / 42 / 162 / 642 vertices for subdivision 0 / 1 / 2 / 3.  Only the vertex
+    set matters to the filter (every reduction runs over the vertices)."""
+    v = np.array(_ICOSAHEDRON_V, dtype=np.float64)
+    v /= np.linalg.norm(v, axis=1)[:, None]
+    faces = np.array(_ICOSAHEDRON_F, dtype=np.int64)
+    for _ in range(int(subdivision)):
+        edges = np.sort(np.concatenate([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]]), axis=1)
+        uniq, inv = np.unique(edges, axis=0, return_inverse=True)
+        mid = (v[uniq[:, 0]] + v[uniq[:, 1]]) / 2.0
+        inv = inv.reshape(3, -1) + len(v)                  # midpoint index of edge (01, 12, 20) of every face
+        v = np.concatenate([v, mid])
+        v /= np.linalg.norm(v, axis=1)[:, None]
+        a, b, c = faces.T
+        ab, bc, ca = inv
+        faces = np.concatenate([np.stack([a, ab, ca], 1), np.stack([ab, b, bc], 1), np.stack([ca, bc, c], 1),
+                                np.stack([ab, bc, ca], 1)])
+    return v * float(radius)
+
+
+def _lbp3d_harmonics(vertices, levels, radius=None):
+    """complex (Nv, levels**2) table Y[v][k], k running over n = 0..levels-1, m = -n..n: the reference's
+    sph_harm(m, n, theta, phi) (imageoperations.py:1238-1248) with theta = arccos(v_2 / R) and phi = arctan2(v_1, v_0) in
+    SciPy's old argument order, i.e. phi is the POLAR angle and theta the azimuth.  Orthonormal harmonics with the
+    Condon-Shortley phase, Y_n^-m = (-1)^m conj(Y_n^m)."""
+    v = np.asarray(vertices, dtype=np.float64)
+    if radius is None:
+        radius = float(np.linalg.norm(v[0]))
+    azimuth = np.arccos(np.true_divide(v[:, 2], radius))
+    polar = np.arctan2(v[:, 1], v[:, 0])
+    x, s = np.cos(polar), np.abs(np.sin(polar))
+    P = {}                                            # associated Legendre P_n^m(x), m >= 0
+    for m in range(levels):
+        pmm = np.ones_like(x)
+        for i in range(1, m + 1):
+            pmm = -pmm * (2 * i - 1) * s
+        P[m, m] = pmm
+        if m + 1 < levels:
+            P[m + 1, m] = x * (2 * m + 1) * pmm
+        for n in range(m + 2, levels):
+            P[n, m] = ((2 * n - 1) * x * P[n - 1, m] - (n + m - 1) * P[n - 2, m]) / (n - m)
+    cols = []
+    for n in range(levels):
+        pos = {}
+        for m in range(n + 1):
+            norm = math.sqrt((2 * n + 1) / (4 * math.pi) * math.factorial(n - m) / math.factorial(n + m))
+            pos[m] = norm * P[n, m] * np.exp(1j * m * azimuth)
+        for m in range(-n, n + 1):
+            cols.append(pos[m] if m >= 0 else (-1) ** m * np.conj(pos[-m]))
+    return np.stack(cols, axis=1)
+
+
+def _lbp3d_tables(levels, radius, subdivision):
+    """host tables of rb_lbp3d_dev: vertices (Nv, 3) and the m >= 0 harmonics (Nv, levels (levels + 1) / 2, [re, im]).
+    The kernel covers subdivision 0..2 (at most 162 vertices) and 1..4 levels; there is no other implementation."""
+    if not (0 <= int(subdivision) <= 2 and 1 <= int(levels) <= 4):
+        raise ValueError(f"LBP 3D: lbp3DIcosphereSubdivision {subdivision} / lbp3DLevels {levels} outside the CUDA "
+                         "kernel's range (subdivision 0..2, levels 1..4)")
+    levels = int(levels)
+    verts = np.ascontiguousarray(_icosphere(int(subdivision), radius), dtype=np.float64)
+    Y = _lbp3d_harmonics(verts, levels, float(radius))
+    keep = [n * n + n + m for n in range(levels) for m in range(n + 1)]              # the m >= 0 columns
+    harm = np.ascontiguousarray(np.stack([Y[:, keep].real, Y[:, keep].imag], axis=-1), dtype=np.float64)
+    return verts, harm
+
+
+def lbp3d_device(img_t: torch.Tensor, roi_t: torch.Tensor, levels=2, radius=1.0, subdivision=1, dtype=None):
+    """3-D LBP of a CUDA volume (Z,Y,X): float64 CUDA tensor [levels + 1, Z, Y, X] holding the level maps m1..m<levels>
+    and the kurtosis map, 0 outside the ROI (roi_t != 0).  `dtype` is the image's original NumPy dtype, which the sphere
+    samples are rounded and clamped to (default: img_t's; a uint16 image reaches the device as int32)."""
+    verts, harm = _lbp3d_tables(levels, radius, subdivision)
+    levels = int(levels)
+    src = img_t.contiguous()
+    if src.dtype not in _TORCH_DT:
+        raise ValueError(f"unsupported pixel type {src.dtype}")
+    dtype = np.dtype(dtype) if dtype is not None else np.dtype(_NP_OF_TORCH[src.dtype])
+    if dtype not in _DT:
+        raise ValueError(f"unsupported pixel type {dtype}")
+    roi = (roi_t != 0).to(torch.uint8).contiguous()
+    if src.dim() != 3 or tuple(roi.shape) != tuple(src.shape):
+        raise ValueError("lbp3d_device needs a 3-D image and a ROI of the same shape")
+    Z, Yn, X = src.shape
+    scratch = torch.empty((Z, Yn, X), dtype=torch.float64, device=src.device)
+    out = torch.empty((levels + 1, Z, Yn, X), dtype=torch.float64, device=src.device)
+    check(lib().rb_lbp3d_dev(_ptr(src), _TORCH_DT[src.dtype], _DT[dtype], _ptr(roi), Z, Yn, X,
+                             verts.ctypes.data_as(C.c_void_p), int(len(verts)), harm.ctypes.data_as(C.c_void_p), levels,
+                             _ptr(scratch), _ptr(out), _stream()), "lbp3d")
+    return out
+
+
+def getLBP3DImage(inputImage, inputMask, **kwargs):
+    """reference generator (imageoperations.py:1169-1314): yields the level maps 'lbp-3D-m1' .. 'lbp-3D-m<lbp3DLevels>'
+    then the spherical kurtosis 'lbp-3D-k', float64 images.  Settings lbp3DLevels (2), lbp3DIcosphereRadius (1, voxels),
+    lbp3DIcosphereSubdivision (1) and label (1).  Deviation: voxels outside the ROI are 0 (the reference leaves them
+    uninitialised)."""
+    arr = I.as_array(inputImage)
+    Nd = arr.ndim
+    if Nd != 3:
+        logger.warning(f"LBP 3D only available for 3 dimensional images, found {Nd} dimensions")
+        return
+    if kwargs.get("force2D", False):
+        logger.warning("Calculating Local Binary Pattern in 3D, but extracting features in 2D. Use with caution!")
+    label = kwargs.get("label", 1)
+    levels = int(kwargs.get("lbp3DLevels", 2))
+    radius = kwargs.get("lbp3DIcosphereRadius", 1)
+    subdivision = int(kwargs.get("lbp3DIcosphereSubdivision", 1))
+    _lbp3d_tables(levels, radius, subdivision)                  # range check before anything reaches the device
+    roi = np.ascontiguousarray(I.as_array(inputMask) == label).view(np.uint8)
+    out = lbp3d_device(_to_device(arr), _to_device(roi), levels, radius, subdivision, arr.dtype).cpu().numpy()
+    for l_idx in range(levels):
+        yield I.like(inputImage, out[l_idx]), f"lbp-3D-m{l_idx + 1}", kwargs
+    yield I.like(inputImage, out[levels]), "lbp-3D-k", kwargs

@@ -1,9 +1,10 @@
 """Device-resident end-to-end pipelines over the hot path (BASELINE.json configs 4 and 5):
 
 * ``voxel_suite_with_filters`` -- Original + wavelet (8 sub-bands) + LoG (one per sigma) derived
-  images -> per-image gray-level discretisation -> the five fused voxel-based texture kernels,
-  everything on one GPU without host round trips (what ``RadiomicsFeatureExtractor.execute(...,
-  voxelBased=True)`` does image type by image type, reference radiomics/featureextractor.py:371-392).
+  images (+ the 3-D LBP images on request) -> per-image gray-level discretisation -> the five fused
+  voxel-based texture kernels, everything on one GPU without host round trips (what
+  ``RadiomicsFeatureExtractor.execute(..., voxelBased=True)`` does image type by image type, reference
+  radiomics/featureextractor.py:371-392).
 * ``segment_batch`` -- segment-based matrices + features for a list of independent cases, sharded
   round-robin over the ranks of the process group with no collective (the reference's own
   parallel model: one case per worker, radiomics/scripts/__init__.py:393-404).
@@ -17,8 +18,10 @@ from ._lib import CLASSES
 
 
 def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1", sigmas=(1.0, 2.0, 3.0),
-                   original=True):
-    """yields (name, CUDA tensor) like the reference's imageType generators"""
+                   original=True, lbp3d=None, mask=None):
+    """yields (name, CUDA tensor) like the reference's imageType generators.  `lbp3d`: a settings dict (lbp3DLevels,
+    lbp3DIcosphereRadius, lbp3DIcosphereSubdivision; {} = the defaults) adds the 3-D LBP level maps and kurtosis map of
+    the ROI `mask` (non-zero voxels) after LoG, as getLBP3DImage names them; None (default) leaves them out."""
     if original:
         yield "original", x
     if wavelet:
@@ -31,18 +34,27 @@ def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1"
         yield "wavelet-LLL", dec["aaa"][crop]
     for s in sigmas or ():
         yield f"log-sigma-{str(float(s)).replace('.', '-')}-mm-3D", IO.log_filter_device(x, float(s), spacing_zyx)
+    if lbp3d is not None:
+        if mask is None:
+            raise ValueError("the LBP 3-D images need the ROI mask")
+        levels = int(lbp3d.get("lbp3DLevels", 2))
+        maps = IO.lbp3d_device(x, mask, levels, lbp3d.get("lbp3DIcosphereRadius", 1),
+                               int(lbp3d.get("lbp3DIcosphereSubdivision", 1)))
+        for n in range(levels):
+            yield f"lbp-3D-m{n + 1}", maps[n]
+        yield "lbp-3D-k", maps[levels]
 
 
 def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CLASSES, spacing_zyx=(1.0, 1.0, 1.0),
-                             wavelet="coif1", sigmas=(1.0, 2.0, 3.0), consume=None, **kw):
+                             wavelet="coif1", sigmas=(1.0, 2.0, 3.0), consume=None, lbp3d=None, **kw):
     """image: CUDA tensor (Z,Y,X) of raw intensities, mask: CUDA uint8/bool.  For every derived
-    image: bin (binWidth/binCount in kw) -> pack -> fused kernels.  `consume(name, cls, maps)` is
-    called with each float64 [F,Z,Y,X] result (maps are reused buffers unless consume keeps them);
-    returns the list of (image name, Ng, number of levels)."""
+    image (`lbp3d`: see derived_images): bin (binWidth/binCount in kw) -> pack -> fused kernels.
+    `consume(name, cls, maps)` is called with each float64 [F,Z,Y,X] result (maps are reused buffers unless consume keeps
+    them); returns the list of (image name, Ng, number of levels)."""
     msk = (mask != 0).to(torch.uint8).contiguous()
     outs = {}
     info = []
-    for name, img in derived_images(image, spacing_zyx, wavelet, sigmas):
+    for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=msk):
         lev32, _ = IO.bin_image_device(img.contiguous(), msk, **kw)
         Ng = int(lev32.max().item())
         lev, presence = voxel.pack_levels(lev32, msk, Ng)
@@ -74,7 +86,8 @@ def segment_batch(cases, classes=tuple(FC.FEATURE_CLASSES), rank=0, world=1, **k
 def derived_images_slab(own: torch.Tensor, Z: int, rank: int, world: int, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1",
                         sigmas=(1.0, 2.0, 3.0), original=True):
     """`derived_images` for a volume that is sharded into z-slabs over the ranks of the default process group
-    (SURVEY.md section 8e): yields (name, this rank's slab of the derived image).
+    (SURVEY.md section 8e): yields (name, this rank's slab of the derived image).  No LBP 3-D here: its B-spline
+    prefilter is a recursion over whole lines along z.
       * wavelet: the transform is periodic, so the slab gets (F-1-F/2) planes from the rank below and F/2 from the rank
         above, ring-closed between rank 0 and the last rank (distributed.SlabHalo(periodic=True)); an odd global Z is
         wrap-padded by handing the last rank a copy of rank 0's first plane, like the reference pads before transforming;

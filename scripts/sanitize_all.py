@@ -1,6 +1,6 @@
 """compute-sanitizer target: ONE small invocation of every kernel family of the library (fused voxel fast
 paths, the generic voxel kernel, the cMatrices builders in segment and voxel-batch mode, discretisation,
-wavelet, LoG, shape, first-order).  Run as
+wavelet, LoG, shape, first-order, 3-D LBP).  Run as
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python scripts/sanitize_all.py [N] [family ...]
 The families are independent so a slow tool can be pointed at one of them."""
 import os
@@ -15,7 +15,7 @@ from pyradiomics_b200 import _lib, cmatrices, cshape, featureclasses as FC, imag
 args = [a for a in sys.argv[1:]]
 N = int(args.pop(0)) if args and args[0].isdigit() else 20
 N16 = N - N % 16 if N >= 16 else N
-fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder"]
+fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d"]
 rng = np.random.default_rng(0)
 
 
@@ -105,4 +105,10 @@ if "firstorder" in fams:
     raw = (vols["smooth"].astype(np.float64) - 1) * 25 + rng.random(mask_full.shape) * 20
     r = FC.RadiomicsFirstOrder(raw, mask_rag.astype(np.int32), voxelBased=True, binWidth=25).execute()
     print("firstorder ok", len(r), flush=True)
+if "lbp3d" in fams:
+    raw = ((vols["smooth"] - 1) * 25 + 3).astype(np.int16)
+    for kw in ({}, {"lbp3DLevels": 4, "lbp3DIcosphereRadius": 1.5, "lbp3DIcosphereSubdivision": 2}):
+        names = [n for _, n, _ in IO.getLBP3DImage(raw, mask_rag.astype(np.uint8), **kw)]
+    torch.cuda.synchronize()
+    print("lbp3d ok", names, flush=True)
 print("sanitize_all done")
