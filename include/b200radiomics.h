@@ -248,6 +248,27 @@ int rb_lbp3d_dev(const void *img_dev, int img_dtype, int sample_dtype, const uin
                  const double *vertices_host, int nv, const double *harmonics_host, int levels,
                  double *coeff_scratch_dev, double *out_dev, void *stream);
 
+/* ---- per-voxel image types (reference radiomics/imageoperations.py:973-1073, getSquareImage, getSquareRootImage,
+ *      getLogarithmImage, getExponentialImage).  out_dev[i] = f(x), x = img_dev[i] as float64, for i < nvoxels:
+ *   RB_PW_SQUARE       (c x)^2                                   c = 1 / sqrt(M)                  (:989-991)
+ *   RB_PW_SQUAREROOT   x > 0: sqrt(x c), x < 0: -sqrt(-x c), else x   c = M                        (:1014-1017)
+ *   RB_PW_LOGARITHM    (x > 0: log(x + 1), x < 0: -log(-(x - 1)), else x) * c
+ *                                                                c = M / log(M + 1)               (:1041-1045)
+ *   RB_PW_EXPONENTIAL  exp(c x)                                  c = log(M) / M                   (:1067-1069)
+ * with M = max|x| over the whole image (rb_minmax_dev with mask_dev = NULL: max(-min, max)).  The caller computes `c`
+ * (the reference's NumPy scalar arithmetic); the products and sqrt are correctly rounded, log / exp are CUDA's (<= 1 ulp).
+ * dtype codes as rb_minmax_dev. */
+enum { RB_PW_SQUARE = 0, RB_PW_SQUAREROOT = 1, RB_PW_LOGARITHM = 2, RB_PW_EXPONENTIAL = 3 };
+int rb_pointwise_image_dev(const void *img_dev, int dtype, long long nvoxels, int kind, double c, double *out_dev,
+                           void *stream);
+/* Gradient magnitude image type (reference radiomics/imageoperations.py:1076-1091, getGradientImage ->
+ * sitk.GradientMagnitudeImageFilter): per axis i in x, y, z order g_i = (-0.5 w_i f[-1] + 0 f[0]) + 0.5 w_i f[+1],
+ * neighbours outside the volume clamped to the edge (zero-flux Neumann), out = sqrt(((0 + gx^2) + gy^2) + gz^2), float64,
+ * every step rounded separately (no FMA).  weights_zyx (HOST, 3 doubles) = 1 / spacing (UseImageSpacing) or ones.  A 2-D
+ * image is passed as Z = 1. */
+int rb_gradient_magnitude_dev(const void *img_dev, int dtype, int Z, int Y, int X, const double *weights_zyx,
+                              double *out_dev, void *stream);
+
 /* ---- segment-mode shape coefficients (SURVEY.md section 8f rank 4) ------------------------------
  * rb_calculate_coefficients replaces calculate_coefficients (radiomics/src/cshape.h:1-2, binding
  *   radiomics/src/_cshape.c:75-113): HOST mask (non-zero = ROI) of `size` = {Z, Y, X} with element

@@ -70,6 +70,8 @@ int shape2d_coefficients_dev(const uint8_t* mask_dev, int Y, int X, long long sy
                              cudaStream_t st);
 int digitize_launch(const void* img, int dt, const uint8_t* mask, long long n, const double* edges, int ne, int32_t* out,
                     cudaStream_t st);
+int pointwise_image_launch(const void* img, int dt, long long n, int kind, double c, double* out, cudaStream_t st);
+int gradient_magnitude_launch(const void* img, int dt, int Z, int Y, int X, const double* w_zyx, double* out, cudaStream_t st);
 int swt_axis_launch(const double* in, int Z, int Y, int X, int axis, const double* lo, const double* hi, int F,
                     double* out_lo, double* out_hi, cudaStream_t st);
 int recursive_gauss_launch(const void* in, int in_is_f32, int Z, int Y, int X, int axis, const double* coef20, float* out,
@@ -339,6 +341,23 @@ int rb_digitize_dev(const void* image_dev, int dtype, const uint8_t* mask_dev, l
   if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
   if (nedges < 1) return fail(RB_ERR_ARG, "need at least one bin edge");
   return digitize_launch(image_dev, dtype, mask_dev, nvoxels, edges_dev, nedges, out_dev, (cudaStream_t)stream);
+}
+// getSquareImage / getSquareRootImage / getLogarithmImage / getExponentialImage, radiomics/imageoperations.py:973-1073
+int rb_pointwise_image_dev(const void* img_dev, int dtype, long long nvoxels, int kind, double c, double* out_dev,
+                           void* stream) {
+  if (!img_dev || !out_dev) return fail(RB_ERR_ARG, "pointwise image: null argument");
+  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (kind < RB_PW_SQUARE || kind > RB_PW_EXPONENTIAL) return fail(RB_ERR_ARG, "pointwise image: unknown kind %d", kind);
+  if (nvoxels < 1) return fail(RB_ERR_ARG, "pointwise image: %lld voxels", nvoxels);
+  return pointwise_image_launch(img_dev, dtype, nvoxels, kind, c, out_dev, (cudaStream_t)stream);
+}
+// getGradientImage (sitk.GradientMagnitudeImageFilter), radiomics/imageoperations.py:1076-1091
+int rb_gradient_magnitude_dev(const void* img_dev, int dtype, int Z, int Y, int X, const double* weights_zyx,
+                              double* out_dev, void* stream) {
+  if (!img_dev || !weights_zyx || !out_dev) return fail(RB_ERR_ARG, "gradient magnitude: null argument");
+  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (Z < 1 || Y < 1 || X < 1) return fail(RB_ERR_ARG, "gradient magnitude: empty volume %d x %d x %d", Z, Y, X);
+  return gradient_magnitude_launch(img_dev, dtype, Z, Y, X, weights_zyx, out_dev, (cudaStream_t)stream);
 }
 int rb_swt_axis_dev(const double* in_dev, int Z, int Y, int X, int axis, const double* dec_lo, const double* dec_hi,
                     int flen, double* out_lo_dev, double* out_hi_dev, void* stream) {

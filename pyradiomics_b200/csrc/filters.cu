@@ -5,6 +5,8 @@
 //     (reference radiomics/imageoperations.py:899-970 -> pywt.swtn(level=1), PyWavelets >= 1.6)
 //   * Laplacian of Gaussian by recursive (IIR) Gaussian filtering, one line per thread
 //     (reference radiomics/imageoperations.py:756-836 -> ITK LaplacianRecursiveGaussianImageFilter)
+//   * the square / squareroot / logarithm / exponential image types, one pass per voxel, and the gradient
+//     magnitude (reference radiomics/imageoperations.py:973-1091 -> ITK GradientMagnitudeImageFilter)
 // All are HBM-streaming kernels: every thread handles consecutive x so loads/stores coalesce; the
 // wavelet pass reads its 6 taps through L1 (neighbouring threads share them).
 #include "common.cuh"
@@ -51,6 +53,65 @@ minmax_kernel(const void* __restrict__ img, int dt, const uint8_t* __restrict__ 
     atomicMin(&keys[0], f64_key(lo));
     atomicMax(&keys[1], f64_key(hi));
     atomicAdd((unsigned long long*)&keys[2], (unsigned long long)cnt);
+  }
+}
+
+// ---- per-voxel image types (reference radiomics/imageoperations.py:973-1073).  The scalar `c` comes from the host,
+// where it is computed by the reference's own NumPy expression from M = max|x|.  Every product and sum is an explicit
+// _rn intrinsic, so no FMA contraction can make a voxel differ from NumPy's; sqrt is correctly rounded, log / exp <= 1 ulp.
+template <int KIND>
+__global__ void __launch_bounds__(256)
+pointwise_image_kernel(const void* __restrict__ img, int dt, long long n, double c, double* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const double x = load_any(img, dt, i);
+    double r;
+    if (KIND == RB_PW_SQUARE) {
+      const double t = __dmul_rn(c, x);
+      r = __dmul_rn(t, t);
+    } else if (KIND == RB_PW_SQUAREROOT) {            // 0 and NaN stay as they are
+      r = x > 0 ? sqrt(__dmul_rn(x, c)) : x < 0 ? -sqrt(__dmul_rn(-x, c)) : x;
+    } else if (KIND == RB_PW_LOGARITHM) {
+      r = __dmul_rn(x > 0 ? log(__dadd_rn(x, 1.0)) : x < 0 ? -log(-__dadd_rn(x, -1.0)) : x, c);
+    } else {
+      r = exp(__dmul_rn(c, x));
+    }
+    out[i] = r;
+  }
+}
+
+// ---- gradient magnitude (ITK GradientMagnitudeImageFilter as called at imageoperations.py:1089-1090): per axis the
+// central-difference inner product ((-0.5 w) f[-1] + 0 f[0]) + (0.5 w) f[+1] in ITK's order, neighbours clamped to the
+// edge (zero-flux Neumann), then sqrt(((0 + gx^2) + gy^2) + gz^2).  The 0 * f[0] term is kept so that inf / NaN spread
+// as they do in ITK.  A thread owns one (y, x) column and marches GRAD_ZCHUNK planes along z, keeping f[z-1], f[z],
+// f[z+1] in registers: one new load from HBM per voxel, the four in-plane neighbours were loaded by the neighbouring
+// threads in the previous step and come from L1.
+constexpr int GRAD_TX = 128, GRAD_ZCHUNK = 32;
+
+__device__ __forceinline__ double central_diff(double fm, double f0, double fp, double w) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(-0.5 * w, fm), __dmul_rn(0.0, f0)), __dmul_rn(0.5 * w, fp));
+}
+
+__global__ void __launch_bounds__(GRAD_TX)
+gradient_magnitude_kernel(const void* __restrict__ img, int dt, int Z, int Y, int X, double wz, double wy, double wx,
+                          double* __restrict__ out) {
+  const int tiles_x = (X + GRAD_TX - 1) / GRAD_TX;
+  const int y = blockIdx.x / tiles_x, x = (blockIdx.x % tiles_x) * GRAD_TX + threadIdx.x;
+  if (x >= X) return;
+  const int z0 = blockIdx.y * GRAD_ZCHUNK, z1 = min(z0 + GRAD_ZCHUNK, Z);
+  const long long plane = (long long)Y * X;
+  const int dxm = x > 0 ? -1 : 0, dxp = x < X - 1 ? 1 : 0;
+  const int dym = y > 0 ? -X : 0, dyp = y < Y - 1 ? X : 0;
+  long long i = (long long)z0 * plane + (long long)y * X + x;
+  double f0 = load_any(img, dt, i);
+  double fm = z0 > 0 ? load_any(img, dt, i - plane) : f0;
+  for (int z = z0; z < z1; z++, i += plane) {
+    const double fp = z < Z - 1 ? load_any(img, dt, i + plane) : f0;
+    const double gx = central_diff(load_any(img, dt, i + dxm), f0, load_any(img, dt, i + dxp), wx);
+    const double gy = central_diff(load_any(img, dt, i + dym), f0, load_any(img, dt, i + dyp), wy);
+    const double gz = central_diff(fm, f0, fp, wz);
+    out[i] = sqrt(__dadd_rn(__dadd_rn(__dadd_rn(0.0, __dmul_rn(gx, gx)), __dmul_rn(gy, gy)), __dmul_rn(gz, gz)));
+    fm = f0;
+    f0 = fp;
   }
 }
 
@@ -307,6 +368,26 @@ static int grid_n(long long n, int block, int per_sm) {
 
 int minmax_launch(const void* img, int dt, const uint8_t* mask, long long n, long long* keys, cudaStream_t st) {
   minmax_kernel<<<grid_n(n, 256, 8), 256, 0, st>>>(img, dt, mask, n, keys);
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+int pointwise_image_launch(const void* img, int dt, long long n, int kind, double c, double* out, cudaStream_t st) {
+  const int grid = grid_n(n, 256, 8);
+  switch (kind) {
+    case RB_PW_SQUARE: pointwise_image_kernel<RB_PW_SQUARE><<<grid, 256, 0, st>>>(img, dt, n, c, out); break;
+    case RB_PW_SQUAREROOT: pointwise_image_kernel<RB_PW_SQUAREROOT><<<grid, 256, 0, st>>>(img, dt, n, c, out); break;
+    case RB_PW_LOGARITHM: pointwise_image_kernel<RB_PW_LOGARITHM><<<grid, 256, 0, st>>>(img, dt, n, c, out); break;
+    case RB_PW_EXPONENTIAL: pointwise_image_kernel<RB_PW_EXPONENTIAL><<<grid, 256, 0, st>>>(img, dt, n, c, out); break;
+    default: return fail(RB_ERR_ARG, "pointwise image: unknown kind %d", kind);
+  }
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+int gradient_magnitude_launch(const void* img, int dt, int Z, int Y, int X, const double* w_zyx, double* out, cudaStream_t st) {
+  const long long columns = (long long)((X + GRAD_TX - 1) / GRAD_TX) * Y;
+  if (columns > 0x7fffffffLL) return fail(RB_ERR_UNSUPPORTED, "gradient magnitude: %d x %d plane too large", Y, X);
+  const dim3 grid((unsigned)columns, (unsigned)((Z + GRAD_ZCHUNK - 1) / GRAD_ZCHUNK));
+  gradient_magnitude_kernel<<<grid, GRAD_TX, 0, st>>>(img, dt, Z, Y, X, w_zyx[0], w_zyx[1], w_zyx[2], out);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }

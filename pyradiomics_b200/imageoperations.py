@@ -1,12 +1,16 @@
 """GPU versions of the pyradiomics image operations that sit on the texture hot path
 (reference radiomics/imageoperations.py): gray-level discretisation (getBinEdges / binImage,
 :67-174), the level-1 stationary wavelet decomposition (getWaveletImage / _swt3, :839-970), the
-Laplacian-of-Gaussian filter (getLoGImage, :756-836) and the 3-D local binary pattern (getLBP3DImage, :1169-1314).  Same function names, arguments and yielded
-tuples as the reference so they can be dropped into ``radiomics.imageoperations``.
+Laplacian-of-Gaussian filter (getLoGImage, :756-836), the per-voxel square / square root /
+logarithm / exponential images (getSquareImage ... getExponentialImage, :973-1073), the gradient
+magnitude (getGradientImage, :1076-1091) and the 3-D local binary pattern (getLBP3DImage,
+:1169-1314).  Same function names, arguments and yielded tuples as the reference so they can be
+dropped into ``radiomics.imageoperations``.
 
-Parity status (DESIGN.md): binning is bit-identical to NumPy; wavelet and LoG restate PyWavelets'
-and ITK's published algorithms -- neither library is available offline and the reference's own
-tests do not pin them (SURVEY.md section 8c) -> "parity unpinned" for those two.
+Parity status (DESIGN.md): binning, square and square root are bit-identical to NumPy, logarithm and
+exponential within CUDA's 1-ulp log / exp; wavelet, LoG and gradient restate PyWavelets' and ITK's
+published algorithms -- neither library is available offline and the reference's own tests do not
+pin them (SURVEY.md section 8c) -> "parity unpinned" for those three.
 """
 from __future__ import annotations
 
@@ -512,6 +516,118 @@ def getLoGImage(inputImage, _inputMask, **kwargs):
                                sigma, spacing, size)
         else:
             logger.warning("applyLoG: sigma must be greater than 0.0: %s", sigma)
+
+
+# ------------------------------------------------------------------------------------ square, square root, logarithm,
+# exponential, gradient
+POINTWISE_KINDS = {"square": 0, "squareroot": 1, "logarithm": 2, "exponential": 3}      # rb_pointwise_image_dev codes
+
+
+def pointwise_scalar(kind, max_abs):
+    """the scalar rb_pointwise_image_dev applies for M = max|x| = `max_abs`, by the reference's own NumPy expressions
+    (imageoperations.py:989, :1014, :1041-1044, :1066-1067), so that it is the reference's to the bit.  Logarithm: the
+    reference divides M by max|transformed image|, which is log(M + 1) whichever sign M comes from (log is monotone and
+    -(x - 1) == 1 + |x| exactly for x < 0), so no second reduction is needed.  That log is taken over an array, as the
+    reference takes it: NumPy may evaluate a 0-d log by another routine than a contiguous array's."""
+    im_max = np.float64(max_abs)
+    with np.errstate(divide="ignore", invalid="ignore"):            # an all-zero image: NaN images, as in the reference
+        if kind == "square":
+            return float(1 / np.sqrt(im_max))
+        if kind == "squareroot":
+            return float(im_max)
+        if kind == "logarithm":
+            return float(im_max / np.log(np.array([im_max]) + 1)[0])
+        if kind == "exponential":
+            return float(np.log(im_max) / im_max)
+    raise ValueError(f"unknown image type {kind!r} (one of {sorted(POINTWISE_KINDS)})")
+
+
+def image_max_abs(x: torch.Tensor) -> float:
+    """M = max|x| over the whole CUDA tensor: one rb_minmax_dev pass without a mask, |max(-min, max)| (the abs turns the
+    -0.0 of an all-zero image into 0.0, as np.abs does).  NaN voxels do not take part (the reference's np.max(np.abs(im))
+    would be NaN and turn the square / logarithm / exponential images into NaN everywhere)."""
+    mn, mx, _ = roi_minmax(x, None)
+    return abs(max(-mn, mx))
+
+
+def pointwise_image_device(x: torch.Tensor, kind: str, max_abs=None):
+    """square / squareroot / logarithm / exponential image (getSquareImage ... getExponentialImage) of a CUDA tensor of
+    any shape -> float64 CUDA tensor of that shape (rb_pointwise_image_dev).  `max_abs`: M = max|x| over the whole
+    image; None reduces it here (a caller that makes several of these types passes one image_max_abs to all)."""
+    if kind not in POINTWISE_KINDS:
+        raise ValueError(f"unknown image type {kind!r} (one of {sorted(POINTWISE_KINDS)})")
+    src = x.contiguous()
+    if src.dtype not in _TORCH_DT:
+        raise ValueError(f"unsupported pixel type {src.dtype}")
+    if max_abs is None:
+        max_abs = image_max_abs(src)
+    out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
+    check(lib().rb_pointwise_image_dev(_ptr(src), _TORCH_DT[src.dtype], C.c_longlong(src.numel()), POINTWISE_KINDS[kind],
+                                       C.c_double(pointwise_scalar(kind, max_abs)), _ptr(out), _stream()), kind)
+    return out
+
+
+def gradient_magnitude_device(x: torch.Tensor, spacing_zyx=None):
+    """gradient magnitude (sitk.GradientMagnitudeImageFilter, getGradientImage) of a CUDA volume (Z,Y,X) or plane (Y,X)
+    -> float64 CUDA tensor of that shape (rb_gradient_magnitude_dev).  `spacing_zyx`: one spacing per axis that the
+    differences are divided by (gradientUseSpacing=True); None = unit weights.  A zero spacing raises ValueError."""
+    src = x.contiguous()
+    if src.dim() not in (2, 3):
+        raise ValueError(f"gradient: 2-D or 3-D image expected, got {src.dim()}-D")
+    if src.dtype not in _TORCH_DT:
+        raise ValueError(f"unsupported pixel type {src.dtype}")
+    w = [1.0] * 3
+    if spacing_zyx is not None:
+        sp = [float(s) for s in spacing_zyx]
+        if len(sp) != src.dim():
+            raise ValueError(f"gradient: {len(sp)} spacings for a {src.dim()}-D image")
+        if 0.0 in sp:
+            raise ValueError(f"gradient: image spacing cannot be zero, got {tuple(sp)}")
+        w[3 - len(sp):] = [1.0 / s for s in sp]
+    Z, Y, X = (1,) * (3 - src.dim()) + tuple(src.shape)
+    out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
+    check(lib().rb_gradient_magnitude_dev(_ptr(src), _TORCH_DT[src.dtype], Z, Y, X, (C.c_double * 3)(*w), _ptr(out),
+                                          _stream()), "gradient")
+    return out
+
+
+def _pointwise_image(inputImage, kind, kwargs):
+    out = pointwise_image_device(_to_device(I.as_array(inputImage)), kind).cpu().numpy()
+    logger.debug("Yielding %s image", kind)
+    yield I.like(inputImage, out), kind, kwargs
+
+
+def getSquareImage(inputImage, _inputMask, **kwargs):
+    """reference generator (imageoperations.py:973-994): (c x)^2 with c = 1 / sqrt(max|x|), float64.  The sign is NOT
+    kept (the reference's docstring says it is; its code, followed here, squares it away)."""
+    yield from _pointwise_image(inputImage, "square", kwargs)
+
+
+def getSquareRootImage(inputImage, _inputMask, **kwargs):
+    """reference generator (imageoperations.py:997-1021): sqrt(x M) for x > 0, -sqrt(-x M) for x < 0, M = max|x|."""
+    yield from _pointwise_image(inputImage, "squareroot", kwargs)
+
+
+def getLogarithmImage(inputImage, _inputMask, **kwargs):
+    """reference generator (imageoperations.py:1024-1049): log(x + 1) for x > 0, -log(1 - x) for x < 0, rescaled by
+    M / log(M + 1), M = max|x|."""
+    yield from _pointwise_image(inputImage, "logarithm", kwargs)
+
+
+def getExponentialImage(inputImage, _inputMask, **kwargs):
+    """reference generator (imageoperations.py:1052-1073): exp(c x) with c = log(M) / M, M = max|x|."""
+    yield from _pointwise_image(inputImage, "exponential", kwargs)
+
+
+def getGradientImage(inputImage, _inputMask, **kwargs):
+    """reference generator (imageoperations.py:1076-1091): gradient magnitude, divided by the image spacing unless
+    gradientUseSpacing=False; float64 (ITK's real type for every scalar input).  2-D and 3-D images."""
+    arr = I.as_array(inputImage)
+    if arr.ndim not in (2, 3):
+        raise ValueError(f"gradient: 2-D or 3-D image expected, got {arr.ndim}-D")
+    spacing = tuple(I.spacing_xyz(inputImage))[::-1] if kwargs.get("gradientUseSpacing", True) else None
+    out = gradient_magnitude_device(_to_device(arr), spacing).cpu().numpy()
+    yield I.like(inputImage, out), "gradient", kwargs
 
 
 # ------------------------------------------------------------------------------------ LBP 3-D

@@ -1,10 +1,10 @@
 """Device-resident end-to-end pipelines over the hot path (BASELINE.json configs 4 and 5):
 
 * ``voxel_suite_with_filters`` -- Original + wavelet (8 sub-bands) + LoG (one per sigma) derived
-  images (+ the 3-D LBP images on request) -> per-image gray-level discretisation -> the five fused
-  voxel-based texture kernels, everything on one GPU without host round trips (what
-  ``RadiomicsFeatureExtractor.execute(..., voxelBased=True)`` does image type by image type, reference
-  radiomics/featureextractor.py:371-392).
+  images (+ the square / squareroot / logarithm / exponential / gradient and 3-D LBP images on
+  request) -> per-image gray-level discretisation -> the five fused voxel-based texture kernels,
+  everything on one GPU without host round trips (what ``RadiomicsFeatureExtractor.execute(...,
+  voxelBased=True)`` does image type by image type, reference radiomics/featureextractor.py:371-392).
 * ``segment_batch`` -- segment-based matrices + features for a list of independent cases, sharded
   round-robin over the ranks of the process group with no collective (the reference's own
   parallel model: one case per worker, radiomics/scripts/__init__.py:393-404).
@@ -17,11 +17,19 @@ from . import _lib, featureclasses as FC, imageoperations as IO, voxel
 from ._lib import CLASSES
 
 
+IMAGE_TYPES = ("square", "squareroot", "logarithm", "exponential", "gradient")
+
+
 def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1", sigmas=(1.0, 2.0, 3.0),
-                   original=True, lbp3d=None, mask=None):
-    """yields (name, CUDA tensor) like the reference's imageType generators.  `lbp3d`: a settings dict (lbp3DLevels,
+                   original=True, lbp3d=None, mask=None, image_types=(), gradient_use_spacing=True):
+    """yields (name, CUDA tensor) like the reference's imageType generators.  `image_types`: names out of IMAGE_TYPES,
+    yielded after LoG in the caller's order as float64 images (one max|x| reduction serves every per-voxel type;
+    `gradient_use_spacing` is getGradientImage's gradientUseSpacing).  `lbp3d`: a settings dict (lbp3DLevels,
     lbp3DIcosphereRadius, lbp3DIcosphereSubdivision; {} = the defaults) adds the 3-D LBP level maps and kurtosis map of
-    the ROI `mask` (non-zero voxels) after LoG, as getLBP3DImage names them; None (default) leaves them out."""
+    the ROI `mask` (non-zero voxels) after those, as getLBP3DImage names them; None (default) leaves them out."""
+    unknown = [t for t in image_types if t not in IMAGE_TYPES]
+    if unknown:
+        raise ValueError(f"unknown image types {unknown} (known: {IMAGE_TYPES})")
     if original:
         yield "original", x
     if wavelet:
@@ -34,6 +42,14 @@ def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1"
         yield "wavelet-LLL", dec["aaa"][crop]
     for s in sigmas or ():
         yield f"log-sigma-{str(float(s)).replace('.', '-')}-mm-3D", IO.log_filter_device(x, float(s), spacing_zyx)
+    max_abs = None
+    for t in image_types:
+        if t == "gradient":
+            yield t, IO.gradient_magnitude_device(x, spacing_zyx if gradient_use_spacing else None)
+            continue
+        if max_abs is None:
+            max_abs = IO.image_max_abs(x)
+        yield t, IO.pointwise_image_device(x, t, max_abs)
     if lbp3d is not None:
         if mask is None:
             raise ValueError("the LBP 3-D images need the ROI mask")
@@ -46,15 +62,18 @@ def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1"
 
 
 def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CLASSES, spacing_zyx=(1.0, 1.0, 1.0),
-                             wavelet="coif1", sigmas=(1.0, 2.0, 3.0), consume=None, lbp3d=None, **kw):
+                             wavelet="coif1", sigmas=(1.0, 2.0, 3.0), consume=None, lbp3d=None, image_types=(),
+                             gradient_use_spacing=True, **kw):
     """image: CUDA tensor (Z,Y,X) of raw intensities, mask: CUDA uint8/bool.  For every derived
-    image (`lbp3d`: see derived_images): bin (binWidth/binCount in kw) -> pack -> fused kernels.
+    image (`image_types`, `gradient_use_spacing`, `lbp3d`: see derived_images): bin (binWidth/binCount in kw) -> pack ->
+    fused kernels.
     `consume(name, cls, maps)` is called with each float64 [F,Z,Y,X] result (maps are reused buffers unless consume keeps
     them); returns the list of (image name, Ng, number of levels)."""
     msk = (mask != 0).to(torch.uint8).contiguous()
     outs = {}
     info = []
-    for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=msk):
+    for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=msk, image_types=image_types,
+                                    gradient_use_spacing=gradient_use_spacing):
         lev32, _ = IO.bin_image_device(img.contiguous(), msk, **kw)
         Ng = int(lev32.max().item())
         lev, presence = voxel.pack_levels(lev32, msk, Ng)
@@ -87,7 +106,9 @@ def derived_images_slab(own: torch.Tensor, Z: int, rank: int, world: int, spacin
                         sigmas=(1.0, 2.0, 3.0), original=True):
     """`derived_images` for a volume that is sharded into z-slabs over the ranks of the default process group
     (SURVEY.md section 8e): yields (name, this rank's slab of the derived image).  No LBP 3-D here: its B-spline
-    prefilter is a recursion over whole lines along z.
+    prefilter is a recursion over whole lines along z.  No square / squareroot / logarithm / exponential / gradient
+    either: the per-voxel types would need max|x| all-reduced over the ranks, the gradient a replicated edge plane at
+    the volume's global z faces.
       * wavelet: the transform is periodic, so the slab gets (F-1-F/2) planes from the rank below and F/2 from the rank
         above, ring-closed between rank 0 and the last rank (distributed.SlabHalo(periodic=True)); an odd global Z is
         wrap-padded by handing the last rank a copy of rank 0's first plane, like the reference pads before transforming;

@@ -1,6 +1,7 @@
 """compute-sanitizer target: ONE small invocation of every kernel family of the library (fused voxel fast
 paths, the generic voxel kernel, the cMatrices builders in segment and voxel-batch mode, discretisation,
-wavelet, LoG, shape, first-order, 3-D LBP).  Run as
+wavelet, LoG, shape, first-order, 3-D LBP, the square / squareroot / logarithm / exponential / gradient
+image types).  Run as
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python scripts/sanitize_all.py [N] [family ...]
 The families are independent so a slow tool can be pointed at one of them."""
 import os
@@ -10,12 +11,12 @@ import numpy as np
 import torch
 
 sys.path.insert(0, ".")
-from pyradiomics_b200 import _lib, cmatrices, cshape, featureclasses as FC, imageoperations as IO, voxel
+from pyradiomics_b200 import _lib, cmatrices, cshape, featureclasses as FC, image as I, imageoperations as IO, voxel
 
 args = [a for a in sys.argv[1:]]
 N = int(args.pop(0)) if args and args[0].isdigit() else 20
 N16 = N - N % 16 if N >= 16 else N
-fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d"]
+fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d", "imagetypes"]
 rng = np.random.default_rng(0)
 
 
@@ -111,4 +112,13 @@ if "lbp3d" in fams:
         names = [n for _, n, _ in IO.getLBP3DImage(raw, mask_rag.astype(np.uint8), **kw)]
     torch.cuda.synchronize()
     print("lbp3d ok", names, flush=True)
+if "imagetypes" in fams:
+    raw = ((vols["smooth"] - 1) * 25 - 300).astype(np.int16)
+    names = []
+    for img in (raw, raw[0].astype(np.uint8), raw.astype(np.float32) / 7):
+        for gen in (IO.getSquareImage, IO.getSquareRootImage, IO.getLogarithmImage, IO.getExponentialImage,
+                    IO.getGradientImage):
+            names += [n for _, n, _ in gen(I.ArrayImage(img, (0.7, 1.1, 2.0)[:img.ndim]), None)]
+    torch.cuda.synchronize()
+    print("imagetypes ok", names[:5], flush=True)
 print("sanitize_all done")
