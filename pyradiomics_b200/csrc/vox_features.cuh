@@ -468,7 +468,7 @@ RB_HD void glcm_voxel(const uint16_t* w, const VoxParams& P, double* out, int* s
   }
   double sum[GLCM_NF]; int cnt[GLCM_NF];
   for (int k = 0; k < GLCM_NF; k++) { sum[k] = 0; cnt[k] = 0; }
-  bool ja_nan = false;
+  bool ja_nan = false, mcc_nan = false;
   for (int a = 0; a < P.na; a++) {
     const int az = P.ang[a][0], ay = P.ang[a][1], ax = P.ang[a][2];
     Entries<ECAP, int> E; E.clear();
@@ -479,13 +479,18 @@ RB_HD void glcm_voxel(const uint16_t* w, const VoxParams& P, double* out, int* s
       E.add(((uint32_t)li << 16) | lj, 1);
       if (P.symmetric) E.add(((uint32_t)lj << 16) | li, 1);
     }
-    bool ok = glcm_angle_features<ECAP, WCAP, NJCAP, int>(E, n, val, P, f, status);
+    int ast = 0;
+    bool ok = glcm_angle_features<ECAP, WCAP, NJCAP, int>(E, n, val, P, f, &ast);
+    if (status) *status |= ast;
+    if (ast & 1) mcc_nan = true;
     if (!ok) { if (P.alive[a >> 5] >> (a & 31) & 1u) ja_nan = true; continue; }
     for (int k = 0; k < GLCM_NF; k++) if (f[k] == f[k]) { sum[k] += f[k]; cnt[k]++; }
   }
   for (int k = 0; k < GLCM_NF; k++) out[k] = cnt[k] ? sum[k] / cnt[k] : NAN;
   // JointAverage is a plain mean over the kept angles (glcm.py:292): NaN propagates
   if (ja_nan) out[G_JointAverage] = NAN;
+  // an angle whose MCC is over the solver's capacity (status bit 0) has no value: the voxel's mean has none either
+  if (mcc_nan) out[G_MCC] = NAN;
 }
 
 // --------------------------------------------------------------------------------------------

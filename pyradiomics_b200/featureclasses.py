@@ -357,7 +357,8 @@ class RadiomicsFeaturesBase:
         if st & 2:
             raise _lib.B200Error("weighted GLCM entry list overflow")
         if st & 1:
-            self.logger.warning("MCC eigen-problem too large for the in-kernel solver at some voxels: NaN stored")
+            self.logger.warning("MCC eigen-problem too large for the in-kernel solver (more than 32 gray levels in one "
+                                "matrix of a voxel's window): NaN stored as the MCC of those voxels")
         arrs = host.numpy()                      # views of ONE page-locked block the returned images keep alive
         for pos, k in enumerate(idx):
             arr = arrs[pos] if self._rawImageArray.ndim == 3 else arrs[pos][0]

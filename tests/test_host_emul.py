@@ -11,7 +11,7 @@ import pytest
 
 import cmatrices_oracle as O
 import pipeline as PL
-from helpers import assert_maps_close, binned, ref_map, voxel_goldens
+from helpers import alive_mask_bruteforce, assert_maps_close, binned, ref_map, voxel_goldens
 from pyradiomics_b200 import _lib
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -43,25 +43,6 @@ def emul():
     subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-Wno-unknown-pragmas", "-o", so + ".%d" % os.getpid(), src])
     os.replace(so + ".%d" % os.getpid(), so)
     return C.CDLL(so)
-
-
-def alive_mask_bruteforce(lev, centers, ang, r3):
-    """which GLCM angles have a co-occurrence inside at least one kernel window (numpy restatement
-    of the reference's 'delete empty angles', radiomics/glcm.py:187-196)."""
-    m = lev != 0
-    out = np.zeros(_lib.ALIVE_WORDS, np.uint32)
-    for ai, a in enumerate(ang):
-        pm = np.zeros_like(m)
-        src = tuple(slice(max(0, -a[d]), lev.shape[d] - max(0, a[d])) for d in range(3))
-        dst = tuple(slice(max(0, a[d]), lev.shape[d] + min(0, a[d])) for d in range(3))
-        pm[src] = m[src] & m[dst]
-        for c in zip(*np.where(centers)):
-            lo = [max(c[d] - r3[d], c[d] - r3[d] - a[d], 0) for d in range(3)]
-            hi = [min(c[d] + r3[d], c[d] + r3[d] - a[d], lev.shape[d] - 1) for d in range(3)]
-            if all(lo[d] <= hi[d] for d in range(3)) and pm[lo[0]:hi[0] + 1, lo[1]:hi[1] + 1, lo[2]:hi[2] + 1].any():
-                out[ai >> 5] |= np.uint32(1 << (ai & 31))
-                break
-    return out
 
 
 def test_feature_name_tables_match_library_order():

@@ -74,7 +74,7 @@ def test_processed_matrices_match_reference_golden(seg, case):
         assert np.abs(P - cases[f"{case}_{cname}_P"]).max() < 1e-3
 
 
-@pytest.mark.parametrize("name,z,kw", voxel_goldens(), ids=[g[0] for g in voxel_goldens()])
+@pytest.mark.parametrize("name,z,kw", voxel_goldens(extra=True), ids=[g[0] for g in voxel_goldens(extra=True)])
 def test_voxel_based_plugin_maps_match_reference(name, z, kw):
     sp = z["spacing"]
     img = I.ArrayImage(z["image"], sp)
