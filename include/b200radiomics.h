@@ -269,6 +269,27 @@ int rb_pointwise_image_dev(const void *img_dev, int dtype, long long nvoxels, in
 int rb_gradient_magnitude_dev(const void *img_dev, int dtype, int Z, int Y, int X, const double *weights_zyx,
                               double *out_dev, void *stream);
 
+/* ---- normalisation and resegmentation (reference radiomics/imageoperations.py:615-742, normalizeImage and
+ *      resegmentMask).  dtype codes as rb_minmax_dev.
+ * rb_roi_moments_dev: over the voxels with mask_dev[i] != 0 (mask_dev NULL = every voxel), in float64:
+ *   out_dev[0] count, [1] NaN count, [2] sum, [3] maximum (NaN if any voxel is NaN, as np.max), and with passes == 2
+ *   [4] sum of (x - mean)^2, mean = [2] / [0] (passes == 1 leaves [4] NaN).  Replaces sitk.Normalize's statistics
+ *   (:638, over the whole image) and the np.max / np.mean / np.std of the ROI (:699, :704-705).  The partial sums go
+ *   to scratch_dev (RB_MOMENTS_SCRATCH_BYTES) from a grid that depends on nvoxels only, and one block adds them in a
+ *   fixed order: the result is bit-identical from run to run and card to card.
+ * rb_normalize_dev: out_dev[i] = ((x - mean) * (1 / sigma)), clamped to [-outliers, outliers] when remove_outliers
+ *   (NaN stays NaN), then * scale, float64, every step rounded separately (:638-652: ITK's ShiftScale form).
+ * rb_resegment_dev: out_dev[i] = 1 if mask_dev[i] != 0 and lower <= x (and x <= upper when nthresholds == 2), else 0
+ *   (:713-722).  lower / upper must already be rounded to the dtype NumPy compares in (float32 for a float32 image).
+ *   counts_dev[0] = ROI voxels, counts_dev[1] = kept voxels. */
+enum { RB_MOMENTS_SCRATCH_BYTES = 40960 };
+int rb_roi_moments_dev(const void *img_dev, int dtype, const uint8_t *mask_dev, long long nvoxels, int passes,
+                       void *scratch_dev, double *out_dev, void *stream);
+int rb_normalize_dev(const void *img_dev, int dtype, long long nvoxels, double mean, double sigma, int remove_outliers,
+                     double outliers, double scale, double *out_dev, void *stream);
+int rb_resegment_dev(const void *img_dev, int dtype, const uint8_t *mask_dev, long long nvoxels, double lower,
+                     double upper, int nthresholds, uint8_t *out_dev, unsigned long long *counts_dev, void *stream);
+
 /* ---- segment-mode shape coefficients (SURVEY.md section 8f rank 4) ------------------------------
  * rb_calculate_coefficients replaces calculate_coefficients (radiomics/src/cshape.h:1-2, binding
  *   radiomics/src/_cshape.c:75-113): HOST mask (non-zero = ROI) of `size` = {Z, Y, X} with element

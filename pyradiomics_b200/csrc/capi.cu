@@ -72,6 +72,12 @@ int digitize_launch(const void* img, int dt, const uint8_t* mask, long long n, c
                     cudaStream_t st);
 int pointwise_image_launch(const void* img, int dt, long long n, int kind, double c, double* out, cudaStream_t st);
 int gradient_magnitude_launch(const void* img, int dt, int Z, int Y, int X, const double* w_zyx, double* out, cudaStream_t st);
+int roi_moments_launch(const void* img, int dt, const uint8_t* mask, long long n, int passes, void* scratch, double* res,
+                       cudaStream_t st);
+int normalize_launch(const void* img, int dt, long long n, double mean, double sigma, int clamp, double outliers,
+                     double scale, double* out, cudaStream_t st);
+int resegment_launch(const void* img, int dt, const uint8_t* mask, long long n, double lo, double hi, int two,
+                     uint8_t* out, unsigned long long* counts, cudaStream_t st);
 int swt_axis_launch(const double* in, int Z, int Y, int X, int axis, const double* lo, const double* hi, int F,
                     double* out_lo, double* out_hi, cudaStream_t st);
 int recursive_gauss_launch(const void* in, int in_is_f32, int Z, int Y, int X, int axis, const double* coef20, float* out,
@@ -358,6 +364,35 @@ int rb_gradient_magnitude_dev(const void* img_dev, int dtype, int Z, int Y, int 
   if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
   if (Z < 1 || Y < 1 || X < 1) return fail(RB_ERR_ARG, "gradient magnitude: empty volume %d x %d x %d", Z, Y, X);
   return gradient_magnitude_launch(img_dev, dtype, Z, Y, X, weights_zyx, out_dev, (cudaStream_t)stream);
+}
+// sitk.Normalize's statistics (radiomics/imageoperations.py:638) and resegmentMask's np.max / np.mean / np.std of the
+// ROI (radiomics/imageoperations.py:699, 704-705)
+int rb_roi_moments_dev(const void* img_dev, int dtype, const uint8_t* mask_dev, long long nvoxels, int passes,
+                       void* scratch_dev, double* out_dev, void* stream) {
+  if (!img_dev || !scratch_dev || !out_dev) return fail(RB_ERR_ARG, "roi moments: null argument");
+  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (nvoxels < 1) return fail(RB_ERR_ARG, "roi moments: %lld voxels", nvoxels);
+  if (passes != 1 && passes != 2) return fail(RB_ERR_ARG, "roi moments: passes must be 1 or 2, got %d", passes);
+  return roi_moments_launch(img_dev, dtype, mask_dev, nvoxels, passes, scratch_dev, out_dev, (cudaStream_t)stream);
+}
+// normalizeImage (sitk.Normalize, removeOutliers, normalizeScale), radiomics/imageoperations.py:615-654
+int rb_normalize_dev(const void* img_dev, int dtype, long long nvoxels, double mean, double sigma, int remove_outliers,
+                     double outliers, double scale, double* out_dev, void* stream) {
+  if (!img_dev || !out_dev) return fail(RB_ERR_ARG, "normalize: null argument");
+  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (nvoxels < 1) return fail(RB_ERR_ARG, "normalize: %lld voxels", nvoxels);
+  return normalize_launch(img_dev, dtype, nvoxels, mean, sigma, remove_outliers != 0, outliers, scale, out_dev,
+                          (cudaStream_t)stream);
+}
+// resegmentMask's thresholding, radiomics/imageoperations.py:713-724
+int rb_resegment_dev(const void* img_dev, int dtype, const uint8_t* mask_dev, long long nvoxels, double lower,
+                     double upper, int nthresholds, uint8_t* out_dev, unsigned long long* counts_dev, void* stream) {
+  if (!img_dev || !mask_dev || !out_dev || !counts_dev) return fail(RB_ERR_ARG, "resegment: null argument");
+  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (nvoxels < 1) return fail(RB_ERR_ARG, "resegment: %lld voxels", nvoxels);
+  if (nthresholds != 1 && nthresholds != 2) return fail(RB_ERR_ARG, "resegment: %d thresholds (1 or 2)", nthresholds);
+  return resegment_launch(img_dev, dtype, mask_dev, nvoxels, lower, upper, nthresholds == 2, out_dev, counts_dev,
+                          (cudaStream_t)stream);
 }
 int rb_swt_axis_dev(const double* in_dev, int Z, int Y, int X, int axis, const double* dec_lo, const double* dec_hi,
                     int flen, double* out_lo_dev, double* out_hi_dev, void* stream) {

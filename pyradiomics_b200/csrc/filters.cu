@@ -7,6 +7,8 @@
 //     (reference radiomics/imageoperations.py:756-836 -> ITK LaplacianRecursiveGaussianImageFilter)
 //   * the square / squareroot / logarithm / exponential image types, one pass per voxel, and the gradient
 //     magnitude (reference radiomics/imageoperations.py:973-1091 -> ITK GradientMagnitudeImageFilter)
+//   * normalisation and resegmentation: a deterministic two-pass float64 ROI reduction, the normalisation pass and
+//     the threshold pass (reference radiomics/imageoperations.py:615-742)
 // All are HBM-streaming kernels: every thread handles consecutive x so loads/stores coalesce; the
 // wavelet pass reads its 6 taps through L1 (neighbouring threads share them).
 #include "common.cuh"
@@ -112,6 +114,143 @@ gradient_magnitude_kernel(const void* __restrict__ img, int dt, int Z, int Y, in
     out[i] = sqrt(__dadd_rn(__dadd_rn(__dadd_rn(0.0, __dmul_rn(gx, gx)), __dmul_rn(gy, gy)), __dmul_rn(gz, gz)));
     fm = f0;
     f0 = fp;
+  }
+}
+
+// ---- normalisation and resegmentation (reference radiomics/imageoperations.py:615-742).
+// roi_moments: count, NaN count, sum, max (pass 1) and sum of (x - mean)^2 (pass 2) of the image or of its mask != 0
+// voxels, in float64.  The grid is fixed (MOM_GRID blocks at most, fewer only for small images), every block writes its
+// partial to scratch and one block adds the partials up in index order, so the result is the same bit pattern on every
+// run and every card.  Pass 2 reads the mean from pass 1's result in device memory: the host does not wait in between.
+constexpr int MOM_THREADS = 256, MOM_GRID = 1024;
+static_assert(RB_MOMENTS_SCRATCH_BYTES >= MOM_GRID * (2 * sizeof(long long) + 3 * sizeof(double)), "moments scratch");
+
+struct MomAcc {
+  long long n, nnan;
+  double sum, max;
+};
+
+// np.max: a NaN anywhere makes the maximum NaN
+__device__ __forceinline__ double nan_max(double a, double b) { return (b > a || b != b) ? b : a; }
+
+__device__ __forceinline__ MomAcc mom_combine(MomAcc a, const MomAcc& b) {
+  a.n += b.n;
+  a.nnan += b.nnan;
+  a.sum = __dadd_rn(a.sum, b.sum);
+  a.max = nan_max(a.max, b.max);
+  return a;
+}
+
+// fixed-shape block reduction (shuffle tree per warp, then warp 0 over the warp results): the same order on every run
+__device__ MomAcc mom_block_reduce(MomAcc v) {
+  __shared__ MomAcc s_w[MOM_THREADS / 32];
+  for (int o = 16; o; o >>= 1) {
+    MomAcc u;
+    u.n = __shfl_down_sync(0xffffffffu, v.n, o);
+    u.nnan = __shfl_down_sync(0xffffffffu, v.nnan, o);
+    u.sum = __shfl_down_sync(0xffffffffu, v.sum, o);
+    u.max = __shfl_down_sync(0xffffffffu, v.max, o);
+    v = mom_combine(v, u);
+  }
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    v = threadIdx.x < MOM_THREADS / 32 ? s_w[threadIdx.x] : MomAcc{0, 0, 0.0, -1.0 / 0.0};
+    for (int o = 16; o; o >>= 1) {
+      MomAcc u;
+      u.n = __shfl_down_sync(0xffffffffu, v.n, o);
+      u.nnan = __shfl_down_sync(0xffffffffu, v.nnan, o);
+      u.sum = __shfl_down_sync(0xffffffffu, v.sum, o);
+      u.max = __shfl_down_sync(0xffffffffu, v.max, o);
+      v = mom_combine(v, u);
+    }
+  }
+  return v;                                               // valid in thread 0
+}
+
+// PASS 1: n, nnan, sum, max into part[blockIdx.x].  PASS 2: sum of (x - mean)^2 into part[blockIdx.x].sum, the mean
+// being res[2] / res[0] of pass 1.
+template <int PASS>
+__global__ void __launch_bounds__(MOM_THREADS)
+roi_moments_kernel(const void* __restrict__ img, int dt, const uint8_t* __restrict__ mask, long long n,
+                   const double* __restrict__ res, MomAcc* __restrict__ part) {
+  MomAcc a{0, 0, 0.0, -1.0 / 0.0};
+  const double mu = PASS == 2 ? __ddiv_rn(res[2], res[0]) : 0.0;
+  for (long long i = (long long)blockIdx.x * MOM_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * MOM_THREADS) {
+    if (mask && !mask[i]) continue;
+    const double x = load_any(img, dt, i);
+    if (PASS == 1) {
+      a.n++;
+      a.nnan += x != x;
+      a.sum = __dadd_rn(a.sum, x);
+      a.max = nan_max(a.max, x);
+    } else {
+      const double d = __dsub_rn(x, mu);
+      a.sum = __dadd_rn(a.sum, __dmul_rn(d, d));
+    }
+  }
+  a = mom_block_reduce(a);
+  if (threadIdx.x == 0) part[blockIdx.x] = a;
+}
+
+// one block: the `nparts` partials in index order -> res[0..3] (PASS 1: n, nnan, sum, max) or res[4] (PASS 2)
+template <int PASS>
+__global__ void __launch_bounds__(MOM_THREADS)
+roi_moments_final_kernel(const MomAcc* __restrict__ part, int nparts, double* __restrict__ res) {
+  MomAcc a{0, 0, 0.0, -1.0 / 0.0};
+  for (int k = threadIdx.x; k < nparts; k += MOM_THREADS) a = mom_combine(a, part[k]);
+  a = mom_block_reduce(a);
+  if (threadIdx.x != 0) return;
+  if (PASS == 1) {
+    res[0] = (double)a.n;
+    res[1] = (double)a.nnan;
+    res[2] = a.sum;
+    res[3] = a.max;
+  } else {
+    res[4] = a.sum;
+  }
+}
+
+// sitk.Normalize (ITK ShiftScale: shift -mean, then scale 1/sigma), the optional clamp to +-outliers and `*= scale`
+// (imageoperations.py:638-652).  Plain comparisons in the clamp keep NaN as NaN, like NumPy's masked assignment; every
+// step is rounded on its own (no FMA).
+__global__ void __launch_bounds__(256)
+normalize_kernel(const void* __restrict__ img, int dt, long long n, double mean, double inv_sigma, int clamp,
+                 double outliers, double scale, double* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    double v = __dmul_rn(__dsub_rn(load_any(img, dt, i), mean), inv_sigma);
+    if (clamp) {
+      if (v > outliers) v = outliers;
+      if (v < -outliers) v = -outliers;
+    }
+    out[i] = __dmul_rn(v, scale);
+  }
+}
+
+// resegmentMask's thresholds (imageoperations.py:713-722): out[i] = mask[i] && lo <= x (&& x <= hi when two).  The
+// thresholds arrive rounded to the dtype NumPy compares in, so the float64 comparison gives NumPy's answer.
+// counts[0] += ROI voxels, counts[1] += kept voxels (integer sums: the same whatever the order).
+__global__ void __launch_bounds__(256)
+resegment_kernel(const void* __restrict__ img, int dt, const uint8_t* __restrict__ mask, long long n, double lo,
+                 double hi, int two, uint8_t* __restrict__ out, unsigned long long* __restrict__ counts) {
+  unsigned long long roi = 0, kept = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    uint8_t k = 0;
+    if (mask[i]) {
+      const double x = load_any(img, dt, i);
+      k = x >= lo && (!two || x <= hi);
+      roi++;
+      kept += k;
+    }
+    out[i] = k;
+  }
+  for (int o = 16; o; o >>= 1) {
+    roi += __shfl_xor_sync(0xffffffffu, roi, o);
+    kept += __shfl_xor_sync(0xffffffffu, kept, o);
+  }
+  if ((threadIdx.x & 31) == 0 && roi) {
+    atomicAdd(&counts[0], roi);
+    atomicAdd(&counts[1], kept);
   }
 }
 
@@ -388,6 +527,35 @@ int gradient_magnitude_launch(const void* img, int dt, int Z, int Y, int X, cons
   if (columns > 0x7fffffffLL) return fail(RB_ERR_UNSUPPORTED, "gradient magnitude: %d x %d plane too large", Y, X);
   const dim3 grid((unsigned)columns, (unsigned)((Z + GRAD_ZCHUNK - 1) / GRAD_ZCHUNK));
   gradient_magnitude_kernel<<<grid, GRAD_TX, 0, st>>>(img, dt, Z, Y, X, w_zyx[0], w_zyx[1], w_zyx[2], out);
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+int roi_moments_launch(const void* img, int dt, const uint8_t* mask, long long n, int passes, void* scratch, double* res,
+                       cudaStream_t st) {
+  const long long need = (n + MOM_THREADS - 1) / MOM_THREADS;
+  const int grid = (int)(need < MOM_GRID ? need : MOM_GRID);      // depends on n only, never on the card
+  MomAcc* part = (MomAcc*)scratch;
+  roi_moments_kernel<1><<<grid, MOM_THREADS, 0, st>>>(img, dt, mask, n, res, part);
+  roi_moments_final_kernel<1><<<1, MOM_THREADS, 0, st>>>(part, grid, res);
+  if (passes == 2) {
+    roi_moments_kernel<2><<<grid, MOM_THREADS, 0, st>>>(img, dt, mask, n, res, part);
+    roi_moments_final_kernel<2><<<1, MOM_THREADS, 0, st>>>(part, grid, res);
+  } else {
+    RB_CUDA(cudaMemsetAsync(res + 4, 0xff, sizeof(double), st));   // NaN: no second pass
+  }
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+int normalize_launch(const void* img, int dt, long long n, double mean, double sigma, int clamp, double outliers,
+                     double scale, double* out, cudaStream_t st) {
+  normalize_kernel<<<grid_n(n, 256, 8), 256, 0, st>>>(img, dt, n, mean, 1.0 / sigma, clamp, outliers, scale, out);
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+int resegment_launch(const void* img, int dt, const uint8_t* mask, long long n, double lo, double hi, int two,
+                     uint8_t* out, unsigned long long* counts, cudaStream_t st) {
+  RB_CUDA(cudaMemsetAsync(counts, 0, 2 * sizeof(unsigned long long), st));
+  resegment_kernel<<<grid_n(n, 256, 8), 256, 0, st>>>(img, dt, mask, n, lo, hi, two, out, counts);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }

@@ -3,11 +3,14 @@
 :67-174), the level-1 stationary wavelet decomposition (getWaveletImage / _swt3, :839-970), the
 Laplacian-of-Gaussian filter (getLoGImage, :756-836), the per-voxel square / square root /
 logarithm / exponential images (getSquareImage ... getExponentialImage, :973-1073), the gradient
-magnitude (getGradientImage, :1076-1091) and the 3-D local binary pattern (getLBP3DImage,
-:1169-1314).  Same function names, arguments and yielded tuples as the reference so they can be
-dropped into ``radiomics.imageoperations``.
+magnitude (getGradientImage, :1076-1091), the 3-D local binary pattern (getLBP3DImage,
+:1169-1314), and the two preprocessing steps in front of them: image normalisation (normalizeImage,
+:615-654) and mask resegmentation (resegmentMask, :657-742).  Same function names, arguments and
+yielded tuples as the reference so they can be dropped into ``radiomics.imageoperations``.
 
-Parity status (DESIGN.md): binning, square and square root are bit-identical to NumPy, logarithm and
+Parity status (DESIGN.md): resegmentation masks equal the reference's (float32 sigma mode up to the
+few-ulp difference of a float64 ROI reduction); normalisation restates ITK's Normalize (unpinned
+details in DESIGN.md section 5); binning, square and square root are bit-identical to NumPy, logarithm and
 exponential within CUDA's 1-ulp log / exp; wavelet, LoG and gradient restate PyWavelets' and ITK's
 published algorithms -- neither library is available offline and the reference's own tests do not
 pin them (SURVEY.md section 8c) -> "parity unpinned" for those three.
@@ -628,6 +631,162 @@ def getGradientImage(inputImage, _inputMask, **kwargs):
     spacing = tuple(I.spacing_xyz(inputImage))[::-1] if kwargs.get("gradientUseSpacing", True) else None
     out = gradient_magnitude_device(_to_device(arr), spacing).cpu().numpy()
     yield I.like(inputImage, out), "gradient", kwargs
+
+
+# ------------------------------------------------------------------------------------ normalisation, resegmentation
+_MOMENTS_SCRATCH_BYTES = 40960                     # RB_MOMENTS_SCRATCH_BYTES
+RESEGMENT_MODES = ("absolute", "relative", "sigma")
+
+
+def _checked_source(x):
+    src = x.contiguous()
+    if src.dtype not in _TORCH_DT:
+        raise ValueError(f"unsupported pixel type {src.dtype}")
+    return src
+
+
+def _roi_moments(src, roi_u8, passes):
+    """rb_roi_moments_dev -> [n, n_nan, sum, max, sum of (x - mean)^2] on the host (one 40-byte copy)"""
+    scratch = torch.empty(_MOMENTS_SCRATCH_BYTES, dtype=torch.uint8, device=src.device)
+    res = torch.empty(5, dtype=torch.float64, device=src.device)
+    check(lib().rb_roi_moments_dev(_ptr(src), _TORCH_DT[src.dtype], _ptr(roi_u8), C.c_longlong(src.numel()), passes,
+                                   _ptr(scratch), _ptr(res), _stream()), "roi moments")
+    return res.cpu().tolist()
+
+
+def _moments_of_roi(src, roi_u8, ddof):
+    n, n_nan, s, mx, ssd = _roi_moments(src, roi_u8, 2)
+    n, n_nan = int(n), int(n_nan)
+    mean = s / n if n else math.nan
+    std = math.sqrt(ssd / (n - ddof)) if n > ddof else math.nan
+    return n, n_nan, mean, std, (mx if n else math.nan)
+
+
+def roi_moments_device(img_t: torch.Tensor, mask_t: torch.Tensor | None = None, label=1, ddof=0):
+    """(n, n_nan, mean, std, max) of the CUDA tensor's voxels with mask_t == label (mask_t None = every voxel), reduced
+    in float64 in a fixed order (rb_roi_moments_dev: the same bits on every run): mean = sum / n, std =
+    sqrt(sum((x - mean)^2) / (n - ddof)), max NaN when any voxel is NaN (np.max).  An empty ROI gives NaN statistics."""
+    roi = None if mask_t is None else (mask_t == label).to(torch.uint8).contiguous()
+    return _moments_of_roi(_checked_source(img_t), roi, ddof)
+
+
+def normalize_image_device(x: torch.Tensor, scale=1, outliers=None, stats=None):
+    """normalizeImage on a CUDA tensor -> float64 CUDA tensor: ((x - mean) * (1 / std)), clamped to [-outliers,
+    outliers] unless `outliers` is None, times `scale` (rb_normalize_dev).  mean and std (N - 1) are those of the WHOLE
+    image, as sitk.Normalize takes them; `stats` = (mean, std) supplies them, for a caller that holds only a crop."""
+    src = _checked_source(x)
+    if stats is None:
+        _, _, mean, std, _ = roi_moments_device(src, ddof=1)
+    else:
+        mean, std = (float(v) for v in stats)
+    out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
+    check(lib().rb_normalize_dev(_ptr(src), _TORCH_DT[src.dtype], C.c_longlong(src.numel()), C.c_double(mean),
+                                 C.c_double(std), int(outliers is not None),
+                                 C.c_double(float(outliers) if outliers is not None else 0.0), C.c_double(float(scale)),
+                                 _ptr(out), _stream()), "normalize")
+    return out
+
+
+def _comparison_value(np_type, t):
+    """the float64 that compares with an np_type voxel (exactly converted to float64) as NumPy compares the voxel with
+    `t`: in np.result_type(np_type, t), where a Python scalar is weak (NEP 50).  A float32 image and a Python float
+    compare in float32, so the threshold is rounded to float32 first.  A Python int against an integer image compares
+    exactly, even out of the dtype's range."""
+    if isinstance(t, int) and np.issubdtype(np_type, np.integer):
+        return float(t)
+    return float(np.result_type(np_type, t).type(t))
+
+
+def resegment_thresholds(np_type, resegmentRange, resegmentMode, max_gl=None, mean_gl=None, sd_gl=None):
+    """the reference's thresholds (imageoperations.py:695-711) from the ROI's np.max (`max_gl`, an np_type scalar) or
+    np.mean / np.std (`mean_gl` / `sd_gl`: float32 scalars for a float32 image, float64 otherwise), with the reference's
+    own expressions so that they have its dtype and value -> (thresholds, the float64 values rb_resegment_dev compares
+    with)."""
+    if resegmentMode == "absolute":
+        thresholds = sorted(resegmentRange)
+    elif resegmentMode == "relative":
+        thresholds = [max_gl * th for th in sorted(resegmentRange)]
+    elif resegmentMode == "sigma":
+        thresholds = [mean_gl + sd_gl * th for th in sorted(resegmentRange)]
+    else:
+        raise ValueError(f"Resegment mode {resegmentMode} not recognized.")
+    return thresholds, [_comparison_value(np_type, t) for t in thresholds]
+
+
+def _stat_type(np_type):
+    """the type np.mean / np.std of an np_type array return"""
+    return np.float32 if np_type == np.float32 else np.float64
+
+
+def resegment_mask_device(img_t: torch.Tensor, mask_t: torch.Tensor, resegmentRange, resegmentMode="absolute", label=1):
+    """resegmentMask on CUDA tensors -> (uint8 CUDA mask: 1 where mask_t == label and the voxel lies within the
+    thresholds, kept voxel count, thresholds as the reference computes them).  The ROI statistics come from one
+    rb_roi_moments_dev (relative mode: one pass for the maximum; sigma mode: two passes) and are rounded to the type
+    NumPy's reductions return; the thresholding is rb_resegment_dev.  Raises the reference's ValueErrors, including
+    when at most one voxel is kept."""
+    if resegmentRange is None:
+        raise ValueError("resegmentRange is None.")
+    if len(resegmentRange) == 0 or len(resegmentRange) > 2:
+        raise ValueError(f"Length {len(resegmentRange)} is not allowed for resegmentRange")
+    logger.debug(f"Resegmenting mask (range {resegmentRange}, mode {resegmentMode})")
+    src = _checked_source(img_t)
+    np_type = _NP_OF_TORCH[src.dtype]
+    roi = (mask_t == label).to(torch.uint8).contiguous()
+    if roi.shape != src.shape:
+        raise ValueError(f"mask shape {tuple(roi.shape)} differs from image shape {tuple(src.shape)}")
+    stats = {}
+    if resegmentMode == "absolute":
+        logger.debug("Resegmenting in absolute mode")
+    elif resegmentMode == "relative":
+        n, _, _, mx, _ = _roi_moments(src, roi, 1)
+        if n == 0:                                              # np.max of an empty array
+            raise ValueError("zero-size array to reduction operation maximum which has no identity")
+        stats["max_gl"] = np_type(mx)
+        logger.debug(f"Resegmenting in relative mode, max {stats['max_gl']}")
+    elif resegmentMode == "sigma":
+        _, _, mean, std, _ = _moments_of_roi(src, roi, 0)
+        st = _stat_type(np_type)
+        stats["mean_gl"], stats["sd_gl"] = st(mean), st(std)
+        logger.debug(f"Resegmenting in sigma mode, mean {stats['mean_gl']}, std {stats['sd_gl']}")
+    thresholds, cmp = resegment_thresholds(np_type, resegmentRange, resegmentMode, **stats)
+    logger.debug(f"Applying lower threshold ({thresholds[0]})")
+    if len(thresholds) == 2:
+        logger.debug(f"Applying upper threshold ({thresholds[1]})")
+    out = torch.empty(src.shape, dtype=torch.uint8, device=src.device)
+    counts = torch.empty(2, dtype=torch.int64, device=src.device)
+    check(lib().rb_resegment_dev(_ptr(src), _TORCH_DT[src.dtype], _ptr(roi), C.c_longlong(src.numel()),
+                                 C.c_double(cmp[0]), C.c_double(cmp[-1]), len(cmp), _ptr(out), _ptr(counts), _stream()),
+          "resegment")
+    oldSize, roiSize = counts.cpu().tolist()
+    if roiSize <= 1:
+        raise ValueError(f"Resegmentation excluded too many voxels with label {label} "
+                         f"(retained {roiSize} voxel(s))! Cannot extract features")
+    logger.debug(f"Resegmentation complete, new size: {roiSize} voxels (excluded {oldSize - roiSize} voxels)")
+    return out, roiSize, thresholds
+
+
+def normalizeImage(image, **kwargs):
+    """reference function (imageoperations.py:615-654): (x - mean) / std over the WHOLE image (std with N - 1), outliers
+    beyond +-removeOutliers clamped, times normalizeScale; float64 image of the input's geometry."""
+    scale = kwargs.get("normalizeScale", 1)
+    outliers = kwargs.get("removeOutliers")
+    logger.debug(f"Normalizing image with scale {scale}")
+    if outliers is not None:
+        logger.debug(f"Removing outliers > {outliers} standard deviations")
+    out = normalize_image_device(_to_device(I.as_array(image)), scale, outliers).cpu().numpy()
+    return I.like(image, out)
+
+
+def resegmentMask(imageNode, maskNode, **kwargs):
+    """reference function (imageoperations.py:657-742): the mask == label voxels within resegmentRange (mode absolute,
+    relative to the ROI maximum, or sigma around the ROI mean) -> int64 mask holding `label`, of the mask's geometry."""
+    resegmentRange = kwargs["resegmentRange"]
+    resegmentMode = kwargs.get("resegmentMode", "absolute")
+    label = kwargs.get("label", 1)
+    out, _, _ = resegment_mask_device(_to_device(I.as_array(imageNode)), _to_device(I.as_array(maskNode)), resegmentRange,
+                                      resegmentMode, label)
+    newMask_arr = out.cpu().numpy().astype(np.int64) * label
+    return I.like(maskNode, newMask_arr)
 
 
 # ------------------------------------------------------------------------------------ LBP 3-D

@@ -63,13 +63,22 @@ def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1"
 
 def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CLASSES, spacing_zyx=(1.0, 1.0, 1.0),
                              wavelet="coif1", sigmas=(1.0, 2.0, 3.0), consume=None, lbp3d=None, image_types=(),
-                             gradient_use_spacing=True, **kw):
+                             gradient_use_spacing=True, normalize=None, resegment=None, **kw):
     """image: CUDA tensor (Z,Y,X) of raw intensities, mask: CUDA uint8/bool.  For every derived
     image (`image_types`, `gradient_use_spacing`, `lbp3d`: see derived_images): bin (binWidth/binCount in kw) -> pack ->
     fused kernels.
+    `normalize` (a dict with normalizeScale, removeOutliers; {} = the defaults) normalises the whole image first and every
+    derived image comes from the normalised one; `resegment` (a dict with resegmentRange, resegmentMode) then resegments
+    the mask against that image, and binning, the texture kernels and the LBP 3-D ROI use the resegmented mask -- the
+    reference's order (featureextractor.py:316-392).  None (default) skips either step.
     `consume(name, cls, maps)` is called with each float64 [F,Z,Y,X] result (maps are reused buffers unless consume keeps
     them); returns the list of (image name, Ng, number of levels)."""
+    if normalize is not None:
+        image = IO.normalize_image_device(image, normalize.get("normalizeScale", 1), normalize.get("removeOutliers"))
     msk = (mask != 0).to(torch.uint8).contiguous()
+    if resegment is not None:
+        msk, _, _ = IO.resegment_mask_device(image, msk, resegment["resegmentRange"],
+                                             resegment.get("resegmentMode", "absolute"))
     outs = {}
     info = []
     for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=msk, image_types=image_types,

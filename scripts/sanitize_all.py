@@ -1,7 +1,7 @@
 """compute-sanitizer target: ONE small invocation of every kernel family of the library (fused voxel fast
 paths, the generic voxel kernel, the cMatrices builders in segment and voxel-batch mode, discretisation,
 wavelet, LoG, shape, first-order, 3-D LBP, the square / squareroot / logarithm / exponential / gradient
-image types).  Run as
+image types, normalisation and resegmentation).  Run as
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python scripts/sanitize_all.py [N] [family ...]
 The families are independent so a slow tool can be pointed at one of them."""
 import os
@@ -16,7 +16,7 @@ from pyradiomics_b200 import _lib, cmatrices, cshape, featureclasses as FC, imag
 args = [a for a in sys.argv[1:]]
 N = int(args.pop(0)) if args and args[0].isdigit() else 20
 N16 = N - N % 16 if N >= 16 else N
-fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d", "imagetypes"]
+fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d", "imagetypes", "preprocess"]
 rng = np.random.default_rng(0)
 
 
@@ -121,4 +121,15 @@ if "imagetypes" in fams:
             names += [n for _, n, _ in gen(I.ArrayImage(img, (0.7, 1.1, 2.0)[:img.ndim]), None)]
     torch.cuda.synchronize()
     print("imagetypes ok", names[:5], flush=True)
+if "preprocess" in fams:
+    raw = ((vols["smooth"] - 1) * 25 - 300).astype(np.int16)
+    kept = []
+    for img in (raw, raw.astype(np.float32) / 7):
+        nimg = IO.normalizeImage(I.ArrayImage(img), normalizeScale=100, removeOutliers=3)
+        for rng_, mode in (([-300], "absolute"), ([0.2, 0.8], "relative"), ([-2, 2], "sigma")):
+            out = IO.resegmentMask(nimg if mode == "sigma" else I.ArrayImage(img), I.ArrayImage(mask_rag.astype(np.uint8)),
+                                   resegmentRange=rng_, resegmentMode=mode)
+            kept.append(int((I.as_array(out) != 0).sum()))
+    torch.cuda.synchronize()
+    print("preprocess ok", kept, flush=True)
 print("sanitize_all done")
