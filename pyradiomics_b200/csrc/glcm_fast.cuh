@@ -372,25 +372,42 @@ struct GlcmAcc {
   bool ja_nan;
 };
 
+#ifdef __CUDA_ARCH__
+#define RB_VMINU2(a, b) __vminu2((a), (b))
+#define RB_VMAXU2(a, b) __vmaxu2((a), (b))
+#else
+static inline uint32_t rb_vminu2(uint32_t a, uint32_t b) {
+  return min(a >> 16, b >> 16) << 16 | min(a & 0xFFFFu, b & 0xFFFFu);
+}
+static inline uint32_t rb_vmaxu2(uint32_t a, uint32_t b) {
+  return max(a >> 16, b >> 16) << 16 | max(a & 0xFFFFu, b & 0xFFFFu);
+}
+#define RB_VMINU2(a, b) rb_vminu2((a), (b))
+#define RB_VMAXU2(a, b) rb_vmaxu2((a), (b))
+#endif
+
 // one angle (slot s) of one voxel.  w: the 27 window levels (stride ws), eq: equality masks.
-template <int NP>
+// FULL: every window level is non-zero (all 27 voxels inside the volume and the ROI), so every pair is valid and
+// n = NP: the validity logic drops out and the denominators are compile-time constants.
+template <int NP, bool FULL>
 RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
                            const GlcmFastTables& T, int s, const VoxParams& P, GlcmAcc& acc) {
   const uint8_t* pA = T.pA[s];
   const uint8_t* pB = T.pB[s];
-  // key1 = (a+b) << 8 | |a-b| identifies the unordered level pair; key2 = |a-b|.  Invalid pairs
-  // (an end outside the mask / volume) get distinct large keys and sort behind the n valid ones.
-  int key1[NP], key2[NP];
+  const int dsh = (int)pB[0] - (int)pA[0];   // every pair of the angle is (p, p + dsh)
+  // key = (a+b) << 16 | |a-b|: one sorting network orders both 16-bit lanes independently (p_{x+y} and p_{x-y}
+  // bins are runs in each lane).  An invalid pair (an end outside the mask / volume) gets 0xFFFF in both lanes and
+  // sorts behind the n valid ones.
+  uint32_t key[NP];
   uint32_t valid = 0, EA = 0, EB = 0;
   int n = 0, Ssum = 0, Sab = 0, Sq = 0, Skd = 0;
   bool selfpair = false;               // a level paired with itself: the level graph has a self-loop
 #pragma unroll
   for (int t = 0; t < NP; t++) {
     const int a = w[pA[t] * ws], b = w[pB[t] * ws];
-    const bool ok = a != 0 && b != 0;
+    const bool ok = FULL || (a != 0 && b != 0);
     const int kd = a > b ? a - b : b - a, ks = a + b;
-    key1[t] = ok ? (ks << 8 | kd) : (0x100000 + t);
-    key2[t] = ok ? kd : (0x1000 + t);
+    key[t] = ok ? (uint32_t)(ks << 16 | kd) : 0xFFFFFFFFu;
     if (ok) {
       valid |= 1u << t; EA |= 1u << pA[t]; EB |= 1u << pB[t];
       n++; Ssum += ks; Sab += a * b; Sq += a * a + b * b; Skd += kd;
@@ -398,7 +415,7 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
     }
   }
   const int orig = T.orig[s];
-  if (n == 0) {
+  if (!FULL && n == 0) {
     if (P.alive[orig >> 5] >> (orig & 31) & 1u) acc.ja_nan = true;
     return;
   }
@@ -407,7 +424,12 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
   // sum_levels R log2 R = sum over the 2n pair ends of log2 R(their level).
   // (Straight-line per-pair code on purpose: a loop over the classes with its shared-memory load in the carried
   // dependence is slower -- 8 to 16 warps per SM cannot hide a 30-cycle chain per class.)
-  double rl = 0;
+  // Merged matrix entries: the pairs equal to pair t = (p, q) as an unordered level pair are the valid pairs
+  // (p', p' + dsh) with levels (L(p), L(q)) or (L(q), L(p)); c counts them (pair t included).  Summed over those c pairs,
+  // log2 cc gives c log2 cc (cc = the entry's count) and 2 cc gives the squared count of the entry (plus its mirror's off
+  // the diagonal).
+  double rl = 0, lgE = 0;
+  int E2 = 0, cmax = 0;
   uint32_t reps = 0, all = 0, comp = 0;
   uint32_t em[NP];
 #pragma unroll
@@ -420,6 +442,11 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
       em[t] = ea | eb;
       all |= em[t];
       if (!comp) comp = em[t];
+      const int c = RB_POPC(((ea & (eb >> dsh)) | (eb & (ea >> dsh))) & EA);
+      const int cc = ea == eb ? 2 * c : c;                  // count of the matrix entry (a pair (i, i) adds 2)
+      lgE += T.log2t[cc];
+      E2 += 2 * cc;
+      cmax = cc > cmax ? cc : cmax;
     }
   }
   const int nlev = RB_POPC(reps);
@@ -441,7 +468,7 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
       // 2-colouring by a breadth-first sweep over class masks (<= 2 nlev closure steps; round 1 swept the pair list
       // instead -- 18 % of this kernel's instructions -- and had moved the test into the solver thread for that reason)
       bool connected;
-      glcm_graph_scan(eq, es, EA, (int)pB[0] - (int)pA[0], EA | EB, false, &connected, &bipartite, true);
+      glcm_graph_scan(eq, es, EA, dsh, EA | EB, false, &connected, &bipartite, true);
     }
     if (comp != all || bipartite) mcc = 1.0;
     else {
@@ -450,9 +477,9 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
       acc.tcls |= (unsigned long long)glcm_task_class(nlev) << (GF_CLS_BITS * s);
     }
   }
-  if (NP == 18) { RB_SORTNET_18(key1); RB_SORTNET_18(key2); }
-  else if (NP == 12) { RB_SORTNET_12(key1); RB_SORTNET_12(key2); }
-  else { RB_SORTNET_8(key1); RB_SORTNET_8(key2); }
+  if (NP == 18) RB_SORTNET2x16_18(key);
+  else if (NP == 12) RB_SORTNET2x16_12(key);
+  else RB_SORTNET2x16_8(key);
   // S = 2n entries' worth of counts.  Every moment below is an exact integer numerator over a
   // power of S (no cancellation between rounded quantities).
   const int S2 = 2 * n;
@@ -466,43 +493,32 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
   const double ct = (double)(2 * (Sq + 2 * Sab) * S2 - 4 * Ssum * Ssum) * invS2;
   const double da = 2.0 * Skd * invS;
   const double dvar = (double)(2 * (Sq - 2 * Sab) * S2 - 4 * Skd * Skd) * invS2;
-  // scan the sorted keys: runs of equal key1 = merged matrix entries (length nn), runs of equal
-  // a+b = p_{x+y} bins, runs of equal key2 = p_{x-y} bins (the |i-j| table features are taken per run)
-  double cs = 0, cp = 0, idm = 0, idmn = 0, id = 0, idn = 0, inv = 0, lgE = 0, lgD = 0, lgS = 0;
+  // scan the sorted lanes: runs of equal a+b (high lane) = p_{x+y} bins, runs of equal |a-b| (low lane) = p_{x-y}
+  // bins (the |i-j| table features are taken per run)
+  double cs = 0, cp = 0, idm = 0, idmn = 0, id = 0, idn = 0, inv = 0, lgD = 0, lgS = 0;
   // a run's length is its end minus its start index.  (The same sums written with three counters incremented per element
   // and reset at run ends gave wrong DifferenceEntropy and SumEntropy maps on an H100 when built for sm_90a with
   // -Xptxas -O2 or -O3 -- tests/test_voxel_gpu.py::test_glcm_fast_path_equals_generic_kernel failed -- and the right ones
   // with -Xptxas -O1.)
-  int E2 = 0, cmax = 0, startK = 0, startS = 0, startD = 0;
+  int startS = 0, startD = 0;
 #pragma unroll
   for (int i = 0; i < NP; i++) {
-    if (i < n) {
-      const int k1 = key1[i], ks = k1 >> 8, kd = k1 & 255, k2 = key2[i];
+    if (FULL || i < n) {
+      const int ks = (int)(key[i] >> 16), kd = (int)(key[i] & 0xFFFFu);
       const double dn = (double)(ks * n - Ssum), d2 = dn * dn;   // (i+j-ux-uy) * n, an integer
       cs += d2 * dn; cp += d2 * d2;
-      const int nx1 = (i + 1 < NP) ? key1[i + 1 < NP ? i + 1 : i] : -1;
-      const int nx2 = (i + 1 < NP) ? key2[i + 1 < NP ? i + 1 : i] : -1;
+      const uint32_t nx = (i + 1 < NP) ? key[i + 1 < NP ? i + 1 : i] : 0xFFFFFFFFu;
       const bool last = (i + 1 == n);
-      if (last || nx1 != k1) {                 // end of a merged-entry run
-        const int runK = i + 1 - startK;
-        const int c = kd ? runK : 2 * runK;    // count of the matrix entry (both orders when i != j)
-        E2 += kd ? 2 * runK * runK : 4 * runK * runK;
-        if (c > cmax) cmax = c;
-        lgE += runK * T.log2t[c];
-        startK = i + 1;
-      }
-      if (last || (nx1 >> 8) != ks) {
-        const int runS = i + 1 - startS;
-        lgS += runS * T.log2t[2 * runS];
-        startS = i + 1;
-      }
-      if (last || nx2 != k2) {                 // end of a |i-j| bin
-        const int runD = i + 1 - startD;
-        const double r = (double)runD;
-        lgD += r * T.log2t[2 * runD];
-        idm += r * T.idm[k2]; idmn += r * T.idmn[k2]; id += r * T.id[k2]; idn += r * T.idn[k2]; inv += r * T.inv[k2];
-        startD = i + 1;
-      }
+      // every element adds its bins' terms, with run length 0 unless a bin ends here (log2t[0] = 0: the sums are
+      // unchanged): no branch per element, so the lanes of a warp stay converged whatever their bin structure
+      const int runS = (last || (int)(nx >> 16) != ks) ? i + 1 - startS : 0;         // a+b bin
+      const int runD = (last || (int)(nx & 0xFFFFu) != kd) ? i + 1 - startD : 0;     // |i-j| bin
+      lgS += runS * T.log2t[2 * runS];
+      const double r = (double)runD;
+      lgD += r * T.log2t[2 * runD];
+      idm += r * T.idm[kd]; idmn += r * T.idmn[kd]; id += r * T.id[kd]; idn += r * T.idn[kd]; inv += r * T.inv[kd];
+      startS = runS ? i + 1 : startS;
+      startD = runD ? i + 1 : startD;
     }
   }
   const double invn = 1.0 / n, invn2 = invn * invn;
@@ -539,25 +555,29 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
 // Phase A of one voxel: everything except the MCC eigen-solves.  w: the 27 window levels (0 =
 // unmasked / outside); eq: scratch for 27 equality masks, element stride es (shared memory on the
 // device).  Writes the 24 means (MCC without the pending tasks) and returns the task bitmask.
+// FULL = true only for a window without a zero level (glcm_window_full).
+template <bool FULL = false>
 RB_HD uint32_t glcm_fast_voxel_phaseA(const uint8_t* w, int ws, uint32_t* eq, int es, const GlcmFastTables& T,
                                       const VoxParams& P, double* out, int* n_ok_out, unsigned long long* tcls_out = nullptr) {
   uint32_t e[27];
   int wl[27];
 #pragma unroll
   for (int p = 0; p < 27; p++) wl[p] = w[p * ws];
-  RB_EQMASKS_27(wl, e);
+  if (FULL) RB_EQMASKS_27_KEY(wl, e);
+  else RB_EQMASKS_27(wl, e);
 #pragma unroll
   for (int p = 0; p < 27; p++) eq[p * es] = e[p];
   GlcmAcc acc;
 #pragma unroll
   for (int k = 0; k < GLCM_NF; k++) acc.sum[k] = 0;
   acc.n_ok = 0; acc.n_imc2 = 0; acc.ja_nan = false; acc.tasks = 0; acc.tcls = 0;
-  // RB_ANGLE_SYNC: on the device the block re-converges before every angle so that its warps walk
-  // the (large, fully unrolled) angle bodies together and share instruction-cache lines -- without
-  // it the kernel is instruction-fetch bound.
-  for (int s = 0; s < 3; s++) { RB_ANGLE_SYNC(); glcm_fast_angle<18>(w, ws, eq, es, T, s, P, acc); }
-  for (int s = 3; s < 9; s++) { RB_ANGLE_SYNC(); glcm_fast_angle<12>(w, ws, eq, es, T, s, P, acc); }
-  for (int s = 9; s < 13; s++) { RB_ANGLE_SYNC(); glcm_fast_angle<8>(w, ws, eq, es, T, s, P, acc); }
+  // RB_ANGLE_SYNC: on the device the block re-converges before every angle of the general body so that its warps walk
+  // the (large, fully unrolled) angle bodies together and share instruction-cache lines -- without it that body is
+  // instruction-fetch bound.  The full-window body runs faster without the barriers (its warps stay in step on their
+  // own: no data-dependent pair validity).
+  for (int s = 0; s < 3; s++) { if (!FULL) RB_ANGLE_SYNC(); glcm_fast_angle<18, FULL>(w, ws, eq, es, T, s, P, acc); }
+  for (int s = 3; s < 9; s++) { if (!FULL) RB_ANGLE_SYNC(); glcm_fast_angle<12, FULL>(w, ws, eq, es, T, s, P, acc); }
+  for (int s = 9; s < 13; s++) { if (!FULL) RB_ANGLE_SYNC(); glcm_fast_angle<8, FULL>(w, ws, eq, es, T, s, P, acc); }
   *n_ok_out = acc.n_ok;
   if (tcls_out) *tcls_out = acc.tcls;
   const double inv = acc.n_ok ? 1.0 / acc.n_ok : NAN;
@@ -575,12 +595,22 @@ RB_HD double glcm_fast_finish_mcc(double partial_mean, int n_ok, uint32_t tasks,
   return n_ok ? partial_mean + add / n_ok : partial_mean;
 }
 
+// all 27 window levels non-zero: phase A may take its full-window body.  (The choice depends on the window alone, so
+// a voxel takes the same body whichever slab or chunk it is computed in.)
+RB_HD bool glcm_window_full(const uint8_t* w, int ws) {
+  bool full = true;
+#pragma unroll
+  for (int p = 0; p < 27; p++) full &= w[p * ws] != 0;
+  return full;
+}
+
 // single-thread composition (host emulation / reference for the two-phase kernel)
 RB_HD void glcm_fast_voxel(const uint8_t* w, int ws, uint32_t* eq, int es, const GlcmFastTables& T,
                            const VoxParams& P, double* out) {
   int n_ok = 0;
   unsigned long long tcls = 0;
-  const uint32_t tasks = glcm_fast_voxel_phaseA(w, ws, eq, es, T, P, out, &n_ok, &tcls);
+  const uint32_t tasks = glcm_window_full(w, ws) ? glcm_fast_voxel_phaseA<true>(w, ws, eq, es, T, P, out, &n_ok, &tcls)
+                                                 : glcm_fast_voxel_phaseA<false>(w, ws, eq, es, T, P, out, &n_ok, &tcls);
   double solved[GF_NA];
   GlcmSolveTables ST;
   glcm_solve_tables_from(T, ST);

@@ -15,7 +15,7 @@ namespace rb {
 // Two kernels per chunk of planes:
 //   A  one thread per centre voxel: window -> equality masks -> all 13 angles, every feature except
 //      the MCC eigen-solves; a voxel that needs k solves reserves k CONSECUTIVE 16-byte queue entries
-//      (voxel, angle slot, n_ok).  No local memory, no block barriers.
+//      (voxel, angle slot, n_ok).
 //   B  one thread per queue entry (= one eigen-task): reloads the voxel's 27 levels and runs the dense register
 //      solve (<= 12 levels) or the register-resident Lanczos recurrence (13..18 levels); result to res[k].
 //   C  one thread per voxel-with-tasks adds its results in slot order to the voxel's MCC (single
@@ -207,6 +207,71 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
 }
 
 // ---- phase A (one thread per centre voxel) and phase C (finish) ---------------------------------
+struct PhaseAVoxel { long long vi, oi; bool center, full; };
+
+// voxel t of the chunk: its 27 window levels to w (stride NT; zeros outside the volume, all zeros if it is not a
+// centre) and whether the window is full (a centre whose 27 levels are all non-zero, see glcm_window_full)
+template <int NT>
+__device__ __forceinline__ PhaseAVoxel glcm_phaseA_load(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
+                                                        const VoxParams& P, int z0, int out_z0, long long t, bool live,
+                                                        uint8_t* w) {
+  const long long plane = (long long)P.Y * P.X;
+  const int z = z0 + (int)((live ? t : 0) / plane);
+  const int rem = (int)((live ? t : 0) % plane);
+  const int y = rem / P.X, x = rem % P.X;
+  PhaseAVoxel v;
+  v.vi = (long long)z * P.sz + (long long)y * P.sy + x;
+  v.oi = (long long)(z - out_z0) * plane + rem;
+  v.center = live && (centers ? centers[(long long)z * plane + rem] != 0 : lev[v.vi] != 0);
+  bool full = v.center;
+#pragma unroll
+  for (int dz = -1; dz <= 1; dz++)
+#pragma unroll
+    for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+      for (int dx = -1; dx <= 1; dx++) {
+        const int zz = z + dz, yy = y + dy, xx = x + dx;
+        const bool in = v.center && zz >= 0 && zz < P.Z && yy >= 0 && yy < P.Y && xx >= 0 && xx < P.X;
+        const uint8_t l = in ? lev[v.vi + (long long)dz * P.sz + (long long)dy * P.sy + dx] : (uint8_t)0;
+        full &= l != 0;
+        w[((dz + 1) * 9 + (dy + 1) * 3 + (dx + 1)) * NT] = l;
+      }
+  v.full = full;
+  return v;
+}
+
+// phase A of one centre voxel; store: write its 24 maps and queue its eigen-tasks (the general body holds barriers, so
+// every thread of the block runs it, idle ones with store = false)
+template <bool FULL, int NT>
+__device__ __forceinline__ void glcm_phaseA_voxel(const uint8_t* w, uint32_t* eq, const GlcmFastTables& T, const VoxParams& P,
+                                                  const PhaseAVoxel& v, bool store, double* __restrict__ out, long long fstride,
+                                                  GlcmTask* __restrict__ queue, unsigned* __restrict__ qcount) {
+  double f[GLCM_NF];
+  int n_ok = 0;
+  unsigned long long tcls = 0;
+  const uint32_t tasks = glcm_fast_voxel_phaseA<FULL>(w, NT, eq, NT, T, P, f, &n_ok, &tcls);
+  if (!store) return;
+#pragma unroll
+  for (int k = 0; k < GLCM_NF; k++) out[k * fstride + v.oi] = f[k];
+  if (tasks) {
+    const int k = __popc(tasks);
+    unsigned q = atomicAdd(qcount, (unsigned)k);
+    bool first = true;
+    for (uint32_t m = tasks; m; m &= m - 1, q++) {
+      GlcmTask e;
+      e.vi = v.vi; e.slot = (uint8_t)(__ffs((int)m) - 1); e.n_ok = (uint8_t)n_ok; e.count = first ? (uint8_t)k : 0;
+      e.cls = (uint8_t)(tcls >> (GF_CLS_BITS * e.slot) & (GF_NCLS - 1)); e.unused = 0.f;
+      queue[q] = e;
+      first = false;
+    }
+  }
+}
+
+// Block-uniform tiles of NT voxels: a centre with a full window runs the full-window body (no validity logic, constant
+// denominators, no barriers), a voxel that is not a centre stores init_value, and a centre whose window is not full (the
+// volume's faces, the ROI's border and holes) goes to the block's list.  The block runs the general body over that
+// list, NT at a time, whenever NT are waiting and once at the end.  (List entries are chunk indices: a chunk of 2^32
+// voxels would need a 1.3 TB eigen-task queue, which glcm_fast_launch fails to allocate first.)
 template <int MINB, int NT>
 __global__ void __launch_bounds__(NT, MINB)
 glcm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
@@ -214,6 +279,8 @@ glcm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ ce
                  double* __restrict__ out, long long fstride, int z0, int z1, int out_z0,
                  GlcmTask* __restrict__ queue, unsigned* __restrict__ qcount) {
   __shared__ GlcmFastTables T;
+  __shared__ unsigned defer[2 * NT];                                // chunk indices of the voxels left to the general body
+  __shared__ unsigned ndefer;
   RB_DYN_SHARED(uint32_t, eqbuf);                                   // [27][NT] equality masks, then [27][NT] window bytes
   uint8_t* const wbuf = reinterpret_cast<uint8_t*>(eqbuf + 27 * NT);
   {
@@ -221,58 +288,42 @@ glcm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ ce
     uint32_t* dst = reinterpret_cast<uint32_t*>(&T);
     for (int i = threadIdx.x; i < (int)(sizeof(GlcmFastTables) / 4); i += NT) dst[i] = src[i];
   }
-  __syncthreads();
   const int tid = threadIdx.x;
-  const long long plane = (long long)P.Y * P.X;
-  const long long total = (long long)(z1 - z0) * plane;
+  if (tid == 0) ndefer = 0;
+  __syncthreads();
+  const long long total = (long long)(z1 - z0) * P.Y * P.X;
   const long long ntiles = (total + NT - 1) / NT;
-  // block-uniform tile loop: every thread runs phase A (on an all-zero window when its voxel is
-  // not a centre / past the end) so the per-angle barriers inside are reached by the whole block
-  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const long long t = tile * NT + tid;
-    const bool live = t < total;
-    const int z = z0 + (int)((live ? t : 0) / plane);
-    const int rem = (int)((live ? t : 0) % plane);
-    const int y = rem / P.X, x = rem % P.X;
-    const long long vi = (long long)z * P.sz + (long long)y * P.sy + x;
-    const long long oi = (long long)(z - out_z0) * plane + rem;
-    const bool is_center = live && (centers ? centers[(long long)z * plane + rem] != 0 : lev[vi] != 0);
-    uint8_t* w = &wbuf[tid];
+  uint8_t* const w = &wbuf[tid];
+  uint32_t* const eq = &eqbuf[tid];
+  // one pass per tile and a last pass with no tile (one call site per body: each is thousands of instructions)
+  for (long long tile = blockIdx.x;; tile += gridDim.x) {
+    const bool more = tile < ntiles;                                 // block-uniform
+    if (more) {
+      const long long t = tile * NT + tid;
+      const bool live = t < total;
+      const PhaseAVoxel v = glcm_phaseA_load<NT>(lev, centers, P, z0, out_z0, t, live, w);
+      if (v.full) {
+        glcm_phaseA_voxel<true, NT>(w, eq, T, P, v, true, out, fstride, queue, qcount);
+      } else if (v.center) {
+        defer[atomicAdd(&ndefer, 1u)] = (unsigned)t;
+      } else if (live) {
 #pragma unroll
-    for (int dz = -1; dz <= 1; dz++)
-#pragma unroll
-      for (int dy = -1; dy <= 1; dy++)
-#pragma unroll
-        for (int dx = -1; dx <= 1; dx++) {
-          const int zz = z + dz, yy = y + dy, xx = x + dx;
-          const bool in = is_center && zz >= 0 && zz < P.Z && yy >= 0 && yy < P.Y && xx >= 0 && xx < P.X;
-          w[((dz + 1) * 9 + (dy + 1) * 3 + (dx + 1)) * NT] =
-              in ? lev[vi + (long long)dz * P.sz + (long long)dy * P.sy + dx] : (uint8_t)0;
-        }
-    double f[GLCM_NF];
-    int n_ok = 0;
-    unsigned long long tcls = 0;
-    const uint32_t tasks = glcm_fast_voxel_phaseA(w, NT, &eqbuf[tid], NT, T, P, f, &n_ok, &tcls);
-    if (!live) continue;
-    if (!is_center) {
-#pragma unroll
-      for (int k = 0; k < GLCM_NF; k++) out[k * fstride + oi] = P.init_value;
-      continue;
-    }
-#pragma unroll
-    for (int k = 0; k < GLCM_NF; k++) out[k * fstride + oi] = f[k];
-    if (tasks) {
-      const int k = __popc(tasks);
-      unsigned q = atomicAdd(qcount, (unsigned)k);
-      bool first = true;
-      for (uint32_t m = tasks; m; m &= m - 1, q++) {
-        GlcmTask e;
-        e.vi = vi; e.slot = (uint8_t)(__ffs((int)m) - 1); e.n_ok = (uint8_t)n_ok; e.count = first ? (uint8_t)k : 0;
-        e.cls = (uint8_t)(tcls >> (GF_CLS_BITS * e.slot) & (GF_NCLS - 1)); e.unused = 0.f;
-        queue[q] = e;
-        first = false;
+        for (int k = 0; k < GLCM_NF; k++) out[k * fstride + v.oi] = P.init_value;
       }
     }
+    __syncthreads();
+    const unsigned nd = ndefer;
+    __syncthreads();
+    // the general body over the last `count` list entries (idle threads run on an all-zero window)
+    const unsigned count = more ? (nd >= NT ? NT : 0) : nd;
+    if (count) {
+      if (tid == 0) ndefer = nd - count;
+      const bool dlive = (unsigned)tid < count;
+      const PhaseAVoxel v = glcm_phaseA_load<NT>(lev, centers, P, z0, out_z0, dlive ? defer[nd - count + tid] : 0, dlive, w);
+      glcm_phaseA_voxel<false, NT>(w, eq, T, P, v, dlive, out, fstride, queue, qcount);
+      __syncthreads();                                               // every entry read before the list grows again
+    }
+    if (!more) break;
   }
 }
 

@@ -114,15 +114,22 @@ int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P
     // latency of this issue-bound kernel; 384 threads sit in between.  B200_GLCM_NT selects the variant for A/B runs.
     static const int nt = getenv("B200_GLCM_NT") ? atoi(getenv("B200_GLCM_NT")) : GF_PHASEA_NT;
     const uint8_t* l8 = (const uint8_t*)lev;
-    const long long need = (total + nt - 1) / nt, cap = (long long)sms * 8;
-    const int grid = (int)(need < cap ? need : cap);
     static bool pa_attr[64] = {false};
+    static int pa_bps[64][3];
     if (!pa_attr[dev & 63]) {
       RB_CUDA(cudaFuncSetAttribute(glcm_fast_kernel<1, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, glcm_phaseA_smem_bytes(256)));
       RB_CUDA(cudaFuncSetAttribute(glcm_fast_kernel<1, 384>, cudaFuncAttributeMaxDynamicSharedMemorySize, glcm_phaseA_smem_bytes(384)));
       RB_CUDA(cudaFuncSetAttribute(glcm_fast_kernel<1, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, glcm_phaseA_smem_bytes(512)));
+      RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pa_bps[dev & 63][0], glcm_fast_kernel<1, 256>, 256, glcm_phaseA_smem_bytes(256)));
+      RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pa_bps[dev & 63][1], glcm_fast_kernel<1, 384>, 384, glcm_phaseA_smem_bytes(384)));
+      RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pa_bps[dev & 63][2], glcm_fast_kernel<1, 512>, 512, glcm_phaseA_smem_bytes(512)));
       pa_attr[dev & 63] = true;
     }
+    // one resident wave of blocks, each walking many tiles: a block runs its list of non-full windows in whole tiles,
+    // so its last, partly filled tile is paid once per block rather than once per short-lived block
+    const int bps = pa_bps[dev & 63][nt == 512 ? 2 : nt == 384 ? 1 : 0];
+    const long long need = (total + nt - 1) / nt, cap = (long long)sms * (bps > 0 ? bps : 1);
+    const int grid = (int)(need < cap ? need : cap);
     if (nt == 512) glcm_fast_kernel<1, 512><<<grid, 512, glcm_phaseA_smem_bytes(512), st>>>(l8, centers, P, T, out, fstride, za, zb, out_z0, Q->q, Q->count);
     else if (nt == 384) glcm_fast_kernel<1, 384><<<grid, 384, glcm_phaseA_smem_bytes(384), st>>>(l8, centers, P, T, out, fstride, za, zb, out_z0, Q->q, Q->count);
     else glcm_fast_kernel<1, 256><<<grid, 256, glcm_phaseA_smem_bytes(256), st>>>(l8, centers, P, T, out, fstride, za, zb, out_z0, Q->q, Q->count);
