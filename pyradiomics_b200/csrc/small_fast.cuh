@@ -4,9 +4,8 @@
 // equality masks of the window like the GLCM / GLRLM fast paths:
 //   GLDM  dependence of a voxel = popcount(close-level mask & static neighbour mask); merged
 //         (level, dependence) counts = popcount(equal-level mask & equal-dependence mask)
-//   NGTDM neighbour sums from static neighbour lists (unmasked voxels carry level 0); the pairwise
-//         level loop is only needed for Busyness / Complexity, Contrast and Strength collapse to
-//         closed forms in integer moments
+//   NGTDM a full-window body in exact integers and a general one; Busyness from one sort, Contrast and
+//         Strength in closed forms of integer moments, only Complexity keeps a pairwise level loop
 //   GLSZM zones of one level = flood fill of its equality mask by separable bitmask dilation
 // __host__ __device__ (tests/host_emul checks them on the CPU; test-only).
 #pragma once
@@ -110,89 +109,182 @@ RB_HD void gldm_fast_voxel(const int* wl, int alpha, const SmallFastTables& T, d
 }
 
 // ---------------------------------------------------------------------------------------- NGTDM
-struct NgtdmPass1 {
-  const int* wl; uint32_t M; const SmallFastTables* T; double* diff;
+// Two bodies, chosen by the window alone (so slab and whole-volume maps agree bit for bit):
+//   full window (a centre whose 27 levels are all non-zero: 97.7 % of a 256^3 volume, all but the faces) -- every
+//     position v has the constant neighbour count cnt_v in {7, 11, 17, 26} and Nvp = 27.  The neighbour sums are
+//     separable 3x3x3 box sums, and diff_v * L = |cnt_v g_v - sum_v| * (L / cnt_v), L = lcm(7, 11, 17, 26) = 34034, is
+//     an integer <= 254 L (8.6 M): class sums and sum_i s_i are exact int32, sum_i n_i s_i is an exact double, and every
+//     feature is rounded only in its last few operations, independently of the summation order.
+//   general window (volume faces, ROI borders, holes) -- zeros are unmasked, counts come from the mask, and
+//     diff_v = |cnt_v g_v - sum_v| * (1 / cnt_v) from the rcp table.
+// Both bodies add each position's diff to its class's lowest position (the representative) in per-thread shared
+// scratch -- 27 fixed steps, no branch per class -- and then compact the classes in place (entry k <= position v, which
+// is already read).  The Busyness denominator sum_{a<b} |i_a n_a - i_b n_b| is an integer: sorting the 27 values
+// x_v = g_v n_v on the representatives (0 elsewhere) gives it as sum_k (2k - 53 + nl) x_(k), the zeros adding nothing.
+// Only Complexity, with its 1 / (n_a + n_b) per pair of classes, keeps a pair loop.
+constexpr int NGTDM_L = 34034;
+
+// neighbour count of window position (z, y, x) in a full 3x3x3 window: 7 at a corner, 11 on an edge, 17 on a face, 26
+RB_HD constexpr int ngtdm_full_cnt(int v) {
+  return (v % 3 == 1 ? 3 : 2) * ((v / 3) % 3 == 1 ? 3 : 2) * (v / 9 == 1 ? 3 : 2) - 1;
+}
+
+// d as a double, exactly, for 0 <= d < 2^32 (on the device: one fp64 add instead of the slower int -> fp64 conversion)
+RB_HD double ngtdm_i2d(int d) {
+#ifdef __CUDA_ARCH__
+  return __hiloint2double(0x43300000, d) - 4503599627370496.0;
+#else
+  return (double)d;
+#endif
+}
+
+// sum_{a<b} |i_a - i_b| (n_a s_a + n_b s_b) / (n_a + n_b) over the nl compacted classes (pk = n << 8 | i, ns = n s)
+RB_HD double ngtdm_complexity_pairs(const int* pk, const double* ns, int st, int nl, const SmallFastTables& T) {
+  double c0 = 0, c1 = 0;
+  for (int a = 0; a + 1 < nl; a++) {
+    const int pa = pk[a * st], na = pa >> 8, ia = pa & 255;
+    const double sa = ns[a * st];
+    int b = a + 1;
+    for (; b + 1 < nl; b += 2) {                // two independent chains
+      const int p0 = pk[b * st], p1 = pk[(b + 1) * st];
+      const int x0 = ia - (p0 & 255), x1 = ia - (p1 & 255);
+      c0 += ngtdm_i2d(x0 < 0 ? -x0 : x0) * ((sa + ns[b * st]) * T.rcp[na + (p0 >> 8)]);
+      c1 += ngtdm_i2d(x1 < 0 ? -x1 : x1) * ((sa + ns[(b + 1) * st]) * T.rcp[na + (p1 >> 8)]);
+    }
+    if (b < nl) {
+      const int p0 = pk[b * st], x0 = ia - (p0 & 255);
+      c0 += ngtdm_i2d(x0 < 0 ? -x0 : x0) * ((sa + ns[b * st]) * T.rcp[na + (p0 >> 8)]);
+    }
+  }
+  return c0 + c1;
+}
+
+// general body: diff_v = |cnt_v g_v - sum_v| / cnt_v (static neighbour lists, unmasked voxels carry level 0) added to
+// the class representative's entry of scr_ns
+struct NgtdmGeneralDiff {
+  const int* wl; const uint32_t* eq; uint32_t M; const SmallFastTables* T; double* scr_ns; int st; double ssum;
   template <int V> RB_HD void at() {
-    if (!wl[V]) { diff[V] = 0; return; }
+    if (!wl[V]) return;
     constexpr uint32_t nb = NB26<V>::value;
     int sum = 0;
 #pragma unroll
-    for (int u = 0; u < 27; u++) if (nb >> u & 1u) sum += wl[u];      // static neighbour list
-    const int cnt = RB_POPC(M & nb);
-    diff[V] = cnt ? fabs((double)wl[V] - (double)sum / (double)cnt) : 0.0;
+    for (int u = 0; u < 27; u++) if (nb >> u & 1u) sum += wl[u];
+    const int cnt = RB_POPC(M & nb), x = cnt * wl[V] - sum;
+    const double d = ngtdm_i2d(x < 0 ? -x : x) * T->rcp[cnt];     // (cnt = 0: x = 0)
+    ssum += d;
+    const int r = RB_CTZ(eq[V]);
+    const double prev = r == V ? 0.0 : scr_ns[r * st];
+    scr_ns[r * st] = prev + d;
   }
 };
 
-// scr_pk / scr_cs: per-thread scratch for the compacted level classes, 27 entries each with element stride st (device:
-// shared memory laid out [entry][thread]; round 1 kept them in dynamically indexed local arrays -- 482 M local loads per
-// 256^3 volume, the kernel was as slow as GLRLM for 5 features).  pk = class size << 8 | level, cs = class sum of diff.
-constexpr int NGTDM_SCR_BYTES = 27 * (int)(sizeof(int) + sizeof(double));
-RB_HD void ngtdm_fast_voxel(const int* wl, const SmallFastTables& T, double* out, int* scr_pk, double* scr_cs, int st) {
+// scr_pk / scr_ns: per-thread scratch of 27 entries each, element stride st (device: shared memory laid out
+// [entry][thread]).  FULL: wl must be a full window (all 27 levels non-zero).
+// NGTDM_ABLATE (developer A/B builds, -D): stop the body early and store stand-in values, to time its stages --
+// 1 after the window sums, 2 after the equality masks, diffs and class sums, 3 after the compaction, 4 after the sort
+#ifndef NGTDM_ABLATE
+#define NGTDM_ABLATE 0
+#endif
+#define NGTDM_ABLATE_AT(STAGE, V0, V1) \
+  if (NGTDM_ABLATE == STAGE) { for (int _k = 0; _k < NGTDM_NF; _k++) out[_k] = (double)(V0) + (double)(V1); return; }
+template <bool FULL>
+RB_HD void ngtdm_fast_body(const int* wl, const SmallFastTables& T, double* out, int* scr_pk, double* scr_ns, int st) {
+  int B = 0, C = 0;
+#pragma unroll
+  for (int v = 0; v < 27; v++) { B += wl[v] * wl[v]; C += wl[v]; }
+  NGTDM_ABLATE_AT(1, B, C)
   uint32_t eq[27];
   RB_EQMASKS_27(wl, eq);
-  uint32_t M = 0, rep = 0;
+  int Nvp = 27, SE = 0;                          // FULL: sum_v diff_v * L
+  double ssum = 0;                               // general: sum_v diff_v
+  if (FULL) {
+    // box sums over the window, separably (x, then y, then z); sum_v = box_v - g_v
+    int bx[27], by[27], bz[27];
+#pragma unroll
+    for (int r = 0; r < 27; r += 3) {
+      bx[r] = wl[r] + wl[r + 1]; bx[r + 1] = bx[r] + wl[r + 2]; bx[r + 2] = wl[r + 1] + wl[r + 2];
+    }
+#pragma unroll
+    for (int r = 0; r < 27; r += 9)
+#pragma unroll
+      for (int x = 0; x < 3; x++) {
+        const int* b = bx + r + x;
+        by[r + x] = b[0] + b[3]; by[r + 3 + x] = by[r + x] + b[6]; by[r + 6 + x] = b[3] + b[6];
+      }
+#pragma unroll
+    for (int yx = 0; yx < 9; yx++) {
+      bz[yx] = by[yx] + by[9 + yx]; bz[9 + yx] = bz[yx] + by[18 + yx]; bz[18 + yx] = by[9 + yx] + by[18 + yx];
+    }
+    // each position's integer diff to its class representative (rep <= v, so the representative's entry is set first)
+#pragma unroll
+    for (int v = 0; v < 27; v++) {
+      const int cnt = ngtdm_full_cnt(v);
+      const int x = (cnt + 1) * wl[v] - bz[v];
+      const int e = (x < 0 ? -x : x) * (NGTDM_L / cnt);
+      SE += e;
+      const int r = RB_CTZ(eq[v]);
+      const int prev = r == v ? 0 : scr_pk[r * st];
+      scr_pk[r * st] = prev + e;
+    }
+  } else {
+    uint32_t M = 0;
+#pragma unroll
+    for (int v = 0; v < 27; v++) if (wl[v]) M |= 1u << v;
+    Nvp = RB_POPC(M);
+    NgtdmGeneralDiff p1{wl, eq, M, &T, scr_ns, st, 0.0};
+    ForPos<0, 27>::go(p1);
+    ssum = p1.ssum;
+  }
+  NGTDM_ABLATE_AT(2, SE + ssum, scr_pk[st] + scr_ns[st])
+  // compact the classes: entry nl <= v is already read.  Non-representatives write a dead entry at nl (overwritten by
+  // the next representative, or past the end).
+  int nl = 0, SL = 0, SL2 = 0;
+  double pw = 0;                                 // sum_i n_i s_i (FULL: times L)
+  int X[27];
 #pragma unroll
   for (int v = 0; v < 27; v++) {
-    if (wl[v]) M |= 1u << v;
-    if (eq[v] && (eq[v] & ((1u << v) - 1)) == 0) rep |= 1u << v;
+    const bool rep = eq[v] && (eq[v] & ((1u << v) - 1)) == 0;
+    const int n = RB_POPC(eq[v]), g = wl[v];
+    const double ns = FULL ? ngtdm_i2d(n) * ngtdm_i2d(scr_pk[v * st]) : ngtdm_i2d(n) * scr_ns[v * st];
+    scr_pk[nl * st] = n << 8 | g;
+    scr_ns[nl * st] = ns;
+    X[v] = rep ? g * n : 0;
+    if (rep) { nl++; SL += g; SL2 += g * g; pw += ns; }
   }
-  double diff[27];
-  NgtdmPass1 p1{wl, M, &T, diff};
-  ForPos<0, 27>::go(p1);
-  const int Nvp = RB_POPC(M), nlev = RB_POPC(rep);
-  // per level: n = class size, i = level, s = class sum of diff -- compacted (data-dependent count)
-  int B = 0, C = 0, SL = 0, SL2 = 0, nl = 0;
-  double ssum = 0, pw = 0;       // sum_i s_i ; sum_i n_i s_i
+  NGTDM_ABLATE_AT(3, nl + SL + X[5] + X[20], pw)
+  RB_NGTDM_SORT27(X);
+  int bd = 0;                                    // sum_{a<b} |i_a n_a - i_b n_b|
 #pragma unroll
-  for (int v = 0; v < 27; v++) {
-    if (wl[v]) { B += wl[v] * wl[v]; C += wl[v]; ssum += diff[v]; pw += diff[v] * (double)RB_POPC(eq[v]); }
-    if (rep >> v & 1u) {
-      double s = 0;
-#pragma unroll
-      for (int u = v; u < 27; u++) if (eq[v] >> u & 1u) s += diff[u];      // (v is the lowest position of its class)
-      scr_pk[nl * st] = RB_POPC(eq[v]) << 8 | wl[v];
-      scr_cs[nl * st] = s;
-      nl++;
-      SL += wl[v]; SL2 += wl[v] * wl[v];
-    }
-  }
-  // pairwise level terms: Busyness denominator sum_ij |i p_i - j p_j|, Complexity numerator
-  double busy = 0, cpx = 0;
-  for (int a = 0; a + 1 < nl; a++) {
-    const int pa = scr_pk[a * st], na = pa >> 8, ia = pa & 255;
-    const double sa = na * scr_cs[a * st];
-    const int ina = ia * na;
-    double cp = 0;
-    int bs = 0;
-    for (int b = a + 1; b < nl; b++) {
-      const int pb = scr_pk[b * st], nb_ = pb >> 8, ib = pb & 255;
-      const int x = ina - ib * nb_;
-      bs += x < 0 ? -x : x;
-      const int d = ia > ib ? ia - ib : ib - ia;
-      cp += (double)d * (sa + nb_ * scr_cs[b * st]) * T.rcp[na + nb_];
-    }
-    busy += (double)bs;
-    cpx += cp;
-  }
-  const double invN = 1.0 / Nvp;
-  busy *= 2.0 * invN;                         // both orders, p = n / Nvp
-  cpx *= 2.0 * invN;                          // sum over ordered pairs, then / Nvp below... (see Complexity)
-  const double ps = pw * invN;                // sum_i p_i s_i
-  out[N_Coarseness] = ps != 0 ? 1.0 / ps : 1e6;
-  const double div = (double)nlev * (nlev - 1);
-  const double con = 2.0 * (double)(Nvp * B - C * C) * invN * invN;     // sum_ij p_i p_j (i-j)^2
-  out[N_Contrast] = div != 0 ? con * ssum * invN / div : 0.0;
-  out[N_Busyness] = busy != 0 ? ps / busy : 0.0;
-  out[N_Complexity] = cpx;                    // = sum_{i != j} |i-j| (p_i s_i + p_j s_j)/(p_i + p_j) / Nvp
-  // Strength = sum_ij (p_i + p_j)(i-j)^2 / sum s = (2/Nvp) (nlev*B - 2*C*SL + Nvp*SL2) / sum s
-  const double str = 2.0 * invN * (double)(nlev * B - 2 * C * SL + Nvp * SL2);
-  out[N_Strength] = ssum != 0 ? str / ssum : 0.0;
+  for (int k = 0; k < 27; k++) bd += (2 * k - 53 + nl) * X[k];
+  NGTDM_ABLATE_AT(4, bd + SL2, pw)
+  const double cpx = ngtdm_complexity_pairs(scr_pk, scr_ns, st, nl, T);
+  // u = the unit of the diffs (FULL: L); p_i = n_i / Nvp
+  const double u = FULL ? (double)NGTDM_L : 1.0, N = (double)Nvp;
+  const double sdiff = FULL ? (double)SE : ssum;
+  out[N_Coarseness] = pw != 0 ? N * u / pw : 1e6;                         // 1 / sum_i p_i s_i
+  const double div = (double)nl * (nl - 1);
+  // Contrast = sum_ij p_i p_j (i-j)^2 * sum s / Nvp / (nl (nl-1)), sum_ij p_i p_j (i-j)^2 = 2 (Nvp B - C^2) / Nvp^2
+  out[N_Contrast] = div != 0 ? 2.0 * (double)(Nvp * B - C * C) * sdiff / (N * N * N * u * div) : 0.0;
+  out[N_Busyness] = bd != 0 ? pw / (2.0 * u * (double)bd) : 0.0;       // sum_i p_i s_i / sum_ij |i p_i - j p_j|
+  out[N_Complexity] = 2.0 * cpx / (N * u);      // sum_{i != j} |i-j| (p_i s_i + p_j s_j) / (p_i + p_j) / Nvp
+  // Strength = sum_ij (p_i + p_j)(i-j)^2 / sum s = (2/Nvp) (nl B - 2 C SL + Nvp SL2) / sum s
+  out[N_Strength] = sdiff != 0 ? 2.0 * u * (double)(nl * B - 2 * C * SL + Nvp * SL2) / (N * sdiff) : 0.0;
 }
-// convenience: private scratch (host emulation)
+
+// a window is full when all 27 levels are non-zero
+RB_HD bool ngtdm_window_full(const int* wl) {
+  bool full = true;
+#pragma unroll
+  for (int v = 0; v < 27; v++) full &= wl[v] != 0;
+  return full;
+}
+
+// convenience: private scratch, body chosen by the window (host emulation)
 RB_HD void ngtdm_fast_voxel(const int* wl, const SmallFastTables& T, double* out) {
-  int pk[27];
-  double cs[27];
-  ngtdm_fast_voxel(wl, T, out, pk, cs, 1);
+  int pk[27] = {0};
+  double ns[27] = {0};
+  if (ngtdm_window_full(wl)) ngtdm_fast_body<true>(wl, T, out, pk, ns, 1);
+  else ngtdm_fast_body<false>(wl, T, out, pk, ns, 1);
 }
 
 // ---------------------------------------------------------------------------------------- GLSZM

@@ -254,7 +254,7 @@ int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& 
 
 // ------------------------------------------------------------------ GLSZM / GLDM / NGTDM fast paths
 // SYNC: block-uniform tiles with a barrier per tile, so the block's warps stream the (large,
-// straight-line) GLDM / NGTDM bodies together and share instruction-cache lines (free-running warps stall
+// straight-line) GLDM body together and share instruction-cache lines (free-running warps stall
 // on instruction fetch).
 template <int CLS, int NT, bool SYNC>
 __global__ void __launch_bounds__(NT)
@@ -262,16 +262,13 @@ small_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
                   const __grid_constant__ VoxParams P, const SmallFastTables* __restrict__ Tg,
                   double* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
   __shared__ SmallFastTables T;
-  // NGTDM: the compacted level classes of every thread, [entry][thread]
-  __shared__ double ng_cs[CLS == C_NGTDM ? 27 * NT : 1];
-  __shared__ int ng_pk[CLS == C_NGTDM ? 27 * NT : 1];
   {
     const uint32_t* src = reinterpret_cast<const uint32_t*>(Tg);
     uint32_t* dst = reinterpret_cast<uint32_t*>(&T);
     for (int i = threadIdx.x; i < (int)(sizeof(SmallFastTables) / 4); i += NT) dst[i] = src[i];
   }
   __syncthreads();
-  constexpr int NF = CLS == C_GLSZM ? GLSZM_NF : CLS == C_GLDM ? GLDM_NF : NGTDM_NF;
+  constexpr int NF = CLS == C_GLSZM ? GLSZM_NF : GLDM_NF;
   const long long plane = (long long)P.Y * P.X;
   const long long total = (long long)(z1 - z0) * plane;
   const long long ntiles = (total + NT - 1) / NT;
@@ -307,11 +304,102 @@ small_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
     }
     double f[16];
     if (CLS == C_GLSZM) glszm_fast_voxel(wl, T, f);
-    else if (CLS == C_GLDM) gldm_fast_voxel(wl, P.alpha, T, f);
-    else ngtdm_fast_voxel(wl, T, f, ng_pk + (CLS == C_NGTDM ? threadIdx.x : 0), ng_cs + (CLS == C_NGTDM ? threadIdx.x : 0), NT);
+    else gldm_fast_voxel(wl, P.alpha, T, f);
     if (!live) continue;
 #pragma unroll
     for (int k = 0; k < NF; k++) out[k * fstride + oi] = is_center ? f[k] : P.init_value;
+  }
+}
+
+// NGTDM: block-uniform tiles of NT voxels.  A centre with a full window runs the full-window body at once, a voxel that
+// is not a centre stores init_value, and any other centre (the volume's faces, the ROI's border and holes) goes to the
+// block's list, which the block runs through the general body NT at a time whenever NT are waiting, and once at the end
+// (the scheme of GLCM phase A: no warp runs both bodies for one tile).  Per-thread scratch for the level classes lives
+// in shared memory, [entry][thread].
+constexpr int NGTDM_NT = 128;
+template <int NT>
+__global__ void __launch_bounds__(NT, 4)
+ngtdm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
+                  const __grid_constant__ VoxParams P, const SmallFastTables* __restrict__ Tg,
+                  double* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
+  __shared__ SmallFastTables T;
+  __shared__ double ng_ns[27 * NT];
+  __shared__ int ng_pk[27 * NT];
+  __shared__ long long defer[2 * NT];                              // chunk indices of the centres left to the general body
+  __shared__ unsigned ndefer;
+  {
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(Tg);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(&T);
+    for (int i = threadIdx.x; i < (int)(sizeof(SmallFastTables) / 4); i += NT) dst[i] = src[i];
+  }
+  const int tid = threadIdx.x;
+  if (tid == 0) ndefer = 0;
+  __syncthreads();
+  const long long plane = (long long)P.Y * P.X;
+  const long long total = (long long)(z1 - z0) * plane;
+  const long long ntiles = (total + NT - 1) / NT;
+  // voxel t of the chunk: its window (zeros outside the volume), output index and whether it is a centre
+  auto load = [&](long long t, int* wl, long long& oi) -> bool {
+    const int z = z0 + (int)(t / plane);
+    const int rem = (int)(t % plane);
+    const int y = rem / P.X, x = rem % P.X;
+    const long long vi = (long long)z * P.sz + (long long)y * P.sy + x;
+    oi = (long long)(z - out_z0) * plane + rem;
+    const bool is_center = centers ? centers[(long long)z * plane + rem] != 0 : lev[vi] != 0;
+    int p = 0;
+#pragma unroll
+    for (int dz = -1; dz <= 1; dz++)
+#pragma unroll
+      for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+        for (int dx = -1; dx <= 1; dx++, p++) {
+          const int zz = z + dz, yy = y + dy, xx = x + dx;
+          const bool in = is_center && zz >= 0 && zz < P.Z && yy >= 0 && yy < P.Y && xx >= 0 && xx < P.X;
+          wl[p] = in ? lev[vi + (long long)dz * P.sz + (long long)dy * P.sy + dx] : 0;
+        }
+    return is_center;
+  };
+  // one pass per tile and a last pass with no tile (one call site per body)
+  for (long long tile = blockIdx.x;; tile += gridDim.x) {
+    const bool more = tile < ntiles;                                 // block-uniform
+    if (more) {
+      const long long t = tile * NT + tid;
+      if (t < total) {
+        int wl[27];
+        long long oi;
+        const bool is_center = load(t, wl, oi);
+        if (is_center && ngtdm_window_full(wl)) {
+          double f[NGTDM_NF];
+          ngtdm_fast_body<true>(wl, T, f, ng_pk + tid, ng_ns + tid, NT);
+#pragma unroll
+          for (int k = 0; k < NGTDM_NF; k++) out[k * fstride + oi] = f[k];
+        } else if (is_center) {
+          defer[atomicAdd(&ndefer, 1u)] = t;
+        } else {
+#pragma unroll
+          for (int k = 0; k < NGTDM_NF; k++) out[k * fstride + oi] = P.init_value;
+        }
+      }
+    }
+    __syncthreads();
+    const unsigned nd = ndefer;
+    __syncthreads();
+    // the general body over the last `count` list entries
+    const unsigned count = more ? (nd >= NT ? NT : 0) : nd;
+    if (count) {
+      if (tid == 0) ndefer = nd - count;
+      if ((unsigned)tid < count) {
+        int wl[27];
+        long long oi;
+        load(defer[nd - count + tid], wl, oi);
+        double f[NGTDM_NF];
+        ngtdm_fast_body<false>(wl, T, f, ng_pk + tid, ng_ns + tid, NT);
+#pragma unroll
+        for (int k = 0; k < NGTDM_NF; k++) out[k * fstride + oi] = f[k];
+      }
+      __syncthreads();                                               // every entry read before the list grows again
+    }
+    if (!more) break;
   }
 }
 
@@ -347,24 +435,30 @@ int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const Vo
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const uint8_t* l8 = (const uint8_t*)lev;
-  static const int mode_env = getenv("B200_SMALL_MODE") ? atoi(getenv("B200_SMALL_MODE")) : -1;   // 0 free-running, 1 sync/128, 2 sync/256, -1: measured best per class
-  const int mode = mode_env >= 0 ? mode_env : cls == C_GLDM ? 2 : 1;
+  if (cls == C_NGTDM) {
+    // one resident wave of blocks, each walking many tiles: a block's last, partly filled list tile is paid once
+    static int ng_bps[64] = {0};
+    if (!ng_bps[dev & 63]) RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ng_bps[dev & 63], ngtdm_fast_kernel<NGTDM_NT>, NGTDM_NT, 0));
+    const long long need = (total + NGTDM_NT - 1) / NGTDM_NT, cap = (long long)sms * (ng_bps[dev & 63] > 0 ? ng_bps[dev & 63] : 1);
+    ngtdm_fast_kernel<NGTDM_NT><<<(int)(need < cap ? need : cap), NGTDM_NT, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+  }
+  static const int mode_env = getenv("B200_SMALL_MODE") ? atoi(getenv("B200_SMALL_MODE")) : -1;   // GLDM: 0 free-running, 1 sync/128, 2 sync/256, -1: measured best
+  const int mode = mode_env >= 0 ? mode_env : 2;
   if (cls == C_GLSZM || mode == 0) {
     long long need = (total + 127) / 128, cap = (long long)sms * 32;
     const int grid = (int)(need < cap ? need : cap);
     if (cls == C_GLSZM) small_fast_kernel<C_GLSZM, 128, false><<<grid, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
-    else if (cls == C_GLDM) small_fast_kernel<C_GLDM, 128, false><<<grid, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
-    else small_fast_kernel<C_NGTDM, 128, false><<<grid, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
+    else small_fast_kernel<C_GLDM, 128, false><<<grid, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
   } else if (mode == 1) {
     long long need = (total + 127) / 128, cap = (long long)sms * 32;
     const int grid = (int)(need < cap ? need : cap);
-    if (cls == C_GLDM) small_fast_kernel<C_GLDM, 128, true><<<grid, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
-    else small_fast_kernel<C_NGTDM, 128, true><<<grid, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
+    small_fast_kernel<C_GLDM, 128, true><<<grid, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
   } else {
     long long need = (total + 255) / 256, cap = (long long)sms * 16;
     const int grid = (int)(need < cap ? need : cap);
-    if (cls == C_GLDM) small_fast_kernel<C_GLDM, 256, true><<<grid, 256, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
-    else small_fast_kernel<C_NGTDM, 128, true><<<grid * 2, 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);   // (its per-thread shared scratch caps the block at 128 threads)
+    small_fast_kernel<C_GLDM, 256, true><<<grid, 256, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
   }
   RB_LAUNCH_CHECK();
   return RB_OK;
