@@ -497,21 +497,13 @@ recursive_gauss_x_kernel(const TIn* __restrict__ in, long long nlines, int X, co
   }
 }
 
-static int grid_n(long long n, int block, int per_sm) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long need = (n + block - 1) / block, cap = (long long)sms * per_sm;
-  return (int)(need < cap ? (need < 1 ? 1 : need) : cap);
-}
-
 int minmax_launch(const void* img, int dt, const uint8_t* mask, long long n, long long* keys, cudaStream_t st) {
-  minmax_kernel<<<grid_n(n, 256, 8), 256, 0, st>>>(img, dt, mask, n, keys);
+  minmax_kernel<<<grid_for(n, 256, 8), 256, 0, st>>>(img, dt, mask, n, keys);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
 int pointwise_image_launch(const void* img, int dt, long long n, int kind, double c, double* out, cudaStream_t st) {
-  const int grid = grid_n(n, 256, 8);
+  const int grid = grid_for(n, 256, 8);
   switch (kind) {
     case RB_PW_SQUARE: pointwise_image_kernel<RB_PW_SQUARE><<<grid, 256, 0, st>>>(img, dt, n, c, out); break;
     case RB_PW_SQUAREROOT: pointwise_image_kernel<RB_PW_SQUAREROOT><<<grid, 256, 0, st>>>(img, dt, n, c, out); break;
@@ -548,21 +540,21 @@ int roi_moments_launch(const void* img, int dt, const uint8_t* mask, long long n
 }
 int normalize_launch(const void* img, int dt, long long n, double mean, double sigma, int clamp, double outliers,
                      double scale, double* out, cudaStream_t st) {
-  normalize_kernel<<<grid_n(n, 256, 8), 256, 0, st>>>(img, dt, n, mean, 1.0 / sigma, clamp, outliers, scale, out);
+  normalize_kernel<<<grid_for(n, 256, 8), 256, 0, st>>>(img, dt, n, mean, 1.0 / sigma, clamp, outliers, scale, out);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
 int resegment_launch(const void* img, int dt, const uint8_t* mask, long long n, double lo, double hi, int two,
                      uint8_t* out, unsigned long long* counts, cudaStream_t st) {
   RB_CUDA(cudaMemsetAsync(counts, 0, 2 * sizeof(unsigned long long), st));
-  resegment_kernel<<<grid_n(n, 256, 8), 256, 0, st>>>(img, dt, mask, n, lo, hi, two, out, counts);
+  resegment_kernel<<<grid_for(n, 256, 8), 256, 0, st>>>(img, dt, mask, n, lo, hi, two, out, counts);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
 int digitize_launch(const void* img, int dt, const uint8_t* mask, long long n, const double* edges, int ne, int32_t* out,
                     cudaStream_t st) {
   const size_t sh = ne <= 4096 ? sizeof(double) * ne : 0;
-  digitize_kernel<<<grid_n(n, 256, 8), 256, sh, st>>>(img, dt, mask, n, edges, ne, out);
+  digitize_kernel<<<grid_for(n, 256, 8), 256, sh, st>>>(img, dt, mask, n, edges, ne, out);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
@@ -572,7 +564,7 @@ int swt_axis_launch(const double* in, int Z, int Y, int X, int axis, const doubl
   SwtFilters W;
   W.F = F;
   for (int j = 0; j < F; j++) { W.lo[j] = lo[j]; W.hi[j] = hi[j]; }
-  swt_axis_kernel<<<grid_n((long long)Z * Y * X, 256, 8), 256, 0, st>>>(in, Z, Y, X, axis, W, out_lo, out_hi);
+  swt_axis_kernel<<<grid_for((long long)Z * Y * X, 256, 8), 256, 0, st>>>(in, Z, Y, X, axis, W, out_lo, out_hi);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
@@ -588,14 +580,8 @@ int swt3d_launch(const double* in, int Z, int Y, int X, const double* lo, const 
   const int grid = ((X + SWT_TX - 1) / SWT_TX) * ((Y + SWT_TY - 1) / SWT_TY);
   const int H = F - 1, NT = SWT_TY * SWT_TX;
   const int smem = (int)sizeof(double) * ((SWT_TY + H) * (SWT_TX + H) + 2 * (SWT_TY + H) * SWT_TX + F * 4 * NT);
-  static bool attr[64] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!attr[dev & 63]) {
-    RB_CUDA(cudaFuncSetAttribute(swt3d_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    RB_CUDA(cudaFuncSetAttribute(swt3d_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    attr[dev & 63] = true;
-  }
+  RB_CUDA(set_max_dynamic_smem(swt3d_kernel<6>, 64 * 1024));
+  RB_CUDA(set_max_dynamic_smem(swt3d_kernel<8>, 96 * 1024));
   if (F == 2) swt3d_kernel<2><<<grid, NT, smem, st>>>(in, Z, Y, X, W, out, band_stride, z_begin, z_end);
   else if (F == 4) swt3d_kernel<4><<<grid, NT, smem, st>>>(in, Z, Y, X, W, out, band_stride, z_begin, z_end);
   else if (F == 6) swt3d_kernel<6><<<grid, NT, smem, st>>>(in, Z, Y, X, W, out, band_stride, z_begin, z_end);
@@ -610,13 +596,13 @@ int recursive_gauss_launch(const void* in, int in_is_f32, int Z, int Y, int X, i
   const int N = axis == 0 ? Z : axis == 1 ? Y : X;
   const long long nlines = (long long)Z * Y * X / N;
   if (axis == 2) {                              // x: lines are contiguous -> tile-transposed kernel, 32 lines per warp
-    const int gx = grid_n((nlines + 31) / 32, 4, 16);
+    const int gx = grid_for((nlines + 31) / 32, 4, 16);
     if (in_is_f32) recursive_gauss_x_kernel<float><<<gx, 128, 0, st>>>((const float*)in, nlines, X, C, out, scratch, scale, accumulate);
     else recursive_gauss_x_kernel<double><<<gx, 128, 0, st>>>((const double*)in, nlines, X, C, out, scratch, scale, accumulate);
     RB_LAUNCH_CHECK();
     return RB_OK;
   }
-  const int grid = grid_n(nlines, 128, 8);
+  const int grid = grid_for(nlines, 128, 8);
   if (in_is_f32) recursive_gauss_axis_kernel<float><<<grid, 128, 0, st>>>((const float*)in, Z, Y, X, axis, C, out, scratch, scale, accumulate);
   else recursive_gauss_axis_kernel<double><<<grid, 128, 0, st>>>((const double*)in, Z, Y, X, axis, C, out, scratch, scale, accumulate);
   RB_LAUNCH_CHECK();

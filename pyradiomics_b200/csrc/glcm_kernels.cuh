@@ -5,6 +5,7 @@
 // structure -- and race-check it with ThreadSanitizer -- without a GPU.
 #pragma once
 #include "glcm_fast.cuh"
+#include "voxel_tiles.cuh"
 
 #ifndef RB_DYN_SHARED          // dynamic shared memory of the launching kernel
 #define RB_DYN_SHARED(type, name) extern __shared__ type name[]
@@ -63,17 +64,7 @@ template <> struct SolveKind<2> { static constexpr int lo = GF_DENSE_MAX_CLS + 1
 __device__ __forceinline__ void glcm_task_window(const uint8_t* __restrict__ lev, const VoxParams& P, long long vi, bool live,
                                                  uint8_t* w) {
   const int z = (int)(vi / P.sz), rem = (int)(vi % P.sz), y = rem / (int)P.sy, x = rem % (int)P.sy;
-  int p = 0;
-#pragma unroll
-  for (int dz = -1; dz <= 1; dz++)
-#pragma unroll
-    for (int dy = -1; dy <= 1; dy++)
-#pragma unroll
-      for (int dx = -1; dx <= 1; dx++, p++) {
-        const int zz = z + dz, yy = y + dy, xx = x + dx;
-        const bool in = live && zz >= 0 && zz < P.Z && yy >= 0 && yy < P.Y && xx >= 0 && xx < P.X;
-        w[p] = in ? lev[vi + (long long)dz * P.sz + (long long)dy * P.sy + dx] : (uint8_t)0;
-      }
+  load_window27(lev, P, z, y, x, vi, live, w, 1);
 }
 
 // sorted positions [begin, end) of the tile: tasks whose level graph has at most N nodes
@@ -207,44 +198,11 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
 }
 
 // ---- phase A (one thread per centre voxel) and phase C (finish) ---------------------------------
-struct PhaseAVoxel { long long vi, oi; bool center, full; };
-
-// voxel t of the chunk: its 27 window levels to w (stride NT; zeros outside the volume, all zeros if it is not a
-// centre) and whether the window is full (a centre whose 27 levels are all non-zero, see glcm_window_full)
-template <int NT>
-__device__ __forceinline__ PhaseAVoxel glcm_phaseA_load(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
-                                                        const VoxParams& P, int z0, int out_z0, long long t, bool live,
-                                                        uint8_t* w) {
-  const long long plane = (long long)P.Y * P.X;
-  const int z = z0 + (int)((live ? t : 0) / plane);
-  const int rem = (int)((live ? t : 0) % plane);
-  const int y = rem / P.X, x = rem % P.X;
-  PhaseAVoxel v;
-  v.vi = (long long)z * P.sz + (long long)y * P.sy + x;
-  v.oi = (long long)(z - out_z0) * plane + rem;
-  v.center = live && (centers ? centers[(long long)z * plane + rem] != 0 : lev[v.vi] != 0);
-  bool full = v.center;
-#pragma unroll
-  for (int dz = -1; dz <= 1; dz++)
-#pragma unroll
-    for (int dy = -1; dy <= 1; dy++)
-#pragma unroll
-      for (int dx = -1; dx <= 1; dx++) {
-        const int zz = z + dz, yy = y + dy, xx = x + dx;
-        const bool in = v.center && zz >= 0 && zz < P.Z && yy >= 0 && yy < P.Y && xx >= 0 && xx < P.X;
-        const uint8_t l = in ? lev[v.vi + (long long)dz * P.sz + (long long)dy * P.sy + dx] : (uint8_t)0;
-        full &= l != 0;
-        w[((dz + 1) * 9 + (dy + 1) * 3 + (dx + 1)) * NT] = l;
-      }
-  v.full = full;
-  return v;
-}
-
 // phase A of one centre voxel; store: write its 24 maps and queue its eigen-tasks (the general body holds barriers, so
 // every thread of the block runs it, idle ones with store = false)
 template <bool FULL, int NT>
 __device__ __forceinline__ void glcm_phaseA_voxel(const uint8_t* w, uint32_t* eq, const GlcmFastTables& T, const VoxParams& P,
-                                                  const PhaseAVoxel& v, bool store, double* __restrict__ out, long long fstride,
+                                                  const ChunkVoxel& v, bool store, double* __restrict__ out, long long fstride,
                                                   GlcmTask* __restrict__ queue, unsigned* __restrict__ qcount) {
   double f[GLCM_NF];
   int n_ok = 0;
@@ -267,11 +225,9 @@ __device__ __forceinline__ void glcm_phaseA_voxel(const uint8_t* w, uint32_t* eq
   }
 }
 
-// Block-uniform tiles of NT voxels: a centre with a full window runs the full-window body (no validity logic, constant
-// denominators, no barriers), a voxel that is not a centre stores init_value, and a centre whose window is not full (the
-// volume's faces, the ROI's border and holes) goes to the block's list.  The block runs the general body over that
-// list, NT at a time, whenever NT are waiting and once at the end.  (List entries are chunk indices: a chunk of 2^32
-// voxels would need a 1.3 TB eigen-task queue, which glcm_fast_launch fails to allocate first.)
+// Phase A over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh).  The window bytes live in shared
+// memory, [27][NT].  (List entries are chunk indices: a chunk of 2^32 voxels would need a 1.3 TB eigen-task queue,
+// which glcm_fast_launch fails to allocate first.)
 template <int MINB, int NT>
 __global__ void __launch_bounds__(NT, MINB)
 glcm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
@@ -283,48 +239,31 @@ glcm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ ce
   __shared__ unsigned ndefer;
   RB_DYN_SHARED(uint32_t, eqbuf);                                   // [27][NT] equality masks, then [27][NT] window bytes
   uint8_t* const wbuf = reinterpret_cast<uint8_t*>(eqbuf + 27 * NT);
-  {
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(Tg);
-    uint32_t* dst = reinterpret_cast<uint32_t*>(&T);
-    for (int i = threadIdx.x; i < (int)(sizeof(GlcmFastTables) / 4); i += NT) dst[i] = src[i];
-  }
-  const int tid = threadIdx.x;
-  if (tid == 0) ndefer = 0;
+  copy_tables_to_shared<NT>(T, Tg);
+  if (threadIdx.x == 0) ndefer = 0;
   __syncthreads();
-  const long long total = (long long)(z1 - z0) * P.Y * P.X;
-  const long long ntiles = (total + NT - 1) / NT;
-  uint8_t* const w = &wbuf[tid];
-  uint32_t* const eq = &eqbuf[tid];
-  // one pass per tile and a last pass with no tile (one call site per body: each is thousands of instructions)
-  for (long long tile = blockIdx.x;; tile += gridDim.x) {
-    const bool more = tile < ntiles;                                 // block-uniform
-    if (more) {
-      const long long t = tile * NT + tid;
-      const bool live = t < total;
-      const PhaseAVoxel v = glcm_phaseA_load<NT>(lev, centers, P, z0, out_z0, t, live, w);
-      if (v.full) {
+  uint8_t* const w = &wbuf[threadIdx.x];
+  uint32_t* const eq = &eqbuf[threadIdx.x];
+  full_window_tiles<NT>((long long)(z1 - z0) * P.Y * P.X, defer, ndefer,
+    [&](long long t, bool live, auto defer_it) {
+      const long long plane = (long long)P.Y * P.X;
+      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t, live);
+      const bool center = live && chunk_center(lev, centers, plane, v);
+      if (load_window27(lev, P, v.z, v.y, v.x, v.vi, center, w, NT)) {
         glcm_phaseA_voxel<true, NT>(w, eq, T, P, v, true, out, fstride, queue, qcount);
-      } else if (v.center) {
-        defer[atomicAdd(&ndefer, 1u)] = (unsigned)t;
+      } else if (center) {
+        defer_it();
       } else if (live) {
 #pragma unroll
         for (int k = 0; k < GLCM_NF; k++) out[k * fstride + v.oi] = P.init_value;
       }
-    }
-    __syncthreads();
-    const unsigned nd = ndefer;
-    __syncthreads();
-    // the general body over the last `count` list entries (idle threads run on an all-zero window)
-    const unsigned count = more ? (nd >= NT ? NT : 0) : nd;
-    if (count) {
-      if (tid == 0) ndefer = nd - count;
-      const bool dlive = (unsigned)tid < count;
-      const PhaseAVoxel v = glcm_phaseA_load<NT>(lev, centers, P, z0, out_z0, dlive ? defer[nd - count + tid] : 0, dlive, w);
-      glcm_phaseA_voxel<false, NT>(w, eq, T, P, v, dlive, out, fstride, queue, qcount);
-      __syncthreads();                                               // every entry read before the list grows again
-    }
-    if (!more) break;
-  }
+    },
+    [&](auto entry, bool live) {                                    // idle threads run on an all-zero window
+      const long long plane = (long long)P.Y * P.X;
+      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, live ? entry() : 0, live);
+      load_window27(lev, P, v.z, v.y, v.x, v.vi, live && chunk_center(lev, centers, plane, v), w, NT);
+      glcm_phaseA_voxel<false, NT>(w, eq, T, P, v, live, out, fstride, queue, qcount);
+    });
 }
 
 
@@ -339,9 +278,7 @@ glcm_fast_finish_kernel(const __grid_constant__ VoxParams P, const GlcmTask* __r
     if (!e.count) continue;
     double add = 0;
     for (int j = 0; j < e.count; j++) add += res[k + j];
-    const int z = (int)(e.vi / P.sz);
     const long long oi = e.vi - (long long)out_z0 * plane;   // contiguous volume: vi = z*plane + rem
-    (void)z;
     mcc_map[oi] += add / e.n_ok;
   }
 }

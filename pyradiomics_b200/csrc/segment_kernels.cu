@@ -253,13 +253,6 @@ __global__ void ngtdm_seg_finish_kernel(const unsigned long long* __restrict__ a
   out[g * 3 + 2] = (double)(g + 1);
 }
 
-static int sm_count() {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
-}
-
 // B200_SEG_TMA=0 forces the cooperative-load staging (A/B runs, tests); default: TMA whenever a tensor map can be built
 static bool seg_tma_enabled() {
   const char* e = getenv("B200_SEG_TMA");

@@ -186,14 +186,6 @@ shape_moments_kernel(const uint8_t* __restrict__ mask, int Z, int Y, int X, unsi
   }
 }
 
-static int grid_for(long long work, int threads, int per_sm) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long need = (work + threads - 1) / threads, cap = (long long)sms * per_sm;
-  return (int)(need < 1 ? 1 : need < cap ? need : cap);
-}
-
 // mask_dev: uint8 [Z][Y][X] with element strides (sz, sy, sx).  out7 (host): area, volume, the four
 // diameters (equal-z, equal-y, equal-x, 3-D) and the number of mesh vertices.
 int shape_coefficients_dev(const uint8_t* mask_dev, int Z, int Y, int X, long long sz, long long sy, long long sx,

@@ -6,6 +6,7 @@
 #include "common.cuh"
 #include "host_common.hpp"
 #include "vox_features.cuh"
+#include "voxel_tiles.cuh"
 
 namespace rb {
 
@@ -18,21 +19,17 @@ voxel_features_kernel(const T* __restrict__ lev, const uint8_t* __restrict__ cen
   const long long total = (long long)(z1 - z0) * plane;
   for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
        t += (long long)gridDim.x * blockDim.x) {
-    const int z = z0 + (int)(t / plane);
-    const int rem = (int)(t % plane);
-    const int y = rem / P.X, x = rem % P.X;
-    const long long vi = (long long)z * P.sz + (long long)y * P.sy + x;
-    const long long oi = (long long)(z - out_z0) * plane + rem;
+    const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t);
+    const bool is_center = chunk_center(lev, centers, plane, v);
     constexpr int NF = CLS == C_GLCM ? GLCM_NF : CLS == C_GLRLM ? GLRLM_NF : CLS == C_GLSZM ? GLSZM_NF
                        : CLS == C_GLDM ? GLDM_NF : NGTDM_NF;
-    const bool is_center = centers ? centers[(long long)z * plane + rem] != 0 : lev[vi] != 0;
     if (!is_center) {
 #pragma unroll
-      for (int k = 0; k < NF; k++) out[k * fstride + oi] = P.init_value;
+      for (int k = 0; k < NF; k++) out[k * fstride + v.oi] = P.init_value;
       continue;
     }
     uint16_t w[WCAP];
-    load_window<T>(lev, P, z, y, x, w);
+    load_window<T>(lev, P, v.z, v.y, v.x, w);
     double f[NF];
     int st = 0;
     if (CLS == C_GLCM) glcm_voxel<WCAP, WEIGHTED>(w, P, f, &st);
@@ -41,7 +38,7 @@ voxel_features_kernel(const T* __restrict__ lev, const uint8_t* __restrict__ cen
     else if (CLS == C_GLDM) gldm_voxel<WCAP>(w, P, f);
     else ngtdm_voxel<WCAP>(w, P, f);
 #pragma unroll
-    for (int k = 0; k < NF; k++) out[k * fstride + oi] = f[k];
+    for (int k = 0; k < NF; k++) out[k * fstride + v.oi] = f[k];
     if (st && status) atomicOr(status, st);
   }
 }
@@ -95,15 +92,6 @@ pack_levels_kernel(const int32_t* __restrict__ image, const uint8_t* __restrict_
     lev[i] = v;
   }
   if (bad && status) atomicOr(status, 1);
-}
-
-static int grid_for(long long n, int block, int per_sm) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long need = (n + block - 1) / block;
-  long long cap = (long long)sms * per_sm;
-  return (int)(need < cap ? (need < 1 ? 1 : need) : cap);
 }
 
 template <typename T, int WCAP>

@@ -158,7 +158,8 @@ extern "C" long long emul_glcm_pipeline(const uint8_t* lev, int Z, int Y, int X,
     GlcmTask* qp = q.data(); double* rp = res.data(); unsigned* cp = &count;
     emu_launch(3, 256, [=]() { glcm_fast_kernel<1, 256>(lev, nullptr, P, T, out, fstride, za, zb, 0, qp, cp); });
     for (unsigned k = 0; k < count; k++) res[k] = -12345.0;
-    // one launch per size group, as voxel_fast.cu does with B200_GLCM_SPLIT=3 (dense kinds) / the whole kind at once
+    // one launch per size group of the n <= 8 and Lanczos kinds and one for the whole n <= 12 kind: glcm_fast_launch
+    // splits the dense kinds the other way round, so between them both paths of `only` run for both dense kinds
     for (int g = 4; g <= 8; g += 2) emu_launch(2, 128, [=]() { glcm_fast_solve_kernel<0>(lev, P, T, qp, cp, rp, g); });
     emu_launch(2, 128, [=]() { glcm_fast_solve_kernel<1>(lev, P, T, qp, cp, rp, 0); });
     for (int g = 18; g >= 14; g -= 2) emu_launch(2, 128, [=]() { glcm_fast_solve_kernel<2>(lev, P, T, qp, cp, rp, g); });
