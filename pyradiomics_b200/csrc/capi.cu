@@ -51,14 +51,15 @@ static bool force_generic() {
 
 int calculate_matrix_host(int mode, const int32_t* image, const uint8_t* mask, const int* size, int nd,
                           const int* distances, int ndist, int Ng, int Nr, int alpha, int force2D, int force2Ddimension,
-                          int kernelRadius, const int* voxels, int nvox, double* out_host, int* angles_out, int* na_out,
-                          const void* levels_dev = nullptr);
+                          int kernelRadius, const int* voxels, int nvox, double* out_host, int* angles_out);
 int glszm_zones_host(const int32_t* image, const uint8_t* mask, const int* size, int nd, int Ng, int force2D,
                      int force2Ddimension, int kernelRadius, const int* voxels, int nvox, int* max_region_out,
                      void** handle_out, const void* levels_dev = nullptr);
-int segment_tile_matrices(const uint8_t* lev, int nd, int Z, int Y, int X, const int* distances, int ndist, int Ng, int alpha,
-                          int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
-                          int* angles_out, int* na_out, cudaStream_t st);
+int segment_matrices(const void* lev, int level_bytes, int nd, int Z, int Y, int X, const int* distances, int ndist, int Ng,
+                     int alpha, int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
+                     int* angles_out, cudaStream_t st);
+int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X, int Ng, int Nr, int force2D, int force2Ddimension,
+                  double* glrlm_host, int* angles_out, cudaStream_t st);
 int glszm_fill_host(void* handle, int Ng, int max_region, double* out_host);
 void glszm_release(void* handle);
 
@@ -218,13 +219,8 @@ int rb_memcpy2d_async(void* dst, unsigned long long dpitch, const void* src, uns
 int rb_maps_to_f32_dev(const double* src_dev, long long src_pitch, float* dst_dev, long long dst_pitch, long long width,
                        long long height, void* stream) {
   if (width <= 0 || height <= 0) return RB_OK;
-  const long long total = width * height;
-  long long blocks = (total + 255) / 256;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (blocks > sms * 16LL) blocks = sms * 16LL;
-  maps_to_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(src_dev, src_pitch, dst_dev, dst_pitch, width, height);
+  maps_to_f32_kernel<<<grid_for(width * height, 256, 16), 256, 0, (cudaStream_t)stream>>>(src_dev, src_pitch, dst_dev,
+                                                                                          dst_pitch, width, height);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
@@ -235,64 +231,58 @@ int rb_voxel_features_host(int cls, const int32_t* image, const uint8_t* mask, i
   const long long n = (long long)Z * Y * X;
   const int nf = kNumFeatures[cls];
   const int lb = rb_level_bytes(settings->Ng);
-  int32_t* d_img = NULL; uint8_t* d_msk = NULL; void* d_lev = NULL; double* d_out = NULL; int* d_status = NULL;
-  uint32_t* d_alive = NULL;
-  int rc = RB_OK;
-  auto cleanup = [&]() { cudaFree(d_img); cudaFree(d_msk); cudaFree(d_lev); cudaFree(d_out); cudaFree(d_status); cudaFree(d_alive); };
-#define RB_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { cleanup(); return fail(_e == cudaErrorMemoryAllocation ? RB_ERR_NOMEM : RB_ERR_CUDA, "%s: %s", #x, cudaGetErrorString(_e)); } } while (0)
-  RB_TRY(cudaMalloc(&d_img, n * 4));
-  RB_TRY(cudaMalloc(&d_msk, n));
-  RB_TRY(cudaMalloc(&d_lev, n * lb));
-  RB_TRY(cudaMalloc(&d_out, sizeof(double) * n * nf));
-  RB_TRY(cudaMalloc(&d_status, 2 * sizeof(int)));
-  RB_TRY(cudaMalloc(&d_alive, RB_ALIVE_WORDS * 4));
-  RB_TRY(cudaMemsetAsync(d_status, 0, 2 * sizeof(int), 0));
-  RB_TRY(cudaMemsetAsync(d_alive, 0, RB_ALIVE_WORDS * 4, 0));
-  RB_TRY(cudaMemcpyAsync(d_img, image, n * 4, cudaMemcpyHostToDevice, 0));
-  RB_TRY(cudaMemcpyAsync(d_msk, mask, n, cudaMemcpyHostToDevice, 0));
-  rc = rb_pack_levels_dev(d_img, d_msk, n, settings->Ng, d_lev, NULL, d_status, 0);
+  DevBuf img, msk, lev, out, status, alive_dev;
+  RB_CUDA(img.alloc(n * 4));
+  RB_CUDA(msk.alloc(n));
+  RB_CUDA(lev.alloc(n * lb));
+  RB_CUDA(out.alloc(sizeof(double) * n * nf));
+  RB_CUDA(status.alloc(2 * sizeof(int)));
+  RB_CUDA(alive_dev.alloc(RB_ALIVE_WORDS * 4));
+  RB_CUDA(cudaMemsetAsync(status.p, 0, 2 * sizeof(int), 0));
+  RB_CUDA(cudaMemsetAsync(alive_dev.p, 0, RB_ALIVE_WORDS * 4, 0));
+  RB_CUDA(cudaMemcpyAsync(img.p, image, n * 4, cudaMemcpyHostToDevice, 0));
+  RB_CUDA(cudaMemcpyAsync(msk.p, mask, n, cudaMemcpyHostToDevice, 0));
+  int rc = rb_pack_levels_dev(img.as<int32_t>(), msk.as<uint8_t>(), n, settings->Ng, lev.p, NULL, status.as<int>(), 0);
+  if (rc) return rc;
   uint32_t alive[RB_ALIVE_WORDS];
-  if (rc == RB_OK && cls == RB_GLCM) {
-    rc = rb_glcm_alive_angles_dev(d_lev, lb, NULL, Z, Y, X, settings, d_alive, 0);
-    if (rc == RB_OK) RB_TRY(cudaMemcpy(alive, d_alive, sizeof alive, cudaMemcpyDeviceToHost));
+  if (cls == RB_GLCM) {
+    rc = rb_glcm_alive_angles_dev(lev.p, lb, NULL, Z, Y, X, settings, alive_dev.as<uint32_t>(), 0);
+    if (rc) return rc;
+    RB_CUDA(cudaMemcpy(alive, alive_dev.p, sizeof alive, cudaMemcpyDeviceToHost));
   }
-  if (rc == RB_OK)
-    rc = rb_voxel_features_dev(cls, d_lev, lb, NULL, Z, Y, X, 0, Z, settings, cls == RB_GLCM ? alive : NULL, d_out, 0, n, 0,
-                               d_status + 1, 0);
-  if (rc == RB_OK) {
-    int st[2] = {0, 0};
-    RB_TRY(cudaMemcpy(st, d_status, sizeof st, cudaMemcpyDeviceToHost));
-    if (st[0] & 1) rc = fail(RB_ERR_LEVEL_RANGE, "gray level outside 1..Ng inside the mask");
-    else if (st[1] & 2) rc = fail(RB_ERR_UNSUPPORTED, "weighted GLCM entry list overflow");
-    else RB_TRY(cudaMemcpy(maps, d_out, sizeof(double) * n * nf, cudaMemcpyDeviceToHost));
-  }
-#undef RB_TRY
-  cleanup();
-  return rc;
+  rc = rb_voxel_features_dev(cls, lev.p, lb, NULL, Z, Y, X, 0, Z, settings, cls == RB_GLCM ? alive : NULL, out.p, 0, n, 0,
+                             status.as<int>() + 1, 0);
+  if (rc) return rc;
+  int st[2] = {0, 0};
+  RB_CUDA(cudaMemcpy(st, status.p, sizeof st, cudaMemcpyDeviceToHost));
+  if (st[0] & 1) return fail(RB_ERR_LEVEL_RANGE, "gray level outside 1..Ng inside the mask");
+  if (st[1] & 2) return fail(RB_ERR_UNSUPPORTED, "weighted GLCM entry list overflow");
+  RB_CUDA(cudaMemcpy(maps, out.p, sizeof(double) * n * nf, cudaMemcpyDeviceToHost));
+  return RB_OK;
 }
 
 int rb_calculate_glcm(const int32_t* image, const uint8_t* mask, const int* size, int nd, const int* distances, int ndist,
                       int Ng, int force2D, int force2Ddimension, int kernelRadius, const int* voxels, int nvox,
                       double* glcm, int* angles) {
   return calculate_matrix_host(0, image, mask, size, nd, distances, ndist, Ng, 0, 0, force2D, force2Ddimension,
-                               kernelRadius, voxels, nvox, glcm, angles, NULL);
+                               kernelRadius, voxels, nvox, glcm, angles);
 }
 int rb_calculate_glrlm(const int32_t* image, const uint8_t* mask, const int* size, int nd, int Ng, int Nr, int force2D,
                        int force2Ddimension, int kernelRadius, const int* voxels, int nvox, double* glrlm, int* angles) {
   return calculate_matrix_host(3, image, mask, size, nd, NULL, 0, Ng, Nr, 0, force2D, force2Ddimension, kernelRadius,
-                               voxels, nvox, glrlm, angles, NULL);
+                               voxels, nvox, glrlm, angles);
 }
 int rb_calculate_gldm(const int32_t* image, const uint8_t* mask, const int* size, int nd, const int* distances, int ndist,
                       int Ng, int alpha, int force2D, int force2Ddimension, int kernelRadius, const int* voxels, int nvox,
                       double* gldm) {
   return calculate_matrix_host(1, image, mask, size, nd, distances, ndist, Ng, 0, alpha, force2D, force2Ddimension,
-                               kernelRadius, voxels, nvox, gldm, NULL, NULL);
+                               kernelRadius, voxels, nvox, gldm, NULL);
 }
 int rb_calculate_ngtdm(const int32_t* image, const uint8_t* mask, const int* size, int nd, const int* distances,
                        int ndist, int Ng, int force2D, int force2Ddimension, int kernelRadius, const int* voxels,
                        int nvox, double* ngtdm) {
   return calculate_matrix_host(2, image, mask, size, nd, distances, ndist, Ng, 0, 0, force2D, force2Ddimension,
-                               kernelRadius, voxels, nvox, ngtdm, NULL, NULL);
+                               kernelRadius, voxels, nvox, ngtdm, NULL);
 }
 // ---- segment-mode matrices from a device-resident packed level volume (no host round trip of the image)
 int rb_segment_texture_dev(const void* levels_dev, int level_bytes, const int* size, int nd, const int* distances, int ndist,
@@ -300,25 +290,15 @@ int rb_segment_texture_dev(const void* levels_dev, int level_bytes, const int* s
                            int* angles) {
   if (!levels_dev || !size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "levels / size");
   if (level_bytes != rb_level_bytes(Ng)) return fail(RB_ERR_ARG, "level_bytes does not match Ng");
-  int dmax = 0;
-  for (int i = 0; i < ndist; i++) dmax = distances[i] > dmax ? distances[i] : dmax;
-  const int Z = nd == 3 ? size[0] : 1, Y = size[nd - 2], X = size[nd - 1];
-  if (level_bytes == 1 && dmax <= 3) {
-    const int rc = segment_tile_matrices((const uint8_t*)levels_dev, nd, Z, Y, X, distances, ndist, Ng, alpha, force2D,
-                                         force2Ddimension, glcm, gldm, ngtdm, angles, NULL, 0);
-    if (rc != RB_ERR_UNSUPPORTED) return rc;
-  }
-  int rc = RB_OK;        // 16-bit levels / long offsets / very many levels: one class at a time through round 1's kernels
-  if (glcm) rc = calculate_matrix_host(0, NULL, NULL, size, nd, distances, ndist, Ng, 0, 0, force2D, force2Ddimension, 0, NULL, 1, glcm, angles, NULL, levels_dev);
-  if (!rc && gldm) rc = calculate_matrix_host(1, NULL, NULL, size, nd, distances, ndist, Ng, 0, alpha, force2D, force2Ddimension, 0, NULL, 1, gldm, NULL, NULL, levels_dev);
-  if (!rc && ngtdm) rc = calculate_matrix_host(2, NULL, NULL, size, nd, distances, ndist, Ng, 0, 0, force2D, force2Ddimension, 0, NULL, 1, ngtdm, NULL, NULL, levels_dev);
-  return rc;
+  return segment_matrices(levels_dev, level_bytes, nd, nd == 3 ? size[0] : 1, size[nd - 2], size[nd - 1], distances, ndist, Ng,
+                          alpha, force2D, force2Ddimension, glcm, gldm, ngtdm, angles, 0);
 }
 int rb_segment_glrlm_dev(const void* levels_dev, int level_bytes, const int* size, int nd, int Ng, int Nr, int force2D,
                          int force2Ddimension, double* glrlm, int* angles) {
   if (!levels_dev || !size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "levels / size");
   if (level_bytes != rb_level_bytes(Ng)) return fail(RB_ERR_ARG, "level_bytes does not match Ng");
-  return calculate_matrix_host(3, NULL, NULL, size, nd, NULL, 0, Ng, Nr, 0, force2D, force2Ddimension, 0, NULL, 1, glrlm, angles, NULL, levels_dev);
+  return segment_glrlm(levels_dev, level_bytes, nd, nd == 3 ? size[0] : 1, size[nd - 2], size[nd - 1], Ng, Nr, force2D,
+                       force2Ddimension, glrlm, angles, 0);
 }
 int rb_segment_glszm_dev(const void* levels_dev, int level_bytes, const int* size, int nd, int Ng, int force2D,
                          int force2Ddimension, int* max_region, void** handle) {
@@ -448,13 +428,12 @@ int rb_calculate_coefficients(const char* mask, const int* size, const int* stri
     for (int y = 0; y < Y; y++)
       for (int x = 0; x < X; x++)
         packed[((size_t)z * Y + y) * X + x] = mask[(long long)z * strides[0] + (long long)y * strides[1] + (long long)x * strides[2]] != 0;
-  uint8_t* d = nullptr;
-  RB_CUDA(cudaMalloc(&d, n));
-  cudaError_t e = cudaMemcpy(d, packed.data(), n, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_CUDA, "shape: %s", cudaGetErrorString(e)); }
+  DevBuf d;
+  RB_CUDA(d.alloc(n));
+  cudaError_t e = cudaMemcpy(d.p, packed.data(), n, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) return fail(RB_ERR_CUDA, "shape: %s", cudaGetErrorString(e));
   double out7[7];
-  const int rc = shape_coefficients_dev(d, Z, Y, X, (long long)Y * X, X, 1, spacing, out7, 0);
-  cudaFree(d);
+  const int rc = shape_coefficients_dev(d.as<uint8_t>(), Z, Y, X, (long long)Y * X, X, 1, spacing, out7, 0);
   if (rc) return rc;
   *surfaceArea = out7[0]; *volume = out7[1];
   for (int q = 0; q < 4; q++) diameters[q] = out7[2 + q];
@@ -470,13 +449,12 @@ int rb_calculate_coefficients2D(const char* mask, const int* size, const int* st
   std::vector<uint8_t> h((size_t)Y * X);
   for (int y = 0; y < Y; y++)
     for (int x = 0; x < X; x++) h[(size_t)y * X + x] = mask[(long long)y * strides[0] + (long long)x * strides[1]] != 0;
-  uint8_t* d = NULL;
-  RB_CUDA(cudaMalloc(&d, h.size()));
-  cudaError_t e = cudaMemcpy(d, h.data(), h.size(), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_CUDA, "shape2D upload: %s", cudaGetErrorString(e)); }
+  DevBuf d;
+  RB_CUDA(d.alloc(h.size()));
+  cudaError_t e = cudaMemcpy(d.p, h.data(), h.size(), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) return fail(RB_ERR_CUDA, "shape2D upload: %s", cudaGetErrorString(e));
   double out4[4];
-  const int rc = shape2d_coefficients_dev(d, Y, X, X, 1, spacing, out4, 0);
-  cudaFree(d);
+  const int rc = shape2d_coefficients_dev(d.as<uint8_t>(), Y, X, X, 1, spacing, out4, 0);
   if (rc) return rc;
   *perimeter = out4[0]; *surface = out4[1]; *diameter = out4[2];
   return RB_OK;

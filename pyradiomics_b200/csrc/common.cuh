@@ -1,5 +1,5 @@
-// Shared host-side plumbing of libb200radiomics: error state, CUDA call checking and the per-device launch state
-// (table blocks, SM count, occupancy, kernel attributes).
+// Shared host-side plumbing of libb200radiomics: error state, CUDA call checking, temporary device buffers and the
+// per-device launch state (table blocks, SM count, occupancy, kernel attributes).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdio.h>
@@ -47,6 +47,18 @@ const T* device_table(Build build, int key = 0) {
   if (cudaMemcpy(d, h.get(), sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(d); return nullptr; }
   return cache[{dev, key}] = d;
 }
+
+// One temporary device buffer, freed (cudaFree, synchronous) when it goes out of scope.  Wrap alloc in RB_CUDA so an
+// allocation failure reports RB_ERR_NOMEM.
+struct DevBuf {
+  void* p = nullptr;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
+  cudaError_t alloc(size_t bytes) { return cudaMalloc(&p, bytes ? bytes : 1); }
+  template <typename U> U* as() const { return (U*)p; }
+};
 
 // SM count of the current device (132 if it cannot be queried)
 inline int sm_count() {

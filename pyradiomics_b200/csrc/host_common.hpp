@@ -47,6 +47,12 @@ inline int generate_angles(const int* size, int nd, const int* distances, int nd
   return na;
 }
 
+// Up to NA_MAX (dz, dy, dx) offsets, passed to the matrix kernels by value
+struct AngleSet {
+  int na;
+  int8_t a[NA_MAX][3];
+};
+
 enum Weighting { W_NONE = 0, W_INFINITY = 1, W_EUCLIDEAN = 2, W_MANHATTAN = 3, W_NO_WEIGHTING = 4 };
 enum TexClass { C_GLCM = 0, C_GLRLM = 1, C_GLSZM = 2, C_GLDM = 3, C_NGTDM = 4 };
 static const int kNumFeatures[5] = {GLCM_NF, GLRLM_NF, GLSZM_NF, GLDM_NF, NGTDM_NF};

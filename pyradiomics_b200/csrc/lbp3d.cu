@@ -32,14 +32,6 @@ lbp3d_kernel(const double* __restrict__ coef, const void* __restrict__ img, int 
   }
 }
 
-static int grid_lbp(long long n, int block, int per_sm) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long need = (n + block - 1) / block, cap = (long long)sms * per_sm;
-  return (int)(need < cap ? (need < 1 ? 1 : need) : cap);
-}
-
 int lbp3d_launch(const void* img, int img_dt, int sample_dt, const uint8_t* roi, int Z, int Y, int X, const double* vertices,
                  int nv, const double* harmonics, int levels, double* coeff_scratch, double* out, cudaStream_t st) {
   if (!img || !roi || !vertices || !harmonics || !coeff_scratch || !out) return fail(RB_ERR_ARG, "lbp3d: null argument");
@@ -63,11 +55,11 @@ int lbp3d_launch(const void* img, int img_dt, int sample_dt, const uint8_t* roi,
     }
   }
   const long long n = (long long)Z * Y * X;
-  lbp3d_to_f64_kernel<<<grid_lbp(n, 256, 8), 256, 0, st>>>(img, img_dt, n, coeff_scratch);
+  lbp3d_to_f64_kernel<<<grid_for(n, 256, 8), 256, 0, st>>>(img, img_dt, n, coeff_scratch);
   RB_LAUNCH_CHECK();
   const int rc = bspline_prefilter_launch(coeff_scratch, Z, Y, X, st, true);
   if (rc) return rc;
-  lbp3d_kernel<<<grid_lbp(n, 128, 16), 128, 0, st>>>(coeff_scratch, img, img_dt, roi, Z, Y, X, T, out);
+  lbp3d_kernel<<<grid_for(n, 128, 16), 128, 0, st>>>(coeff_scratch, img, img_dt, roi, Z, Y, X, T, out);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }

@@ -177,14 +177,6 @@ resample_kernel(const void* __restrict__ src, int src_dt, const __grid_constant_
   }
 }
 
-static int grid_rs(long long n, int block, int per_sm) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long need = (n + block - 1) / block, cap = (long long)sms * per_sm;
-  return (int)(need < cap ? (need < 1 ? 1 : need) : cap);
-}
-
 template <bool EXACT>
 static int bspline_prefilter_run(double* coeffs, int Z, int Y, int X, cudaStream_t st) {
   if (Z < 1 || Y < 1 || X < 1) return fail(RB_ERR_ARG, "empty volume");
@@ -194,13 +186,13 @@ static int bspline_prefilter_run(double* coeffs, int Z, int Y, int X, cudaStream
     const size_t sh = (size_t)4 * 32 * (X + 1) * sizeof(double);
     if (sh <= 200 * 1024) {
       cudaFuncSetAttribute(bspline_prefilter_x_kernel<EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh);
-      bspline_prefilter_x_kernel<EXACT><<<grid_rs((n / X + 31) / 32, 4, 4), 128, sh, st>>>(coeffs, n / X, X);
+      bspline_prefilter_x_kernel<EXACT><<<grid_for((n / X + 31) / 32, 4, 4), 128, sh, st>>>(coeffs, n / X, X);
     } else {
-      bspline_prefilter_kernel<EXACT><<<grid_rs(n / X, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 2);
+      bspline_prefilter_kernel<EXACT><<<grid_for(n / X, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 2);
     }
   }
-  if (Y > 1) bspline_prefilter_kernel<EXACT><<<grid_rs(n / Y, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 1);
-  if (Z > 1) bspline_prefilter_kernel<EXACT><<<grid_rs(n / Z, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 0);
+  if (Y > 1) bspline_prefilter_kernel<EXACT><<<grid_for(n / Y, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 1);
+  if (Z > 1) bspline_prefilter_kernel<EXACT><<<grid_for(n / Z, 128, 8), 128, 0, st>>>(coeffs, Z, Y, X, 0);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
@@ -219,7 +211,7 @@ int resample_launch(const void* src, int src_dt, const int* in_size, void* dst, 
   for (int d = 0; d < 3; d++) { G.start[d] = start[d]; G.step[d] = step[d]; }
   const long long n = (long long)G.oz * G.oy * G.ox;
   if (n <= 0) return RB_OK;
-  resample_kernel<<<grid_rs(n, 256, 8), 256, 0, st>>>(src, src_dt, G, interp, default_value, dst, dst_dt);
+  resample_kernel<<<grid_for(n, 256, 8), 256, 0, st>>>(src, src_dt, G, interp, default_value, dst, dst_dt);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }

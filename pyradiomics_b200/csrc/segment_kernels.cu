@@ -1,19 +1,24 @@
 // Segment-based texture matrices of ONE ROI from a device-resident packed level volume (reference
 // radiomics/src/cmatrices.c: calculate_glcm :4-92, calculate_gldm :660-754, calculate_ngtdm :543-658, calculate_glrlm
-// :299-541, calculate_glszm :94-279).  Round-2 rebuild of the segment path on the north-star design:
+// :299-541).
 //
-//   seg_tile_kernel   GLCM + GLDM + NGTDM in ONE pass: a CTA stages a (TZ+2H) x (TY+2H) x 96-byte box of the level
-//                     volume in shared memory -- by TMA (cp.async.bulk.tensor.3d, out-of-volume coordinates are
-//                     zero-filled by the hardware = "unmasked", double-buffered on an mbarrier) when the row pitch
-//                     allows a tensor map, else by cooperative loads -- walks the 13 / 26 offsets in shared memory
-//                     and accumulates into per-CTA shared-memory histograms (GLCM Ng x Ng x Na when it fits), flushed
-//                     once per CTA with coalesced atomics.
-//   seg_glrlm_kernel  every voxel that ENDS a run (successor outside / unmasked / another level) walks back to the run's
-//                     start: all voxels work, loads coalesce along x (round 1: one thread per LINE start walked the
-//                     whole line -- most of the volume's threads idle).  The reference's "angle without
-//                     a line of two voxels loses its length-1 column" rule (cmatrices.c:524-534) comes from a
-//                     pigeonhole count: some line holds two masked voxels <=> #masked voxels > #lines that hold any.
-//   ccl_*             GLSZM zones: union-find with the tile's equal-level neighbours merged in shared memory first.
+//   segment_matrices       GLCM + GLDM + NGTDM in one pass, by one of two kernels with the same flags and accumulators:
+//     seg_tile_kernel      8-bit levels, offsets up to 3 and histograms that fit shared memory: a CTA stages a
+//                          (TZ+2H) x (TY+2H) x 96-byte box of the level volume in shared memory -- by TMA
+//                          (cp.async.bulk.tensor.3d, out-of-volume coordinates are zero-filled by the hardware =
+//                          "unmasked", double-buffered on an mbarrier) when the row pitch allows a tensor map, else by
+//                          cooperative loads -- walks the 13 / 26 offsets in shared memory and accumulates into per-CTA
+//                          shared-memory histograms (GLCM Ng x Ng x Na when it fits), flushed once per CTA with
+//                          coalesced atomics.
+//     seg_direct_kernel    everything else (16-bit levels, longer offsets, more levels): one thread per voxel, global
+//                          loads, the GLCM histogram privatised in shared memory when it fits.
+//   segment_glrlm          seg_glrlm_ends_kernel: every voxel that ENDS a run (successor outside / unmasked / another
+//                          level) walks back to the run's start: all voxels work, loads coalesce along x.  The
+//                          reference's "angle without a line of two voxels loses its length-1 column" rule
+//                          (cmatrices.c:524-534) comes from a pigeonhole count: some line holds two masked voxels <=>
+//                          #masked voxels > #lines that hold any.
+// Integer counts are exact; NGTDM's s_i is accumulated as integers T[g][count] += |g*count - sum| and divided by count
+// once at the end, so both kernels give bit-identical matrices.
 #include <cuda.h>
 
 #include <vector>
@@ -164,6 +169,53 @@ seg_tile_kernel(const uint8_t* __restrict__ lev, SegVol V, const __grid_constant
   if (flags & 4) for (int i = tid; i < Ng * ng_cols; i += ST_THREADS) if (s_ng[i]) atomicAdd(&ngtdm_acc[i], s_ng[i]);
 }
 
+// Same flags and accumulator layouts as seg_tile_kernel (A = the unidirectional offsets; GLDM / NGTDM also use their
+// mirrors).  The GLCM histogram lives in shared memory when glcm_shared.
+template <typename T>
+__global__ void __launch_bounds__(256)
+seg_direct_kernel(const T* __restrict__ lev, SegVol V, const __grid_constant__ AngleSet A, int Ng, int alpha, int flags,
+                  int glcm_shared, unsigned* __restrict__ glcm_hist, unsigned* __restrict__ gldm_hist,
+                  unsigned long long* __restrict__ ngtdm_acc) {
+  extern __shared__ unsigned s_glcm[];
+  const int n_gl = glcm_shared ? Ng * Ng * A.na : 0;
+  for (int i = threadIdx.x; i < n_gl; i += blockDim.x) s_glcm[i] = 0;
+  __syncthreads();
+  unsigned* gl = glcm_shared ? s_glcm : glcm_hist;
+  const int ng_cols = 2 * A.na + 2, gd_cols = 2 * (2 * A.na) + 1;
+  const long long n = (long long)V.Z * V.Y * V.X, plane = (long long)V.Y * V.X;
+  auto in = [&](int z, int y, int x) { return z >= 0 && z < V.Z && y >= 0 && y < V.Y && x >= 0 && x < V.X; };
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x) {
+    const int gi = lev[t];
+    if (!gi) continue;
+    const int z = (int)(t / plane), rem = (int)(t % plane), y = rem / V.X, x = rem % V.X;
+    int dep = 0, cnt = 0, sum = 0;
+    for (int a = 0; a < A.na; a++) {
+      const int dz = A.a[a][0], dy = A.a[a][1], dx = A.a[a][2];
+      const long long off = dz * V.pitch_z + dy * V.pitch_y + dx;
+      const int gj = in(z + dz, y + dy, x + dx) ? lev[t + off] : 0;
+      if ((flags & 1) && gj) atomicAdd(&gl[((size_t)(gi - 1) * Ng + (gj - 1)) * A.na + a], 1u);
+      if (flags & 6) {
+        const int gr = in(z - dz, y - dy, x - dx) ? lev[t - off] : 0;
+        if (gj) { cnt++; sum += gj; const int d = gi > gj ? gi - gj : gj - gi; dep += d <= alpha; }
+        if (gr) { cnt++; sum += gr; const int d = gi > gr ? gi - gr : gr - gi; dep += d <= alpha; }
+      }
+    }
+    if (flags & 2) atomicAdd(&gldm_hist[(gi - 1) * gd_cols + dep], 1u);
+    if (flags & 4) {
+      atomicAdd(&ngtdm_acc[(gi - 1) * ng_cols], 1ull);
+      if (cnt) {
+        long long num = (long long)gi * cnt - sum;
+        if (num < 0) num = -num;
+        if (num) atomicAdd(&ngtdm_acc[(gi - 1) * ng_cols + 1 + cnt], (unsigned long long)num);
+      }
+    }
+  }
+  if (glcm_shared) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_gl; i += blockDim.x) if (s_glcm[i]) atomicAdd(&glcm_hist[i], s_glcm[i]);
+  }
+}
+
 // ---- GLRLM by run ends ----------------------------------------------------------------------------------------------
 // hist[((g-1)*Nr + len-1)*na + a]; short runs (len <= RL_SH) of every (level, angle) are counted in shared memory first.
 constexpr int RL_SH = 4;
@@ -259,32 +311,8 @@ static bool seg_tma_enabled() {
   return !(e && e[0] == '0');
 }
 
-// GLCM (flag 1) / GLDM (2) / NGTDM (4) of one packed uint8 level volume in one pass; outputs are HOST float64 buffers in
-// the reference layouts (NULL = not wanted).  3-D volumes or 2-D (Z = 1).
-int segment_tile_matrices(const uint8_t* lev, int nd, int Z, int Y, int X, const int* distances, int ndist, int Ng, int alpha,
-                          int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
-                          int* angles_out, int* na_out, cudaStream_t st) {
-  int size[3] = {Z, Y, X};
-  const int* sz = nd == 3 ? size : size + 1;
-  std::vector<int> ang;
-  const int f2 = force2D ? force2Ddimension : -1;
-  const int na = generate_angles(sz, nd, distances, ndist, false, f2, ang);
-  if (na <= 0) return fail(RB_ERR_ARG, "Error getting angle count.");
-  if (na > NW_MAX) return fail(RB_ERR_UNSUPPORTED, "more than %d angles", NW_MAX);
-  SegAngles A;
-  A.na = na;
-  int H = 0;
-  for (int a = 0; a < na; a++)
-    for (int d = 0; d < 3; d++) {
-      const int v = d < 3 - nd ? 0 : ang[a * nd + d - (3 - nd)];
-      A.a[a][d] = (int8_t)v;
-      H = v > H ? v : (-v > H ? -v : H);
-    }
-  if (na_out) *na_out = na;
-  if (angles_out) memcpy(angles_out, ang.data(), sizeof(int) * ang.size());
-  const int flags = (glcm_host ? 1 : 0) | (gldm_host ? 2 : 0) | (ngtdm_host ? 4 : 0);
-  if (!flags) return RB_OK;
-  SegTileGeom G;
+// seg_tile_kernel's plan for a volume, or 0 when its shared memory would exceed 220 KB
+static size_t tile_plan(int Z, int Y, int X, int H, int Ng, int na, int flags, SegTileGeom& G) {
   G.H = H;
   if (Z == 1) { G.tz = 1; G.ty = 32; } else { G.tz = 4; G.ty = 8; }
   G.bx = ST_BX; G.by = G.ty + 2 * H; G.bz = G.tz + 2 * H;
@@ -294,25 +322,21 @@ int segment_tile_matrices(const uint8_t* lev, int nd, int Z, int Y, int X, const
   size_t smem = 2 * (size_t)box_al + ((flags & 4) ? n_ng * 8 : 0) + ((flags & 2) ? n_gd * 4 : 0);
   G.glcm_shared = (flags & 1) && smem + n_gl * 4 <= 200 * 1024;
   if (G.glcm_shared) smem += n_gl * 4;
-  if (smem > 220 * 1024) return fail(RB_ERR_UNSUPPORTED, "segment tile kernel: Ng=%d with %d angles does not fit shared memory", Ng, na);
-  unsigned *d_gl = nullptr, *d_gd = nullptr;
-  unsigned long long* d_ng = nullptr;
-  double* d_out = nullptr;
-  const size_t n_out = n_gl > n_gd ? n_gl : n_gd;
-  auto cleanup = [&]() { cudaFree(d_gl); cudaFree(d_gd); cudaFree(d_ng); cudaFree(d_out); };
-#define SEG_TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { cleanup(); return fail(_e == cudaErrorMemoryAllocation ? RB_ERR_NOMEM : RB_ERR_CUDA, "%s: %s", #x, cudaGetErrorString(_e)); } } while (0)
-  if (flags & 1) { SEG_TRY(cudaMalloc(&d_gl, n_gl * 4)); SEG_TRY(cudaMemsetAsync(d_gl, 0, n_gl * 4, st)); }
-  if (flags & 2) { SEG_TRY(cudaMalloc(&d_gd, n_gd * 4)); SEG_TRY(cudaMemsetAsync(d_gd, 0, n_gd * 4, st)); }
-  if (flags & 4) { SEG_TRY(cudaMalloc(&d_ng, n_ng * 8)); SEG_TRY(cudaMemsetAsync(d_ng, 0, n_ng * 8, st)); }
-  SEG_TRY(cudaMalloc(&d_out, (n_out > 3 * (size_t)Ng ? n_out : 3 * (size_t)Ng) * 8));
-  SegVol V{Z, Y, X, (long long)X, (long long)Y * X};
+  return smem > 220 * 1024 ? 0 : smem;
+}
+
+static int launch_tile(const uint8_t* lev, SegVol V, const AngleSet& A, const SegTileGeom& G, size_t smem, int Ng, int alpha,
+                       int flags, unsigned* d_gl, unsigned* d_gd, unsigned long long* d_ng, cudaStream_t st) {
+  SegAngles S;
+  S.na = A.na;
+  memcpy(S.a, A.a, sizeof(S.a[0]) * A.na);
   // tensor map: needs a 16-byte aligned base and row / plane pitches that are multiples of 16 bytes
   CUtensorMap tmap;
   memset(&tmap, 0, sizeof tmap);
-  bool tma = seg_tma_enabled() && (X % 16 == 0) && (((uintptr_t)lev & 15) == 0);
+  bool tma = seg_tma_enabled() && (V.X % 16 == 0) && (((uintptr_t)lev & 15) == 0);
   if (tma) {
-    const cuuint64_t gdim[3] = {(cuuint64_t)X, (cuuint64_t)Y, (cuuint64_t)Z};
-    const cuuint64_t gstr[2] = {(cuuint64_t)X, (cuuint64_t)X * (cuuint64_t)Y};
+    const cuuint64_t gdim[3] = {(cuuint64_t)V.X, (cuuint64_t)V.Y, (cuuint64_t)V.Z};
+    const cuuint64_t gstr[2] = {(cuuint64_t)V.X, (cuuint64_t)V.X * (cuuint64_t)V.Y};
     const cuuint32_t bdim[3] = {(cuuint32_t)G.bx, (cuuint32_t)G.by, (cuuint32_t)G.bz};
     const cuuint32_t estr[3] = {1, 1, 1};
     // the driver entry point is looked up at run time: the library must load on a box without libcuda (the CPU tests)
@@ -339,36 +363,101 @@ int segment_tile_matrices(const uint8_t* lev, int nd, int Z, int Y, int X, const
   int grid = sm_count() * per_sm;
   if (grid > ntiles) grid = ntiles;
   if (tma) {
-    SEG_TRY(cudaFuncSetAttribute(seg_tile_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    seg_tile_kernel<true><<<grid, ST_THREADS, smem, st>>>(lev, V, A, G, Ng, alpha, flags, tmap, d_gl, d_gd, d_ng);
+    RB_CUDA(cudaFuncSetAttribute(seg_tile_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    seg_tile_kernel<true><<<grid, ST_THREADS, smem, st>>>(lev, V, S, G, Ng, alpha, flags, tmap, d_gl, d_gd, d_ng);
   } else {
-    SEG_TRY(cudaFuncSetAttribute(seg_tile_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    seg_tile_kernel<false><<<grid, ST_THREADS, smem, st>>>(lev, V, A, G, Ng, alpha, flags, tmap, d_gl, d_gd, d_ng);
+    RB_CUDA(cudaFuncSetAttribute(seg_tile_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    seg_tile_kernel<false><<<grid, ST_THREADS, smem, st>>>(lev, V, S, G, Ng, alpha, flags, tmap, d_gl, d_gd, d_ng);
   }
-  SEG_TRY(cudaGetLastError());
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+
+template <typename T>
+static int launch_direct(const T* lev, SegVol V, const AngleSet& A, int Ng, int alpha, int flags, unsigned* d_gl,
+                         unsigned* d_gd, unsigned long long* d_ng, cudaStream_t st) {
+  const long long n = (long long)V.Z * V.Y * V.X;
+  if (n <= 0 || n >= (1ll << 31)) return fail(RB_ERR_UNSUPPORTED, "volume must have 1..2^31-1 voxels");
+  const size_t sh = (size_t)Ng * Ng * A.na * 4;
+  const int glcm_shared = (flags & 1) && sh <= 160 * 1024;
+  if (glcm_shared) RB_CUDA(cudaFuncSetAttribute(seg_direct_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
+  seg_direct_kernel<T><<<grid_for(n, 256, glcm_shared ? 1 : 8), 256, glcm_shared ? sh : 0, st>>>(lev, V, A, Ng, alpha, flags,
+                                                                                             glcm_shared, d_gl, d_gd, d_ng);
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+
+// GLCM / GLDM / NGTDM of one packed level volume (uint8 or uint16) in one pass; outputs are HOST float64 buffers in the
+// reference layouts (NULL = not wanted), angles_out gets the unidirectional offsets.  3-D volumes or 2-D (Z = 1).
+int segment_matrices(const void* lev, int level_bytes, int nd, int Z, int Y, int X, const int* distances, int ndist, int Ng,
+                     int alpha, int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
+                     int* angles_out, cudaStream_t st) {
+  int size[3] = {Z, Y, X};
+  const int* sz = nd == 3 ? size : size + 1;
+  std::vector<int> ang;
+  const int na = generate_angles(sz, nd, distances, ndist, false, force2D ? force2Ddimension : -1, ang);
+  if (na <= 0) return fail(RB_ERR_ARG, "Error getting angle count.");
+  if (Ng < 1 || Ng > 65535) return fail(RB_ERR_UNSUPPORTED, "Ng=%d outside 1..65535", Ng);
+  // GLCM counts the na offsets, GLDM / NGTDM each offset and its mirror
+  const int na_max = (gldm_host || ngtdm_host) ? NA_MAX / 2 : NA_MAX;
+  if (na > na_max) return fail(RB_ERR_UNSUPPORTED, "more than %d angles", NA_MAX);
+  if (angles_out) memcpy(angles_out, ang.data(), sizeof(int) * ang.size());
+  const int flags = (glcm_host ? 1 : 0) | (gldm_host ? 2 : 0) | (ngtdm_host ? 4 : 0);
+  if (!flags) return RB_OK;
+  AngleSet A;
+  A.na = na;
+  int H = 0;
+  for (int a = 0; a < na; a++)
+    for (int d = 0; d < 3; d++) {
+      const int v = d < 3 - nd ? 0 : ang[a * nd + d - (3 - nd)];
+      A.a[a][d] = (int8_t)v;
+      H = v > H ? v : (-v > H ? -v : H);
+    }
+  const size_t n_gl = (size_t)Ng * Ng * na, n_gd = (size_t)Ng * (2 * (2 * na) + 1), n_ng = (size_t)Ng * (2 * na + 2);
+  DevBuf gl, gd, ng, out;
+  if (flags & 1) { RB_CUDA(gl.alloc(n_gl * 4)); RB_CUDA(cudaMemsetAsync(gl.p, 0, n_gl * 4, st)); }
+  if (flags & 2) { RB_CUDA(gd.alloc(n_gd * 4)); RB_CUDA(cudaMemsetAsync(gd.p, 0, n_gd * 4, st)); }
+  if (flags & 4) { RB_CUDA(ng.alloc(n_ng * 8)); RB_CUDA(cudaMemsetAsync(ng.p, 0, n_ng * 8, st)); }
+  // float64 staging for the largest requested matrix only: an unrequested GLCM at 16-bit Ng would be gigabytes
+  size_t n_out = 3 * (size_t)Ng;
+  if ((flags & 1) && n_gl > n_out) n_out = n_gl;
+  if ((flags & 2) && n_gd > n_out) n_out = n_gd;
+  RB_CUDA(out.alloc(n_out * 8));
+  unsigned *d_gl = gl.as<unsigned>(), *d_gd = gd.as<unsigned>();
+  unsigned long long* d_ng = ng.as<unsigned long long>();
+  const SegVol V{Z, Y, X, (long long)X, (long long)Y * X};
+  SegTileGeom G;
+  const size_t smem = level_bytes == 1 && H <= 3 && na <= NW_MAX ? tile_plan(Z, Y, X, H, Ng, na, flags, G) : 0;
+  const int rc = smem ? launch_tile((const uint8_t*)lev, V, A, G, smem, Ng, alpha, flags, d_gl, d_gd, d_ng, st)
+                 : level_bytes == 1 ? launch_direct((const uint8_t*)lev, V, A, Ng, alpha, flags, d_gl, d_gd, d_ng, st)
+                                    : launch_direct((const uint16_t*)lev, V, A, Ng, alpha, flags, d_gl, d_gd, d_ng, st);
+  if (rc) return rc;
   const int cg = sm_count() * 4;
+  double* d_out = out.as<double>();
   if (flags & 1) {
     u32_to_f64_kernel<<<cg, 256, 0, st>>>(d_gl, (long long)n_gl, d_out);
-    SEG_TRY(cudaMemcpyAsync(glcm_host, d_out, n_gl * 8, cudaMemcpyDeviceToHost, st));
-    SEG_TRY(cudaStreamSynchronize(st));
+    RB_CUDA(cudaMemcpyAsync(glcm_host, d_out, n_gl * 8, cudaMemcpyDeviceToHost, st));
+    RB_CUDA(cudaStreamSynchronize(st));
   }
   if (flags & 2) {
     u32_to_f64_kernel<<<cg, 256, 0, st>>>(d_gd, (long long)n_gd, d_out);
-    SEG_TRY(cudaMemcpyAsync(gldm_host, d_out, n_gd * 8, cudaMemcpyDeviceToHost, st));
-    SEG_TRY(cudaStreamSynchronize(st));
+    RB_CUDA(cudaMemcpyAsync(gldm_host, d_out, n_gd * 8, cudaMemcpyDeviceToHost, st));
+    RB_CUDA(cudaStreamSynchronize(st));
   }
   if (flags & 4) {
     ngtdm_seg_finish_kernel<<<(Ng + 127) / 128, 128, 0, st>>>(d_ng, Ng, 2 * na, d_out);
-    SEG_TRY(cudaMemcpyAsync(ngtdm_host, d_out, (size_t)Ng * 3 * 8, cudaMemcpyDeviceToHost, st));
-    SEG_TRY(cudaStreamSynchronize(st));
+    RB_CUDA(cudaMemcpyAsync(ngtdm_host, d_out, (size_t)Ng * 3 * 8, cudaMemcpyDeviceToHost, st));
+    RB_CUDA(cudaStreamSynchronize(st));
   }
-  cleanup();
   return RB_OK;
 }
 
 // GLRLM of one packed level volume (uint8 or uint16) -> HOST float64 [Ng][Nr][Na]
 int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X, int Ng, int Nr, int force2D, int force2Ddimension,
-                  double* glrlm_host, int* angles_out, int* na_out, cudaStream_t st) {
+                  double* glrlm_host, int* angles_out, cudaStream_t st) {
+  if (Ng < 1 || Ng > 65535) return fail(RB_ERR_UNSUPPORTED, "Ng=%d outside 1..65535", Ng);
+  const long long n = (long long)Z * Y * X;
+  if (n <= 0 || n >= (1ll << 31)) return fail(RB_ERR_UNSUPPORTED, "volume must have 1..2^31-1 voxels");
   int size[3] = {Z, Y, X};
   const int* sz = nd == 3 ? size : size + 1;
   std::vector<int> ang;
@@ -380,44 +469,38 @@ int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X,
   A.na = na;
   for (int a = 0; a < na; a++)
     for (int d = 0; d < 3; d++) A.a[a][d] = d < 3 - nd ? 0 : (int8_t)ang[a * nd + d - (3 - nd)];
-  if (na_out) *na_out = na;
   if (angles_out) memcpy(angles_out, ang.data(), sizeof(int) * ang.size());
   const size_t per = (size_t)Ng * Nr * na;
-  unsigned* d_h = nullptr;
-  unsigned long long* d_c = nullptr;
-  int* d_st = nullptr;
-  double* d_out = nullptr;
-  auto cleanup = [&]() { cudaFree(d_h); cudaFree(d_c); cudaFree(d_st); cudaFree(d_out); };
-  SEG_TRY(cudaMalloc(&d_h, per * 4));
-  SEG_TRY(cudaMalloc(&d_c, (1 + (size_t)na) * 8));
-  SEG_TRY(cudaMalloc(&d_st, 4));
-  SEG_TRY(cudaMalloc(&d_out, per * 8));
-  SEG_TRY(cudaMemsetAsync(d_h, 0, per * 4, st));
-  SEG_TRY(cudaMemsetAsync(d_c, 0, (1 + (size_t)na) * 8, st));
-  SEG_TRY(cudaMemsetAsync(d_st, 0, 4, st));
-  SegVol V{Z, Y, X, (long long)X, (long long)Y * X};
-  const long long n = (long long)Z * Y * X;
-  long long need = (n + 255) / 256, cap = (long long)sm_count() * 8;
-  const int grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
+  DevBuf h, c, status, out;
+  RB_CUDA(h.alloc(per * 4));
+  RB_CUDA(c.alloc((1 + (size_t)na) * 8));
+  RB_CUDA(status.alloc(4));
+  RB_CUDA(out.alloc(per * 8));
+  RB_CUDA(cudaMemsetAsync(h.p, 0, per * 4, st));
+  RB_CUDA(cudaMemsetAsync(c.p, 0, (1 + (size_t)na) * 8, st));
+  RB_CUDA(cudaMemsetAsync(status.p, 0, 4, st));
+  unsigned* d_h = h.as<unsigned>();
+  unsigned long long* d_c = c.as<unsigned long long>();
+  int* d_st = status.as<int>();
+  const SegVol V{Z, Y, X, (long long)X, (long long)Y * X};
+  const int grid = grid_for(n, 256, 8);
   const size_t sh = (size_t)Ng * RL_SH * na * 4 <= 96 * 1024 ? (size_t)Ng * RL_SH * na * 4 : 0;
   if (level_bytes == 1) {
-    SEG_TRY(cudaFuncSetAttribute(seg_glrlm_ends_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    RB_CUDA(cudaFuncSetAttribute(seg_glrlm_ends_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     seg_glrlm_ends_kernel<uint8_t><<<grid, 256, sh, st>>>((const uint8_t*)lev, V, A, Ng, Nr, d_h, d_c, d_st);
   } else {
-    SEG_TRY(cudaFuncSetAttribute(seg_glrlm_ends_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    RB_CUDA(cudaFuncSetAttribute(seg_glrlm_ends_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     seg_glrlm_ends_kernel<uint16_t><<<grid, 256, sh, st>>>((const uint16_t*)lev, V, A, Ng, Nr, d_h, d_c, d_st);
   }
-  SEG_TRY(cudaGetLastError());
-  glrlm_to_f64_kernel<<<sm_count() * 4, 256, 0, st>>>(d_h, (long long)per, d_out, d_c, Nr, na);
-  SEG_TRY(cudaGetLastError());
+  RB_LAUNCH_CHECK();
+  glrlm_to_f64_kernel<<<sm_count() * 4, 256, 0, st>>>(d_h, (long long)per, out.as<double>(), d_c, Nr, na);
+  RB_LAUNCH_CHECK();
   int stv = 0;
-  SEG_TRY(cudaMemcpyAsync(&stv, d_st, 4, cudaMemcpyDeviceToHost, st));
-  SEG_TRY(cudaMemcpyAsync(glrlm_host, d_out, per * 8, cudaMemcpyDeviceToHost, st));
-  SEG_TRY(cudaStreamSynchronize(st));
-  cleanup();
+  RB_CUDA(cudaMemcpyAsync(&stv, d_st, 4, cudaMemcpyDeviceToHost, st));
+  RB_CUDA(cudaMemcpyAsync(glrlm_host, out.p, per * 8, cudaMemcpyDeviceToHost, st));
+  RB_CUDA(cudaStreamSynchronize(st));
   if (stv & 1) return fail(RB_ERR_LEVEL_RANGE, "Calculation of GLRLM Failed: run longer than Nr");
   return RB_OK;
 }
-#undef SEG_TRY
 
 }  // namespace rb

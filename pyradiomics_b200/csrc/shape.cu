@@ -196,8 +196,9 @@ int shape_coefficients_dev(const uint8_t* mask_dev, int Z, int Y, int X, long lo
   int rc = shape_load_tables();
   if (rc) return rc;
   struct Dev { ShapeAcc acc; unsigned long long cursor; unsigned long long dia[4]; };
-  Dev* d = nullptr;
-  RB_CUDA(cudaMalloc(&d, sizeof(Dev)));
+  DevBuf dev;
+  RB_CUDA(dev.alloc(sizeof(Dev)));
+  Dev* d = dev.as<Dev>();
   cudaMemsetAsync(d, 0, sizeof(Dev), st);
   const long long ncubes = (long long)(Z - 1) * (Y - 1) * (X - 1);
   const int grid = grid_for(ncubes, 256, 8);
@@ -205,37 +206,34 @@ int shape_coefficients_dev(const uint8_t* mask_dev, int Z, int Y, int X, long lo
   Dev h;
   cudaError_t e = cudaMemcpyAsync(&h, d, sizeof(Dev), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_CUDA, "shape mesh pass: %s", cudaGetErrorString(e)); }
+  if (e != cudaSuccess) return fail(RB_ERR_CUDA, "shape mesh pass: %s", cudaGetErrorString(e));
   out7[0] = h.acc.area; out7[1] = h.acc.vol6 / 6; out7[6] = (double)h.acc.nverts;
   if (h.acc.nverts) {
-    ushort4* verts = nullptr;
-    e = cudaMalloc(&verts, sizeof(ushort4) * h.acc.nverts);
-    if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_NOMEM, "shape: %llu mesh vertices do not fit", h.acc.nverts); }
+    DevBuf vbuf;
+    if (vbuf.alloc(sizeof(ushort4) * h.acc.nverts) != cudaSuccess) return fail(RB_ERR_NOMEM, "shape: %llu mesh vertices do not fit", h.acc.nverts);
+    ushort4* verts = vbuf.as<ushort4>();
     shape_mesh_kernel<<<grid, 256, 0, st>>>(mask_dev, Z, Y, X, sz, sy, sx, spacing[0], spacing[1], spacing[2], &d->acc, verts, &d->cursor);
     const long long nt = ((long long)h.acc.nverts + DT - 1) / DT;
     shape_diameter_kernel<<<grid_for(nt, 1, 8), DT, 0, st>>>(verts, (long long)h.acc.nverts, spacing[0], spacing[1], spacing[2], d->dia);
     e = cudaMemcpyAsync(&h, d, sizeof(Dev), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(verts);
-    if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_CUDA, "shape diameter pass: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(RB_ERR_CUDA, "shape diameter pass: %s", cudaGetErrorString(e));
     for (int q = 0; q < 4; q++) {
       double v;
       memcpy(&v, &h.dia[q], 8);
       out7[2 + q] = sqrt(v);
     }
   }
-  cudaFree(d);
   return RB_OK;
 }
 
 int shape_moments_dev(const uint8_t* mask_dev, int Z, int Y, int X, unsigned long long* out10, cudaStream_t st) {
-  unsigned long long* d = nullptr;
-  RB_CUDA(cudaMalloc(&d, 80));
-  cudaMemsetAsync(d, 0, 80, st);
-  shape_moments_kernel<<<grid_for((long long)Z * Y * X, 256, 8), 256, 0, st>>>(mask_dev, Z, Y, X, d);
-  cudaError_t e = cudaMemcpyAsync(out10, d, 80, cudaMemcpyDeviceToHost, st);
+  DevBuf d;
+  RB_CUDA(d.alloc(80));
+  cudaMemsetAsync(d.p, 0, 80, st);
+  shape_moments_kernel<<<grid_for((long long)Z * Y * X, 256, 8), 256, 0, st>>>(mask_dev, Z, Y, X, d.as<unsigned long long>());
+  cudaError_t e = cudaMemcpyAsync(out10, d.p, 80, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaFree(d);
   if (e != cudaSuccess) return fail(RB_ERR_CUDA, "shape moments: %s", cudaGetErrorString(e));
   return RB_OK;
 }
@@ -330,8 +328,9 @@ int shape2d_coefficients_dev(const uint8_t* mask_dev, int Y, int X, long long sy
   if (Y < 2 || X < 2) return RB_OK;
   if (Y > 32767 || X > 32767) return fail(RB_ERR_ARG, "shape2D: dimensions above 32767 are not supported");
   struct Dev { Shape2DAcc acc; unsigned long long cursor, best; };
-  Dev* d = nullptr;
-  RB_CUDA(cudaMalloc(&d, sizeof(Dev)));
+  DevBuf dev;
+  RB_CUDA(dev.alloc(sizeof(Dev)));
+  Dev* d = dev.as<Dev>();
   cudaMemsetAsync(d, 0, sizeof(Dev), st);
   const long long nsq = (long long)(Y - 1) * (X - 1);
   const int grid = grid_for(nsq, 256, 8);
@@ -339,26 +338,24 @@ int shape2d_coefficients_dev(const uint8_t* mask_dev, int Y, int X, long long sy
   Dev h;
   cudaError_t e = cudaMemcpyAsync(&h, d, sizeof(Dev), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_CUDA, "shape2D pass: %s", cudaGetErrorString(e)); }
+  if (e != cudaSuccess) return fail(RB_ERR_CUDA, "shape2D pass: %s", cudaGetErrorString(e));
   out4[0] = h.acc.perimeter;
   out4[1] = h.acc.area8 * 0.125 * spacing[0] * spacing[1];
   out4[3] = (double)h.acc.nverts;
   if (h.acc.nverts) {
-    ushort2* verts = nullptr;
-    e = cudaMalloc(&verts, sizeof(ushort2) * h.acc.nverts);
-    if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_NOMEM, "shape2D: %llu vertices do not fit", h.acc.nverts); }
+    DevBuf vbuf;
+    if (vbuf.alloc(sizeof(ushort2) * h.acc.nverts) != cudaSuccess) return fail(RB_ERR_NOMEM, "shape2D: %llu vertices do not fit", h.acc.nverts);
+    ushort2* verts = vbuf.as<ushort2>();
     shape2d_kernel<<<grid, 256, 0, st>>>(mask_dev, Y, X, sy, sx, spacing[0], spacing[1], &d->acc, verts, &d->cursor);
     const long long nt = ((long long)h.acc.nverts + 255) / 256;
     shape2d_diameter_kernel<<<grid_for(nt, 1, 8), 256, 0, st>>>(verts, (long long)h.acc.nverts, spacing[0], spacing[1], &d->best);
     e = cudaMemcpyAsync(&h, d, sizeof(Dev), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(verts);
-    if (e != cudaSuccess) { cudaFree(d); return fail(RB_ERR_CUDA, "shape2D diameter pass: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(RB_ERR_CUDA, "shape2D diameter pass: %s", cudaGetErrorString(e));
     double v;
     memcpy(&v, &h.best, 8);
     out4[2] = sqrt(v);
   }
-  cudaFree(d);
   return RB_OK;
 }
 

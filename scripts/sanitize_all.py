@@ -81,6 +81,11 @@ if "matrix" in fams:
     print("matrix tma/coop ok", flush=True)
     cmatrices.calculate_glcm(lev[3], mask_rag[3], [1, 2], 32, False, -1)          # 2-D
     cmatrices.calculate_glszm(lev[3], mask_rag[3], 32, int(mask_rag[3].sum()), False, -1)
+    # the direct segment kernel: 16-bit levels (all three matrices in one pass), and offsets > 3 in 2-D
+    levd, _ = voxel.pack_levels(torch.as_tensor(lev + 268).cuda(), torch.as_tensor(mask_rag).cuda(), 300)
+    cmatrices.segment_texture_device(levd, [1, 2], 300, 0, False, -1)
+    cmatrices.calculate_glcm(lev[3], mask_rag[3], [1, 4], 32, False, -1)
+    print("matrix direct ok", flush=True)
 
 if "filters" in fams:
     raw = (vols["smooth"].astype(np.float64) - 1) * 25 + rng.random(mask_full.shape) * 20

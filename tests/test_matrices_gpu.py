@@ -144,11 +144,11 @@ def test_segment_mode_at_scale_properties():
     assert (Z[0] * np.arange(1, Z.shape[2] + 1)[None, :]).sum() == N ** 3
 
 
-# ---- round 2: tile-staged fused segment kernel (TMA / cooperative), run-end GLRLM, device-resident entry points
+# ---- segment kernels: the tile-staged fused kernel (TMA / cooperative), the direct kernel, run-end GLRLM, device entry points
 @pytest.mark.parametrize("shape,dist", [((20, 33, 64), [1]), ((9, 17, 48), [1, 2]), ((1, 40, 80), [1]), ((37, 29, 23), [1, 3])])
-def test_segment_kernels_tma_equals_cooperative_equals_legacy(shape, dist, monkeypatch):
+def test_segment_kernels_tma_equals_cooperative_equals_oracle(shape, dist, monkeypatch):
     """the fused GLCM + GLDM + NGTDM tile kernel with its box staged by TMA (row pitch a multiple of 16 bytes) or by
-    cooperative loads, and the run-end GLRLM kernel, against round 1's one-thread-per-voxel kernels: identical matrices"""
+    cooperative loads, and the run-end GLRLM kernel: identical matrices, equal to the oracle"""
     import torch
     from pyradiomics_b200 import cmatrices, voxel
     rng = np.random.default_rng(12)
@@ -157,23 +157,19 @@ def test_segment_kernels_tma_equals_cooperative_equals_legacy(shape, dist, monke
     lev = rng.integers(1, 25, shape).astype(np.int32)
     msk = rng.random(shape) < 0.8
     res = {}
-    modes = ("tma", "coop", "legacy")
-    for mode in modes:
+    for mode in ("tma", "coop"):
         monkeypatch.setenv("B200_SEG_TMA", "0" if mode == "coop" else "1")
-        monkeypatch.setenv("B200_SEG_LEGACY", "1" if mode == "legacy" else "0")
         P, ang = cmatrices.calculate_glcm(lev, msk, dist, 24, False, -1)
         R, _ = cmatrices.calculate_glrlm(lev, msk, 24, max(shape), False, -1)
         res[mode] = (P, cmatrices.calculate_gldm(lev, msk, dist, 24, 1, False, -1), cmatrices.calculate_ngtdm(lev, msk, dist, 24, False, -1), R)
-    res["tma"] = res.get("tma", res["coop"])
     for k in range(4):
         assert np.array_equal(res["tma"][k], res["coop"][k])
-        if k == 2:      # s_i is an fp64 sum: exact-integer accumulation in both, same division order -> still identical
-            assert np.allclose(res["tma"][k], res["legacy"][k], rtol=1e-14, atol=0)
-        else:
-            assert np.array_equal(res["tma"][k], res["legacy"][k])
+    ref = (O.calculate_glcm(lev, msk, dist, 24, False, -1)[0], O.calculate_gldm(lev, msk, dist, 24, 1, False, -1),
+           O.calculate_ngtdm(lev, msk, dist, 24, False, -1), O.calculate_glrlm(lev, msk, 24, max(shape), False, -1)[0])
+    for k in range(4):
+        _same(res["tma"][k], ref[k], ngtdm=k == 2)
     # the same from a device-resident packed level volume, all three matrices in one pass
-    monkeypatch.setenv("B200_SEG_TMA", "1" if "tma" in modes else "0")
-    monkeypatch.setenv("B200_SEG_LEGACY", "0")
+    monkeypatch.setenv("B200_SEG_TMA", "1")
     levd, _ = voxel.pack_levels(torch.as_tensor(lev).cuda(), torch.as_tensor(msk).cuda(), 24)
     d = cmatrices.segment_texture_device(levd, dist, 24, 1, False, -1)
     assert np.array_equal(d["glcm"][0], res["tma"][0]) and np.array_equal(d["gldm"], res["tma"][1]) and np.array_equal(d["ngtdm"], res["tma"][2])
@@ -181,6 +177,70 @@ def test_segment_kernels_tma_equals_cooperative_equals_legacy(shape, dist, monke
     assert np.array_equal(Rd, res["tma"][3])
     Zd = cmatrices.calculate_glszm_device(levd, 24, False, -1)
     assert np.array_equal(Zd, cmatrices.calculate_glszm(lev, msk, 24, int(msk.sum()), False, -1))
+
+
+def test_segment_tile_kernel_equals_direct_kernel():
+    """levels 1..24 as an 8-bit volume (Ng = 24: tile kernel) and as a 16-bit one (Ng = 300: direct kernel): the leading
+    24 levels of the Ng = 300 matrices are the Ng = 24 matrices bit for bit, NGTDM s_i included"""
+    import torch
+    from pyradiomics_b200 import cmatrices, voxel
+    rng = np.random.default_rng(21)
+    lev = rng.integers(1, 25, (19, 31, 48)).astype(np.int32)
+    msk = rng.random(lev.shape) < 0.8
+    dist = [1, 2]
+    got = {}
+    for Ng in (24, 300):
+        levd, _ = voxel.pack_levels(torch.as_tensor(lev).cuda(), torch.as_tensor(msk).cuda(), Ng)
+        assert levd.element_size() == (1 if Ng == 24 else 2)
+        d = cmatrices.segment_texture_device(levd, dist, Ng, 1, False, -1)
+        h = (cmatrices.calculate_glcm(lev, msk, dist, Ng, False, -1)[0], cmatrices.calculate_gldm(lev, msk, dist, Ng, 1, False, -1),
+             cmatrices.calculate_ngtdm(lev, msk, dist, Ng, False, -1))
+        got[Ng] = ((d["glcm"][0], d["gldm"], d["ngtdm"]), h)
+    for api in range(2):
+        small, big = got[24][api], got[300][api]
+        assert np.array_equal(big[0][:, :24, :24], small[0]) and not big[0][:, 24:].any() and not big[0][:, :, 24:].any()
+        assert np.array_equal(big[1][:, :24], small[1]) and not big[1][:, 24:].any()
+        assert np.array_equal(big[2][:, :24], small[2]) and not big[2][:, 24:, :2].any()
+
+
+@pytest.mark.parametrize("case", ["2d_long_offsets", "3d_glcm_193_offsets", "3d_many_levels", "16bit_one_pass"])
+def test_segment_direct_kernel_triggers_match_oracle(case):
+    """one input for each reason the direct kernel runs instead of the tile kernel, against the oracle"""
+    import torch
+    from pyradiomics_b200 import cmatrices, voxel
+    from pyradiomics_b200._lib import B200Error
+    rng = np.random.default_rng(33)
+    shape, dist, Ng = {"2d_long_offsets": ((40, 50), [1, 4], 24),            # offsets > 3; GLCM privatised in shared memory
+                       "3d_glcm_193_offsets": ((9, 11, 13), [4], 8),         # 193 unidirectional offsets: GLCM only
+                       "3d_many_levels": ((10, 12, 14), [1, 2, 3], 200),     # GLDM / NGTDM histograms overflow shared memory
+                       "16bit_one_pass": ((14, 17, 33), [1, 2], 300)}[case]
+    lev = rng.integers(1, Ng + 1, shape).astype(np.int32)
+    msk = rng.random(shape) < 0.8
+    P, ang = cmatrices.calculate_glcm(lev, msk, dist, Ng, False, -1)
+    Pr, ang_r = O.calculate_glcm(lev, msk, dist, Ng, False, -1)
+    _same(P, Pr)
+    assert np.array_equal(ang, ang_r)
+    if case == "3d_glcm_193_offsets":
+        assert ang.shape[0] == 193
+        with pytest.raises(B200Error):
+            cmatrices.calculate_gldm(lev, msk, dist, Ng, 1, False, -1)
+        with pytest.raises(B200Error):
+            cmatrices.calculate_ngtdm(lev, msk, dist, Ng, False, -1)
+        levd, _ = voxel.pack_levels(torch.as_tensor(lev).cuda(), torch.as_tensor(msk).cuda(), Ng)
+        d = cmatrices.segment_texture_device(levd, dist, Ng, 1, False, -1, glcm=True, gldm=False, ngtdm=False)
+        _same(d["glcm"][0], Pr)
+        assert np.array_equal(d["glcm"][1], ang_r)
+        with pytest.raises(B200Error):
+            cmatrices.segment_texture_device(levd, dist, Ng, 1, False, -1, glcm=True, gldm=True, ngtdm=False)
+        return
+    D, N = O.calculate_gldm(lev, msk, dist, Ng, 1, False, -1), O.calculate_ngtdm(lev, msk, dist, Ng, False, -1)
+    _same(cmatrices.calculate_gldm(lev, msk, dist, Ng, 1, False, -1), D)
+    _same(cmatrices.calculate_ngtdm(lev, msk, dist, Ng, False, -1), N, ngtdm=True)
+    levd, _ = voxel.pack_levels(torch.as_tensor(lev).cuda(), torch.as_tensor(msk).cuda(), Ng)
+    d = cmatrices.segment_texture_device(levd, dist, Ng, 1, False, -1)
+    _same(d["glcm"][0], Pr)
+    _same(d["gldm"], D)
+    _same(d["ngtdm"], N, ngtdm=True)
 
 
 def test_glrlm_single_voxel_lines_rule_from_pigeonhole_counts():
@@ -195,3 +255,24 @@ def test_glrlm_single_voxel_lines_rule_from_pigeonhole_counts():
     got, ang = cmatrices.calculate_glrlm(lev, msk, 8, 7, False, -1)
     ref, ang_r = O.calculate_glrlm(lev, msk, 8, 7, False, -1)
     assert np.array_equal(ang, ang_r) and np.array_equal(got, ref)
+
+
+@pytest.mark.parametrize("dist", [[1], [1, 2, 3]])
+def test_segment_gldm_ngtdm_at_the_largest_ng(dist):
+    """GLDM / NGTDM without GLCM at Ng = 65535 (16-bit levels, direct kernel), host and device APIs, against the oracle:
+    their device buffers scale with Ng, not Ng^2"""
+    import torch
+    from pyradiomics_b200 import cmatrices, voxel
+    rng = np.random.default_rng(44)
+    Ng = 65535
+    lev = rng.choice(np.array([1, 2, 3, 300, 301, 40000, 65534, 65535], np.int32), (6, 7, 8))
+    msk = rng.random(lev.shape) < 0.8
+    N = O.calculate_ngtdm(lev, msk, dist, Ng, False, -1)
+    _same(cmatrices.calculate_ngtdm(lev, msk, dist, Ng, False, -1), N, ngtdm=True)
+    levd, _ = voxel.pack_levels(torch.as_tensor(lev).cuda(), torch.as_tensor(msk).cuda(), Ng)
+    d = cmatrices.segment_texture_device(levd, dist, Ng, 1, False, -1, glcm=False, gldm=dist == [1], ngtdm=True)
+    _same(d["ngtdm"], N, ngtdm=True)
+    if dist == [1]:          # (at [1, 2, 3] the float64 GLDM alone is 0.36 GB on the host per copy)
+        D = O.calculate_gldm(lev, msk, dist, Ng, 1, False, -1)
+        _same(cmatrices.calculate_gldm(lev, msk, dist, Ng, 1, False, -1), D)
+        _same(d["gldm"], D)
