@@ -248,6 +248,28 @@ int rb_lbp3d_dev(const void *img_dev, int img_dtype, int sample_dtype, const uin
                  const double *vertices_host, int nv, const double *harmonics_host, int levels,
                  double *coeff_scratch_dev, double *out_dev, void *stream);
 
+/* ---- 2-D local binary pattern image type (reference radiomics/imageoperations.py:1094-1166, getLBP2DImage ->
+ *      skimage.feature.local_binary_pattern), every slice of a (Z, Y, X) volume in one call.
+ * The slices are cut along `axis` as the reference's swapaxes(0, axis) does: axis 0 -> rows y, cols x; axis 1 -> rows z,
+ *   cols x; axis 2 -> rows y, cols z.  A 2-D image is passed as Z = 1, axis 0.
+ * For pixel (r, c) of a slice and k = 0..P-1 (rp_host / cp_host: P HOST doubles, round(-R sin(2 pi k / P), 5) and
+ *   round(R cos(2 pi k / P), 5)):
+ *   t_k = bilinear sample at (r + rp[k], c + cp[k]): minr = floor, maxr = ceil, dr = r - minr (columns alike),
+ *         top = (1 - dc) tl + dc tr, bottom = (1 - dc) bl + dc br, t_k = (1 - dr) top + dr bottom, every operation rounded
+ *         on its own (no FMA); a corner outside the slice reads 0;
+ *   s_k = (t_k - centre >= 0);
+ *   RB_LBP2D_DEFAULT      sum_k s_k 2^k
+ *   RB_LBP2D_ROR          the minimum over the P right rotations (v >> 1) | ((v & 1) << (P - 1)) of DEFAULT
+ *   RB_LBP2D_UNIFORM      changes = #{k < P - 1: s_k != s_k+1} (not circular); sum_k s_k if changes <= 2, else P + 1
+ *   RB_LBP2D_NRI_UNIFORM  changes > 2: P (P - 1) + 2; no ones: 0; all ones: P (P - 1) + 1; else 1 + (n_ones - 1) P + rot,
+ *                         rot = n_ones - first_zero if s_0 = 1, else P - first_one
+ *   RB_LBP2D_VAR          sum += t, sq += t t over k, v = (sq - sum sum / P) / P; v if v != 0, else NaN
+ * out_dev: float64 (Z, Y, X), the input's layout.  img dtype codes as rb_minmax_dev.  1 <= P <= 31 (the library's int32
+ *   weights overflow beyond), else RB_ERR_UNSUPPORTED; an unknown method or axis is RB_ERR_ARG. */
+enum { RB_LBP2D_DEFAULT = 0, RB_LBP2D_ROR = 1, RB_LBP2D_UNIFORM = 2, RB_LBP2D_NRI_UNIFORM = 3, RB_LBP2D_VAR = 4 };
+int rb_lbp2d_dev(const void *img_dev, int dtype, int Z, int Y, int X, int axis, int P, const double *rp_host,
+                 const double *cp_host, int method, double *out_dev, void *stream);
+
 /* ---- per-voxel image types (reference radiomics/imageoperations.py:973-1073, getSquareImage, getSquareRootImage,
  *      getLogarithmImage, getExponentialImage).  out_dev[i] = f(x), x = img_dev[i] as float64, for i < nvoxels:
  *   RB_PW_SQUARE       (c x)^2                                   c = 1 / sqrt(M)                  (:989-991)

@@ -3,7 +3,8 @@
 :67-174), the level-1 stationary wavelet decomposition (getWaveletImage / _swt3, :839-970), the
 Laplacian-of-Gaussian filter (getLoGImage, :756-836), the per-voxel square / square root /
 logarithm / exponential images (getSquareImage ... getExponentialImage, :973-1073), the gradient
-magnitude (getGradientImage, :1076-1091), the 3-D local binary pattern (getLBP3DImage,
+magnitude (getGradientImage, :1076-1091), the 2-D local binary pattern (getLBP2DImage, :1094-1166,
+skimage.feature.local_binary_pattern restated), the 3-D local binary pattern (getLBP3DImage,
 :1169-1314), and the two preprocessing steps in front of them: image normalisation (normalizeImage,
 :615-654) and mask resegmentation (resegmentMask, :657-742).  Same function names, arguments and
 yielded tuples as the reference so they can be dropped into ``radiomics.imageoperations``.
@@ -13,7 +14,8 @@ few-ulp difference of a float64 ROI reduction); normalisation restates ITK's Nor
 details in DESIGN.md section 5); binning, square and square root are bit-identical to NumPy, logarithm and
 exponential within CUDA's 1-ulp log / exp; wavelet, LoG and gradient restate PyWavelets' and ITK's
 published algorithms -- neither library is available offline and the reference's own tests do not
-pin them (SURVEY.md section 8c) -> "parity unpinned" for those three.
+pin them (SURVEY.md section 8c) -> "parity unpinned" for those three.  LBP 2-D pins the reference's
+wrapper and restates scikit-image's local_binary_pattern bit for bit; scikit-image itself is unavailable to pin it.
 """
 from __future__ import annotations
 
@@ -913,3 +915,81 @@ def getLBP3DImage(inputImage, inputMask, **kwargs):
     for l_idx in range(levels):
         yield I.like(inputImage, out[l_idx]), f"lbp-3D-m{l_idx + 1}", kwargs
     yield I.like(inputImage, out[levels]), "lbp-3D-k", kwargs
+
+
+LBP2D_METHODS = {"default": 0, "ror": 1, "uniform": 2, "nri_uniform": 3, "var": 4}      # RB_LBP2D_*
+LBP2D_MAX_SAMPLES = 31
+
+
+def _lbp2d_params(samples, radius, method):
+    """(P, method code, rp, cp) of rb_lbp2d_dev, checked before anything reaches the device.  The offsets are
+    skimage's own expressions, round(-R sin(2 pi k / P), 5) and round(R cos(2 pi k / P), 5).  An unknown method raises
+    KeyError (the library's method dictionary); P outside 1..31 (its int32 weights 2**arange(P) overflow beyond) or a
+    radius that is not a finite number > 0 raises ValueError."""
+    code = LBP2D_METHODS[method.lower()]
+    if isinstance(samples, (bool, np.bool_)) or not isinstance(samples, (int, np.integer)) \
+            or not 1 <= samples <= LBP2D_MAX_SAMPLES:
+        raise ValueError(f"LBP 2D: lbp2DSamples {samples!r} outside the CUDA kernel's range (an integer 1..31)")
+    R = float(radius)
+    if not (math.isfinite(R) and R > 0):
+        raise ValueError(f"LBP 2D: lbp2DRadius {radius!r} must be a finite number > 0")
+    P = int(samples)
+    rp = np.ascontiguousarray(np.round(- R * np.sin(2 * np.pi * np.arange(P, dtype=np.float64) / P), 5))
+    cp = np.ascontiguousarray(np.round(R * np.cos(2 * np.pi * np.arange(P, dtype=np.float64) / P), 5))
+    return P, code, rp, cp
+
+
+def lbp2d_device(img_t: torch.Tensor, axis=0, samples=8, radius=1, method="uniform"):
+    """2-D LBP (skimage.feature.local_binary_pattern(slice, P=samples, R=radius, method=method)) of every slice of a CUDA
+    volume (Z,Y,X) cut along `axis` as getLBP2DImage cuts it (swapaxes(0, axis): axis 0 -> (y, x) slices, 1 -> (z, x),
+    2 -> (y, z)), or of a CUDA plane (Y,X) -> float64 CUDA tensor of the input's shape (rb_lbp2d_dev).  No cast to the
+    image's dtype: getLBP2DImage does that on the host, as the reference does."""
+    P, code, rp, cp = _lbp2d_params(samples, radius, method)
+    src = img_t.contiguous()
+    if src.dim() not in (2, 3):
+        raise ValueError(f"LBP 2D: 2-D or 3-D image expected, got {src.dim()}-D")
+    if src.dtype not in _TORCH_DT:
+        raise ValueError(f"unsupported pixel type {src.dtype}")
+    if src.dim() == 2:
+        axis = 0
+    elif isinstance(axis, (int, np.integer)) and -3 <= axis <= 2:
+        axis = int(axis) % 3                                    # swapaxes' negative axes
+    else:
+        raise ValueError(f"LBP 2D: force2Ddimension {axis!r} (0, 1 or 2)")
+    Z, Y, X = (1,) * (3 - src.dim()) + tuple(src.shape)
+    out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
+    check(lib().rb_lbp2d_dev(_ptr(src), _TORCH_DT[src.dtype], Z, Y, X, int(axis), P, rp.ctypes.data_as(C.c_void_p),
+                             cp.ctypes.data_as(C.c_void_p), code, _ptr(out), _stream()), "lbp2d")
+    return out
+
+
+def getLBP2DImage(inputImage, _inputMask, **kwargs):
+    """reference generator (imageoperations.py:1094-1166): the local binary pattern of skimage.feature, slice by slice.
+    Settings lbp2DRadius (1), lbp2DSamples (8, what the reference's code uses; its docstring says 9), lbp2DMethod
+    ('uniform'), force2Ddimension (0, read even without force2D; a warning is logged when force2D is off).  A 3-D image
+    keeps its dtype (each float64 slice is assigned into a copy of the image, as the reference does: NumPy's cast,
+    truncation and out-of-range values included); a 2-D image gives float64.  Other dimensionalities: a warning and
+    nothing.  Yields (image, 'lbp-2D', kwargs)."""
+    radius = kwargs.get("lbp2DRadius", 1)
+    samples = kwargs.get("lbp2DSamples", 8)
+    method = kwargs.get("lbp2DMethod", "uniform")
+    arr = I.as_array(inputImage)
+    Nd = arr.ndim
+    if Nd in (2, 3):
+        _lbp2d_params(samples, radius, method)                  # range check before anything reaches the device
+    if Nd == 3:
+        if not kwargs.get("force2D", False):
+            logger.warning("Calculating Local Binary Pattern in 2D, but extracting features in 3D. Use with caution!")
+        axis = kwargs.get("force2Ddimension", 0)
+        out = lbp2d_device(_to_device(arr), axis, samples, radius, method).cpu().numpy()
+        im_arr = np.array(arr).swapaxes(0, axis)
+        out = out.swapaxes(0, axis)
+        for idx in range(im_arr.shape[0]):
+            im_arr[idx, ...] = np.ascontiguousarray(out[idx])
+        im_arr = im_arr.swapaxes(0, axis)
+    elif Nd == 2:
+        im_arr = lbp2d_device(_to_device(arr), 0, samples, radius, method).cpu().numpy()
+    else:
+        logger.warning("LBP 2D is only available for 2D or 3D with forced 2D extraction")
+        return
+    yield I.like(inputImage, im_arr), "lbp-2D", kwargs
