@@ -183,8 +183,11 @@ int rb_segment_glszm_dev(const void *levels_dev, int level_bytes, const int *siz
                          int force2Ddimension, int *max_region, void **handle);
 
 /* ---- gray-level discretisation and pre-filters (device pointers, asynchronous) --------------
- * dtype codes for `image_dev`: 0 int16, 1 int32, 2 float32, 3 float64, 4 uint8, 5 uint16, 6 int64.
- * rb_minmax_dev: ROI minimum / maximum (mask_dev may be NULL = all voxels) as order-preserving
+ * Pixel types: every `dtype` argument is an rb_dtype code; any other value gives RB_ERR_ARG. */
+typedef enum {
+  RB_DT_INT16 = 0, RB_DT_INT32 = 1, RB_DT_FLOAT32 = 2, RB_DT_FLOAT64 = 3, RB_DT_UINT8 = 4, RB_DT_UINT16 = 5, RB_DT_INT64 = 6
+} rb_dtype;
+/* rb_minmax_dev: ROI minimum / maximum (mask_dev may be NULL = all voxels) as order-preserving
  *   int64 keys in keys_dev[0..1] plus the voxel count in keys_dev[2]; initialise keys_dev to
  *   {INT64_MAX, INT64_MIN, 0}; decode a key k with  bits = k >= 0 ? k : k ^ INT64_MAX.
  *   Replaces the Python-level min()/max() of getBinEdges (radiomics/imageoperations.py:128-129).

@@ -10,11 +10,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import check, lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
+from ._lib import check, lib, ptr
 
 
 def _arrays(image, mask):
@@ -56,8 +52,8 @@ def generate_angles(size, distances, bidirectional, force2D, force2Ddimension):
     nd = int(size.shape[0])
     cap = max(1, (2 * int(d.max()) + 1) ** nd) if d.size else 1
     buf = np.empty((cap, nd), dtype=np.int32)
-    na = lib().rb_generate_angles(_p(size), nd, _p(d), int(d.size), int(bool(bidirectional)), int(bool(force2D)),
-                                  int(force2Ddimension), _p(buf), cap)
+    na = lib().rb_generate_angles(ptr(size), nd, ptr(d), int(d.size), int(bool(bidirectional)), int(bool(force2D)),
+                                  int(force2Ddimension), ptr(buf), cap)
     if na <= 0:
         raise RuntimeError("Error getting angle count.")
     return buf[:na].copy()
@@ -69,8 +65,8 @@ def calculate_glcm(image, mask, distances, Ng, force2D, force2Ddimension, kernel
     ang = generate_angles(size, d, 0, force2D, force2Ddimension)
     v, nvox = _voxels(voxels, img.ndim, kernelRadius)
     out = np.empty((nvox, Ng, Ng, ang.shape[0]), dtype=np.float64)
-    check(lib().rb_calculate_glcm(_p(img), _p(msk), _p(size), img.ndim, _p(d), int(d.size), int(Ng), int(bool(force2D)),
-                                  int(force2Ddimension), int(kernelRadius), _p(v), nvox, _p(out), None), "GLCM")
+    check(lib().rb_calculate_glcm(ptr(img), ptr(msk), ptr(size), img.ndim, ptr(d), int(d.size), int(Ng), int(bool(force2D)),
+                                  int(force2Ddimension), int(kernelRadius), ptr(v), nvox, ptr(out), None), "GLCM")
     return out, ang
 
 
@@ -79,8 +75,8 @@ def calculate_glrlm(image, mask, Ng, Nr, force2D, force2Ddimension, kernelRadius
     ang = generate_angles(size, [1], 0, force2D, force2Ddimension)
     v, nvox = _voxels(voxels, img.ndim, kernelRadius)
     out = np.empty((nvox, Ng, int(Nr), ang.shape[0]), dtype=np.float64)
-    check(lib().rb_calculate_glrlm(_p(img), _p(msk), _p(size), img.ndim, int(Ng), int(Nr), int(bool(force2D)),
-                                   int(force2Ddimension), int(kernelRadius), _p(v), nvox, _p(out), None), "GLRLM")
+    check(lib().rb_calculate_glrlm(ptr(img), ptr(msk), ptr(size), img.ndim, int(Ng), int(Nr), int(bool(force2D)),
+                                   int(force2Ddimension), int(kernelRadius), ptr(v), nvox, ptr(out), None), "GLRLM")
     return out, ang
 
 
@@ -90,12 +86,12 @@ def calculate_glszm(image, mask, Ng, Ns, force2D, force2Ddimension, kernelRadius
     v, nvox = _voxels(voxels, img.ndim, kernelRadius)
     mx = C.c_int(0)
     handle = C.c_void_p()
-    check(lib().rb_calculate_glszm(_p(img), _p(msk), _p(size), img.ndim, int(Ng), int(bool(force2D)),
-                                   int(force2Ddimension), int(kernelRadius), _p(v), nvox, C.byref(mx), C.byref(handle)),
+    check(lib().rb_calculate_glszm(ptr(img), ptr(msk), ptr(size), img.ndim, int(Ng), int(bool(force2D)),
+                                   int(force2Ddimension), int(kernelRadius), ptr(v), nvox, C.byref(mx), C.byref(handle)),
           "GLSZM")
     max_region = max(1, mx.value)
     out = np.empty((nvox, Ng, max_region), dtype=np.float64)
-    check(lib().rb_fill_glszm(handle, int(Ng), max_region, _p(out)), "GLSZM")
+    check(lib().rb_fill_glszm(handle, int(Ng), max_region, ptr(out)), "GLSZM")
     return out
 
 
@@ -105,8 +101,8 @@ def calculate_ngtdm(image, mask, distances, Ng, force2D, force2Ddimension, kerne
     generate_angles(size, d, 1, force2D, force2Ddimension)
     v, nvox = _voxels(voxels, img.ndim, kernelRadius)
     out = np.empty((nvox, Ng, 3), dtype=np.float64)
-    check(lib().rb_calculate_ngtdm(_p(img), _p(msk), _p(size), img.ndim, _p(d), int(d.size), int(Ng), int(bool(force2D)),
-                                   int(force2Ddimension), int(kernelRadius), _p(v), nvox, _p(out)), "NGTDM")
+    check(lib().rb_calculate_ngtdm(ptr(img), ptr(msk), ptr(size), img.ndim, ptr(d), int(d.size), int(Ng), int(bool(force2D)),
+                                   int(force2Ddimension), int(kernelRadius), ptr(v), nvox, ptr(out)), "NGTDM")
     return out
 
 
@@ -116,8 +112,8 @@ def calculate_gldm(image, mask, distances, Ng, alpha, force2D, force2Ddimension,
     ang = generate_angles(size, d, 1, force2D, force2Ddimension)
     v, nvox = _voxels(voxels, img.ndim, kernelRadius)
     out = np.empty((nvox, Ng, 2 * ang.shape[0] + 1), dtype=np.float64)
-    check(lib().rb_calculate_gldm(_p(img), _p(msk), _p(size), img.ndim, _p(d), int(d.size), int(Ng), int(alpha),
-                                  int(bool(force2D)), int(force2Ddimension), int(kernelRadius), _p(v), nvox, _p(out)),
+    check(lib().rb_calculate_gldm(ptr(img), ptr(msk), ptr(size), img.ndim, ptr(d), int(d.size), int(Ng), int(alpha),
+                                  int(bool(force2D)), int(force2Ddimension), int(kernelRadius), ptr(v), nvox, ptr(out)),
           "GLDM")
     return out
 
@@ -131,13 +127,13 @@ def _dev_args(levels):
     assert isinstance(levels, torch.Tensor) and levels.is_cuda and levels.is_contiguous() and levels.ndim in (2, 3)
     size = np.array(levels.shape, dtype=np.int32)
     lb = 1 if levels.dtype == torch.uint8 else 2
-    return C.c_void_p(levels.data_ptr()), lb, size
+    return levels.data_ptr(), lb, size
 
 
 def segment_texture_device(levels, distances, Ng, alpha, force2D, force2Ddimension, glcm=True, gldm=True, ngtdm=True):
     """GLCM, GLDM and NGTDM of one ROI in ONE pass over the device-resident level volume (rb_segment_texture_dev):
     {"glcm": (P [1,Ng,Ng,Na], angles), "gldm": P [1,Ng,2*Na_bi+1], "ngtdm": P [1,Ng,3]} for the requested ones"""
-    ptr, lb, size = _dev_args(levels)
+    lev, lb, size = _dev_args(levels)
     d = _distances(distances)
     ang = generate_angles(size, d, 0, force2D, force2Ddimension)
     ang_bi = generate_angles(size, d, 1, force2D, force2Ddimension)
@@ -145,8 +141,8 @@ def segment_texture_device(levels, distances, Ng, alpha, force2D, force2Ddimensi
     P_glcm = np.empty((1, Ng, Ng, ang.shape[0]), dtype=np.float64) if glcm else None
     P_gldm = np.empty((1, Ng, 2 * ang_bi.shape[0] + 1), dtype=np.float64) if gldm else None
     P_ngtdm = np.empty((1, Ng, 3), dtype=np.float64) if ngtdm else None
-    check(lib().rb_segment_texture_dev(ptr, lb, _p(size), int(size.size), _p(d), int(d.size), int(Ng), int(alpha), int(bool(force2D)),
-                                       int(force2Ddimension), _p(P_glcm), _p(P_gldm), _p(P_ngtdm), None), "GLCM/GLDM/NGTDM")
+    check(lib().rb_segment_texture_dev(lev, lb, ptr(size), int(size.size), ptr(d), int(d.size), int(Ng), int(alpha), int(bool(force2D)),
+                                       int(force2Ddimension), ptr(P_glcm), ptr(P_gldm), ptr(P_ngtdm), None), "GLCM/GLDM/NGTDM")
     if glcm:
         out["glcm"] = (P_glcm, ang)
     if gldm:
@@ -157,22 +153,22 @@ def segment_texture_device(levels, distances, Ng, alpha, force2D, force2Ddimensi
 
 
 def calculate_glrlm_device(levels, Ng, Nr, force2D, force2Ddimension):
-    ptr, lb, size = _dev_args(levels)
+    lev, lb, size = _dev_args(levels)
     ang = generate_angles(size, [1], 0, force2D, force2Ddimension)
     out = np.empty((1, Ng, int(Nr), ang.shape[0]), dtype=np.float64)
-    check(lib().rb_segment_glrlm_dev(ptr, lb, _p(size), int(size.size), int(Ng), int(Nr), int(bool(force2D)), int(force2Ddimension),
-                                     _p(out), None), "GLRLM")
+    check(lib().rb_segment_glrlm_dev(lev, lb, ptr(size), int(size.size), int(Ng), int(Nr), int(bool(force2D)), int(force2Ddimension),
+                                     ptr(out), None), "GLRLM")
     return out, ang
 
 
 def calculate_glszm_device(levels, Ng, force2D, force2Ddimension):
-    ptr, lb, size = _dev_args(levels)
+    lev, lb, size = _dev_args(levels)
     generate_angles(size, [1], 1, force2D, force2Ddimension)
     mx = C.c_int(0)
     handle = C.c_void_p()
-    check(lib().rb_segment_glszm_dev(ptr, lb, _p(size), int(size.size), int(Ng), int(bool(force2D)), int(force2Ddimension),
+    check(lib().rb_segment_glszm_dev(lev, lb, ptr(size), int(size.size), int(Ng), int(bool(force2D)), int(force2Ddimension),
                                      C.byref(mx), C.byref(handle)), "GLSZM")
     max_region = max(1, mx.value)
     out = np.empty((1, Ng, max_region), dtype=np.float64)
-    check(lib().rb_fill_glszm(handle, int(Ng), max_region, _p(out)), "GLSZM")
+    check(lib().rb_fill_glszm(handle, int(Ng), max_region, ptr(out)), "GLSZM")
     return out

@@ -10,7 +10,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import check, lib
+from ._lib import check, lib, ptr, stream
 
 _fallback = None        # the reference's _cshape module, set by featureclasses.install()
 
@@ -34,9 +34,7 @@ def calculate_coefficients(mask, pixelSpacing):
     strides = np.array([s // msk.itemsize for s in msk.strides], dtype=np.int32)
     sa, vol = C.c_double(), C.c_double()
     dia = (C.c_double * 4)()
-    rc = lib().rb_calculate_coefficients(msk.ctypes.data_as(C.c_char_p), size.ctypes.data_as(C.c_void_p),
-                                         strides.ctypes.data_as(C.c_void_p), sp.ctypes.data_as(C.c_void_p),
-                                         C.byref(sa), C.byref(vol), dia)
+    rc = lib().rb_calculate_coefficients(ptr(msk), ptr(size), ptr(strides), ptr(sp), C.byref(sa), C.byref(vol), dia)
     if rc:
         check(rc, "Calculation of Shape coefficients failed.")
     return sa.value, vol.value, tuple(dia)
@@ -54,9 +52,8 @@ def calculate_coefficients2D(mask, pixelSpacing):
     size = np.array(msk.shape, dtype=np.int32)
     strides = np.array([s // msk.itemsize for s in msk.strides], dtype=np.int32)
     per, sur, dia = C.c_double(), C.c_double(), C.c_double()
-    rc = lib().rb_calculate_coefficients2D(msk.ctypes.data_as(C.c_char_p), size.ctypes.data_as(C.c_void_p),
-                                           strides.ctypes.data_as(C.c_void_p), sp.ctypes.data_as(C.c_void_p),
-                                           C.byref(per), C.byref(sur), C.byref(dia))
+    rc = lib().rb_calculate_coefficients2D(ptr(msk), ptr(size), ptr(strides), ptr(sp), C.byref(per), C.byref(sur),
+                                           C.byref(dia))
     if rc:
         check(rc, "Calculation of Shape coefficients failed.")
     return per.value, sur.value, dia.value
@@ -64,24 +61,18 @@ def calculate_coefficients2D(mask, pixelSpacing):
 
 def coefficients_device(mask_t, spacing_zyx):
     """same for a contiguous uint8 CUDA tensor [Z, Y, X]; returns (area, volume, diameters, n_vertices)"""
-    import torch
-
     sp = (C.c_double * 3)(*[float(s) for s in spacing_zyx])
     out = (C.c_double * 7)()
     Z, Y, X = mask_t.shape
-    check(lib().rb_shape_coefficients_dev(C.c_void_p(mask_t.data_ptr()), Z, Y, X, sp, out,
-                                          C.c_void_p(torch.cuda.current_stream().cuda_stream)), "shape coefficients")
+    check(lib().rb_shape_coefficients_dev(ptr(mask_t), Z, Y, X, sp, out, stream()), "shape coefficients")
     return out[0], out[1], tuple(out[2:6]), int(out[6])
 
 
 def moments_device(mask_t):
     """exact integer sums {N, z, y, x, zz, zy, zx, yy, yx, xx} over the ROI voxels (Python ints)"""
-    import torch
-
     out = (C.c_ulonglong * 10)()
     Z, Y, X = mask_t.shape
-    check(lib().rb_shape_moments_dev(C.c_void_p(mask_t.data_ptr()), Z, Y, X, out,
-                                     C.c_void_p(torch.cuda.current_stream().cuda_stream)), "shape moments")
+    check(lib().rb_shape_moments_dev(ptr(mask_t), Z, Y, X, out, stream()), "shape moments")
     return [int(v) for v in out]
 
 

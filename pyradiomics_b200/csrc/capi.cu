@@ -6,6 +6,7 @@
 
 #include "common.cuh"
 #include "host_common.hpp"
+#include "pixel.cuh"
 
 namespace rb {
 
@@ -120,11 +121,11 @@ static const char* kGldmNames[] = {"DependenceEntropy", "DependenceNonUniformity
 static const char* kNgtdmNames[] = {"Busyness", "Coarseness", "Complexity", "Contrast", "Strength"};
 static const char** kNames[5] = {kGlcmNames, kGlrlmNames, kGlszmNames, kGldmNames, kNgtdmNames};
 
-static VoxSettings to_settings(const rb_voxel_settings* s) {
-  VoxSettings v;
-  static_assert(sizeof(VoxSettings) == sizeof(rb_voxel_settings), "settings mirror out of sync");
-  memcpy(&v, s, sizeof v);
-  return v;
+// RB_ERR_ARG unless every code is an rb_dtype.  Each entry point that takes pixel types runs it before any CUDA call.
+static int check_dtypes(std::initializer_list<int> codes) {
+  for (int dt : codes)
+    if (!dtype_valid(dt)) return fail(RB_ERR_ARG, "unknown dtype code %d", dt);
+  return RB_OK;
 }
 
 __global__ void maps_to_f32_kernel(const double* __restrict__ src, long long sp, float* __restrict__ dst, long long dp,
@@ -182,7 +183,7 @@ int rb_pack_levels_dev(const int32_t* image_dev, const uint8_t* mask_dev, long l
 int rb_glcm_alive_angles_dev(const void* levels_dev, int level_bytes, const uint8_t* centers_dev, int Z, int Y, int X,
                              const rb_voxel_settings* settings, uint32_t* alive_dev, void* stream) {
   VoxParams P;
-  if (fill_vox_params(C_GLCM, Z, Y, X, to_settings(settings), P)) return fail(RB_ERR_ARG, "bad voxel settings");
+  if (fill_vox_params(C_GLCM, Z, Y, X, *settings, P)) return fail(RB_ERR_ARG, "bad voxel settings");
   return glcm_alive_angles(levels_dev, level_bytes, centers_dev, P, alive_dev, (cudaStream_t)stream);
 }
 
@@ -194,7 +195,7 @@ int rb_voxel_features_dev(int cls, const void* levels_dev, int level_bytes, cons
   if (out_is_f32) return fail(RB_ERR_UNSUPPORTED, "float32 maps not implemented yet");
   if (z0 < 0 || z1 > Z || z0 > z1) return fail(RB_ERR_ARG, "bad z range");
   VoxParams P;
-  if (fill_vox_params(cls, Z, Y, X, to_settings(settings), P)) return fail(RB_ERR_ARG, "bad voxel settings");
+  if (fill_vox_params(cls, Z, Y, X, *settings, P)) return fail(RB_ERR_ARG, "bad voxel settings");
   if (alive_host && cls == C_GLCM) memcpy(P.alive, alive_host, sizeof P.alive);
   if (!force_generic() && glcm_fast_applicable(cls, level_bytes, P))
     return glcm_fast_launch(levels_dev, centers_dev, P, (double*)out_dev, out_feature_stride, z0, z1, out_z0,
@@ -321,12 +322,12 @@ void rb_glszm_release(void* handle) { glszm_release(handle); }
 
 int rb_minmax_dev(const void* image_dev, int dtype, const uint8_t* mask_dev, long long nvoxels, long long* keys_dev,
                   void* stream) {
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   return minmax_launch(image_dev, dtype, mask_dev, nvoxels, keys_dev, (cudaStream_t)stream);
 }
 int rb_digitize_dev(const void* image_dev, int dtype, const uint8_t* mask_dev, long long nvoxels, const double* edges_dev,
                     int nedges, int32_t* out_dev, void* stream) {
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   if (nedges < 1) return fail(RB_ERR_ARG, "need at least one bin edge");
   return digitize_launch(image_dev, dtype, mask_dev, nvoxels, edges_dev, nedges, out_dev, (cudaStream_t)stream);
 }
@@ -334,7 +335,7 @@ int rb_digitize_dev(const void* image_dev, int dtype, const uint8_t* mask_dev, l
 int rb_pointwise_image_dev(const void* img_dev, int dtype, long long nvoxels, int kind, double c, double* out_dev,
                            void* stream) {
   if (!img_dev || !out_dev) return fail(RB_ERR_ARG, "pointwise image: null argument");
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   if (kind < RB_PW_SQUARE || kind > RB_PW_EXPONENTIAL) return fail(RB_ERR_ARG, "pointwise image: unknown kind %d", kind);
   if (nvoxels < 1) return fail(RB_ERR_ARG, "pointwise image: %lld voxels", nvoxels);
   return pointwise_image_launch(img_dev, dtype, nvoxels, kind, c, out_dev, (cudaStream_t)stream);
@@ -343,7 +344,7 @@ int rb_pointwise_image_dev(const void* img_dev, int dtype, long long nvoxels, in
 int rb_gradient_magnitude_dev(const void* img_dev, int dtype, int Z, int Y, int X, const double* weights_zyx,
                               double* out_dev, void* stream) {
   if (!img_dev || !weights_zyx || !out_dev) return fail(RB_ERR_ARG, "gradient magnitude: null argument");
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   if (Z < 1 || Y < 1 || X < 1) return fail(RB_ERR_ARG, "gradient magnitude: empty volume %d x %d x %d", Z, Y, X);
   return gradient_magnitude_launch(img_dev, dtype, Z, Y, X, weights_zyx, out_dev, (cudaStream_t)stream);
 }
@@ -352,7 +353,7 @@ int rb_gradient_magnitude_dev(const void* img_dev, int dtype, int Z, int Y, int 
 int rb_roi_moments_dev(const void* img_dev, int dtype, const uint8_t* mask_dev, long long nvoxels, int passes,
                        void* scratch_dev, double* out_dev, void* stream) {
   if (!img_dev || !scratch_dev || !out_dev) return fail(RB_ERR_ARG, "roi moments: null argument");
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   if (nvoxels < 1) return fail(RB_ERR_ARG, "roi moments: %lld voxels", nvoxels);
   if (passes != 1 && passes != 2) return fail(RB_ERR_ARG, "roi moments: passes must be 1 or 2, got %d", passes);
   return roi_moments_launch(img_dev, dtype, mask_dev, nvoxels, passes, scratch_dev, out_dev, (cudaStream_t)stream);
@@ -361,7 +362,7 @@ int rb_roi_moments_dev(const void* img_dev, int dtype, const uint8_t* mask_dev, 
 int rb_normalize_dev(const void* img_dev, int dtype, long long nvoxels, double mean, double sigma, int remove_outliers,
                      double outliers, double scale, double* out_dev, void* stream) {
   if (!img_dev || !out_dev) return fail(RB_ERR_ARG, "normalize: null argument");
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   if (nvoxels < 1) return fail(RB_ERR_ARG, "normalize: %lld voxels", nvoxels);
   return normalize_launch(img_dev, dtype, nvoxels, mean, sigma, remove_outliers != 0, outliers, scale, out_dev,
                           (cudaStream_t)stream);
@@ -370,7 +371,7 @@ int rb_normalize_dev(const void* img_dev, int dtype, long long nvoxels, double m
 int rb_resegment_dev(const void* img_dev, int dtype, const uint8_t* mask_dev, long long nvoxels, double lower,
                      double upper, int nthresholds, uint8_t* out_dev, unsigned long long* counts_dev, void* stream) {
   if (!img_dev || !mask_dev || !out_dev || !counts_dev) return fail(RB_ERR_ARG, "resegment: null argument");
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   if (nvoxels < 1) return fail(RB_ERR_ARG, "resegment: %lld voxels", nvoxels);
   if (nthresholds != 1 && nthresholds != 2) return fail(RB_ERR_ARG, "resegment: %d thresholds (1 or 2)", nthresholds);
   return resegment_launch(img_dev, dtype, mask_dev, nvoxels, lower, upper, nthresholds == 2, out_dev, counts_dev,
@@ -387,6 +388,7 @@ int rb_bspline_prefilter_dev(double* coeffs_dev, int Z, int Y, int X, void* stre
 int rb_resample_dev(const void* src_dev, int src_dtype, const int* in_size_zyx, void* dst_dev, int dst_dtype, const int* out_size_zyx,
                     const double* start_zyx, const double* step_zyx, int interpolator, double default_value, void* stream) {
   if (!src_dev || !dst_dev || !in_size_zyx || !out_size_zyx || !start_zyx || !step_zyx) return fail(RB_ERR_ARG, "null argument");
+  if (int rc = check_dtypes({src_dtype, dst_dtype})) return rc;
   return resample_launch(src_dev, src_dtype, in_size_zyx, dst_dev, dst_dtype, out_size_zyx, start_zyx, step_zyx, interpolator,
                          default_value, (cudaStream_t)stream);
 }
@@ -394,11 +396,13 @@ int rb_resample_dev(const void* src_dev, int src_dtype, const int* in_size_zyx, 
 int rb_lbp3d_dev(const void* img_dev, int img_dtype, int sample_dtype, const uint8_t* roi_u8_dev, int Z, int Y, int X,
                  const double* vertices_host, int nv, const double* harmonics_host, int levels, double* coeff_scratch_dev,
                  double* out_dev, void* stream) {
+  if (int rc = check_dtypes({img_dtype, sample_dtype})) return rc;
   return lbp3d_launch(img_dev, img_dtype, sample_dtype, roi_u8_dev, Z, Y, X, vertices_host, nv, harmonics_host, levels,
                       coeff_scratch_dev, out_dev, (cudaStream_t)stream);
 }
 int rb_lbp2d_dev(const void* img_dev, int dtype, int Z, int Y, int X, int axis, int P, const double* rp_host,
                  const double* cp_host, int method, double* out_dev, void* stream) {
+  if (int rc = check_dtypes({dtype})) return rc;
   return lbp2d_launch(img_dev, dtype, Z, Y, X, axis, P, rp_host, cp_host, method, out_dev, (cudaStream_t)stream);
 }
 
@@ -472,7 +476,7 @@ int rb_firstorder_voxel_dev(const void* image_dev, int dtype, const uint8_t* mas
                             const void* levels_dev, int level_bytes, int Z, int Y, int X, int rz, int ry, int rx,
                             double voxelArrayShift, double voxel_volume, double initValue, double* out_dev,
                             long long out_feature_stride, int z0, int z1, int out_z0, void* stream) {
-  if (dtype < 0 || dtype > 6) return fail(RB_ERR_ARG, "unknown dtype code %d", dtype);
+  if (int rc = check_dtypes({dtype})) return rc;
   if (level_bytes != 1 && level_bytes != 2) return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
   if (rz < 0 || ry < 0 || rx < 0 || z0 < 0 || z1 > Z || z0 > z1) return fail(RB_ERR_ARG, "bad window / z range");
   return firstorder_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, level_bytes, Z, Y, X, rz, ry, rx,

@@ -12,23 +12,9 @@
 // All are HBM-streaming kernels: every thread handles consecutive x so loads/stores coalesce; the
 // wavelet pass reads its 6 taps through L1 (neighbouring threads share them).
 #include "common.cuh"
+#include "pixel.cuh"
 
 namespace rb {
-
-enum DType { DT_I16 = 0, DT_I32 = 1, DT_F32 = 2, DT_F64 = 3, DT_U8 = 4, DT_U16 = 5, DT_I64 = 6 };
-
-template <typename T> __device__ __forceinline__ double as_f64(const void* p, long long i) { return (double)((const T*)p)[i]; }
-__device__ __forceinline__ double load_any(const void* p, int dt, long long i) {
-  switch (dt) {
-    case DT_I16: return as_f64<int16_t>(p, i);
-    case DT_I32: return as_f64<int32_t>(p, i);
-    case DT_F32: return as_f64<float>(p, i);
-    case DT_F64: return as_f64<double>(p, i);
-    case DT_U8: return as_f64<uint8_t>(p, i);
-    case DT_U16: return as_f64<uint16_t>(p, i);
-    default: return as_f64<long long>(p, i);
-  }
-}
 
 // order-preserving map double <-> signed 64-bit, so atomicMin/atomicMax work on doubles
 __device__ __forceinline__ long long f64_key(double v) {
@@ -43,7 +29,7 @@ minmax_kernel(const void* __restrict__ img, int dt, const uint8_t* __restrict__ 
   long long cnt = 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     if (mask && !mask[i]) continue;
-    const double v = load_any(img, dt, i);
+    const double v = load_f64(img, dt, i);
     lo = v < lo ? v : lo; hi = v > hi ? v : hi; cnt++;
   }
   for (int o = 16; o; o >>= 1) {
@@ -65,7 +51,7 @@ template <int KIND>
 __global__ void __launch_bounds__(256)
 pointwise_image_kernel(const void* __restrict__ img, int dt, long long n, double c, double* __restrict__ out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const double x = load_any(img, dt, i);
+    const double x = load_f64(img, dt, i);
     double r;
     if (KIND == RB_PW_SQUARE) {
       const double t = __dmul_rn(c, x);
@@ -104,12 +90,12 @@ gradient_magnitude_kernel(const void* __restrict__ img, int dt, int Z, int Y, in
   const int dxm = x > 0 ? -1 : 0, dxp = x < X - 1 ? 1 : 0;
   const int dym = y > 0 ? -X : 0, dyp = y < Y - 1 ? X : 0;
   long long i = (long long)z0 * plane + (long long)y * X + x;
-  double f0 = load_any(img, dt, i);
-  double fm = z0 > 0 ? load_any(img, dt, i - plane) : f0;
+  double f0 = load_f64(img, dt, i);
+  double fm = z0 > 0 ? load_f64(img, dt, i - plane) : f0;
   for (int z = z0; z < z1; z++, i += plane) {
-    const double fp = z < Z - 1 ? load_any(img, dt, i + plane) : f0;
-    const double gx = central_diff(load_any(img, dt, i + dxm), f0, load_any(img, dt, i + dxp), wx);
-    const double gy = central_diff(load_any(img, dt, i + dym), f0, load_any(img, dt, i + dyp), wy);
+    const double fp = z < Z - 1 ? load_f64(img, dt, i + plane) : f0;
+    const double gx = central_diff(load_f64(img, dt, i + dxm), f0, load_f64(img, dt, i + dxp), wx);
+    const double gy = central_diff(load_f64(img, dt, i + dym), f0, load_f64(img, dt, i + dyp), wy);
     const double gz = central_diff(fm, f0, fp, wz);
     out[i] = sqrt(__dadd_rn(__dadd_rn(__dadd_rn(0.0, __dmul_rn(gx, gx)), __dmul_rn(gy, gy)), __dmul_rn(gz, gz)));
     fm = f0;
@@ -178,7 +164,7 @@ roi_moments_kernel(const void* __restrict__ img, int dt, const uint8_t* __restri
   const double mu = PASS == 2 ? __ddiv_rn(res[2], res[0]) : 0.0;
   for (long long i = (long long)blockIdx.x * MOM_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * MOM_THREADS) {
     if (mask && !mask[i]) continue;
-    const double x = load_any(img, dt, i);
+    const double x = load_f64(img, dt, i);
     if (PASS == 1) {
       a.n++;
       a.nnan += x != x;
@@ -218,7 +204,7 @@ __global__ void __launch_bounds__(256)
 normalize_kernel(const void* __restrict__ img, int dt, long long n, double mean, double inv_sigma, int clamp,
                  double outliers, double scale, double* __restrict__ out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    double v = __dmul_rn(__dsub_rn(load_any(img, dt, i), mean), inv_sigma);
+    double v = __dmul_rn(__dsub_rn(load_f64(img, dt, i), mean), inv_sigma);
     if (clamp) {
       if (v > outliers) v = outliers;
       if (v < -outliers) v = -outliers;
@@ -237,7 +223,7 @@ resegment_kernel(const void* __restrict__ img, int dt, const uint8_t* __restrict
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     uint8_t k = 0;
     if (mask[i]) {
-      const double x = load_any(img, dt, i);
+      const double x = load_f64(img, dt, i);
       k = x >= lo && (!two || x <= hi);
       roi++;
       kept += k;
@@ -265,7 +251,7 @@ digitize_kernel(const void* __restrict__ img, int dt, const uint8_t* __restrict_
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     int32_t b = 0;
     if (!mask || mask[i]) {
-      const double x = load_any(img, dt, i);
+      const double x = load_f64(img, dt, i);
       int lo = 0, hi = ne;
       while (lo < hi) { const int mid = (lo + hi) >> 1; if (e[mid] <= x) lo = mid + 1; else hi = mid; }
       b = lo;

@@ -2,20 +2,9 @@
 // intensities + discretised levels and evaluates firstorder_voxel<> (firstorder.cuh).
 #include "common.cuh"
 #include "firstorder.cuh"
+#include "pixel.cuh"
 
 namespace rb {
-
-__device__ __forceinline__ double fo_load(const void* p, int dt, long long i) {
-  switch (dt) {
-    case 0: return (double)((const int16_t*)p)[i];
-    case 1: return (double)((const int32_t*)p)[i];
-    case 2: return (double)((const float*)p)[i];
-    case 3: return ((const double*)p)[i];
-    case 4: return (double)((const uint8_t*)p)[i];
-    case 5: return (double)((const uint16_t*)p)[i];
-    default: return (double)((const long long*)p)[i];
-  }
-}
 
 struct FoParams {
   int Z, Y, X, rz, ry, rx, z0, z1, out_z0, dtype, level_bytes;
@@ -48,7 +37,7 @@ firstorder_kernel(const void* __restrict__ img, const uint8_t* __restrict__ mask
           if (zz < 0 || zz >= P.Z || yy < 0 || yy >= P.Y || xx < 0 || xx >= P.X) continue;
           const long long j = (long long)zz * plane + (long long)yy * P.X + xx;
           if (mask && !mask[j]) continue;
-          xs[n++] = fo_load(img, P.dtype, j);
+          xs[n++] = load_f64(img, P.dtype, j);
           w[wn] = P.level_bytes == 1 ? (uint16_t)((const uint8_t*)lev)[j] : ((const uint16_t*)lev)[j];
         }
     double f[FIRSTORDER_NF];

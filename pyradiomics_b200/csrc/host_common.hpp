@@ -6,6 +6,7 @@
 
 #include <vector>
 
+#include "../../include/b200radiomics.h"
 #include "vox_features.cuh"
 
 namespace rb {
@@ -71,18 +72,7 @@ inline double angle_weight(const int* a3, const double* spacing_zyx, int weighti
   return glcm ? exp(-dist * dist) : dist;
 }
 
-struct VoxSettings {      // mirror of rb_voxel_settings in include/b200radiomics.h
-  int kernelRadius;
-  int force2D, force2Ddimension;
-  int ndist; int distances[8];
-  int symmetricalGLCM;
-  int weighting;
-  double spacing_zyx[3];
-  int gldm_a;
-  double initValue;
-  int Ng;               // max level of the ROI
-  int n_roi_levels;
-};
+using VoxSettings = rb_voxel_settings;
 
 // Build the launch parameter block of one class for a (Z,Y,X) volume.  Returns 0 or a negative
 // error (-3 bad argument / unsupported size).

@@ -26,7 +26,6 @@ lbp2d_kernel(const void* __restrict__ img, int dt, int Z, int Y, int X, int axis
 int lbp2d_launch(const void* img, int dt, int Z, int Y, int X, int axis, int P, const double* rp, const double* cp, int method,
                  double* out, cudaStream_t st) {
   if (!img || !rp || !cp || !out) return fail(RB_ERR_ARG, "lbp2d: null argument");
-  if (dt < 0 || dt > 6) return fail(RB_ERR_ARG, "lbp2d: unknown dtype code %d", dt);
   if (Z < 1 || Y < 1 || X < 1) return fail(RB_ERR_ARG, "lbp2d: empty volume %d x %d x %d", Z, Y, X);
   if (axis < 0 || axis > 2) return fail(RB_ERR_ARG, "lbp2d: axis %d (0..2)", axis);
   if (method < LBP2D_DEFAULT || method > LBP2D_VAR) return fail(RB_ERR_ARG, "lbp2d: unknown method code %d", method);

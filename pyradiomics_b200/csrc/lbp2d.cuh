@@ -11,7 +11,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#include "lbp3d.cuh"                             // RB_HD, lbp_load
+#include "lbp3d.cuh"                             // RB_HD, load_f64
 
 namespace rb {
 
@@ -48,7 +48,7 @@ struct Lbp2dSlice {
 
 RB_HD double lbp2d_pixel_value(const Lbp2dSlice& s, long long r, long long c) {
   if (r < 0 || r >= s.rows || c < 0 || c >= s.cols) return 0.0;
-  return lbp_load(s.img, s.dt, s.base + r * s.rs + c * s.cs);
+  return load_f64(s.img, s.dt, s.base + r * s.rs + c * s.cs);
 }
 
 RB_HD double lbp2d_sample(const Lbp2dSlice& s, double r, double c) {

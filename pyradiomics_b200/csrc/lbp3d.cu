@@ -15,7 +15,7 @@ int bspline_prefilter_launch(double* coeffs, int Z, int Y, int X, cudaStream_t s
 
 __global__ void __launch_bounds__(256) lbp3d_to_f64_kernel(const void* __restrict__ img, int dt, long long n, double* __restrict__ out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    out[i] = lbp_load(img, dt, i);
+    out[i] = load_f64(img, dt, i);
 }
 
 __global__ void __launch_bounds__(128)
@@ -35,7 +35,6 @@ lbp3d_kernel(const double* __restrict__ coef, const void* __restrict__ img, int 
 int lbp3d_launch(const void* img, int img_dt, int sample_dt, const uint8_t* roi, int Z, int Y, int X, const double* vertices,
                  int nv, const double* harmonics, int levels, double* coeff_scratch, double* out, cudaStream_t st) {
   if (!img || !roi || !vertices || !harmonics || !coeff_scratch || !out) return fail(RB_ERR_ARG, "lbp3d: null argument");
-  if (img_dt < 0 || img_dt > 6 || sample_dt < 0 || sample_dt > 6) return fail(RB_ERR_ARG, "lbp3d: unknown dtype code");
   if (Z < 1 || Y < 1 || X < 1 || nv < 1 || levels < 1) return fail(RB_ERR_ARG, "lbp3d: empty volume, sphere or level list");
   if (nv > LBP_MAX_NV || levels > LBP_MAX_LEVELS)
     return fail(RB_ERR_UNSUPPORTED, "lbp3d: %d vertices / %d levels (at most %d, icosphere subdivision 2, and %d)", nv, levels,

@@ -10,22 +10,13 @@
 #include <math.h>
 #include <stdint.h>
 
-#ifndef RB_HD
-#ifdef __CUDACC__
-#define RB_HD __host__ __device__ __forceinline__
-#else
-#define RB_HD inline
-#endif
-#endif
+#include "pixel.cuh"                              // RB_HD, rb_dtype, load_f64
 
 namespace rb {
 
 constexpr int LBP_MAX_NV = 162;                 // icosphere subdivision 2
 constexpr int LBP_MAX_LEVELS = 4;
 constexpr int LBP_MAX_KPOS = LBP_MAX_LEVELS * (LBP_MAX_LEVELS + 1) / 2;    // harmonics with m >= 0
-
-// dtype codes of rb_minmax_dev
-enum { LBP_I16 = 0, LBP_I32 = 1, LBP_F32 = 2, LBP_F64 = 3, LBP_U8 = 4, LBP_U16 = 5, LBP_I64 = 6 };
 
 // Sphere vertices and harmonics table; passed by value to the kernel (__grid_constant__, < 32 KB of parameters).
 // y_re / y_im [v][n (n + 1) / 2 + m] = Y_n^m(vertex v) for m >= 0; Y_n^-m = (-1)^m conj(Y_n^m).
@@ -35,18 +26,6 @@ struct Lbp3dTables {
   double y_re[LBP_MAX_NV][LBP_MAX_KPOS];
   double y_im[LBP_MAX_NV][LBP_MAX_KPOS];
 };
-
-RB_HD double lbp_load(const void* p, int dt, long long i) {
-  switch (dt) {
-    case LBP_I16: return (double)((const int16_t*)p)[i];
-    case LBP_I32: return (double)((const int32_t*)p)[i];
-    case LBP_F32: return (double)((const float*)p)[i];
-    case LBP_F64: return ((const double*)p)[i];
-    case LBP_U8: return (double)((const uint8_t*)p)[i];
-    case LBP_U16: return (double)((const uint16_t*)p)[i];
-    default: return (double)((const long long*)p)[i];
-  }
-}
 
 // SciPy's cast of an interpolated value to an integer output: +-0.5 towards the sign, clamp, truncate
 RB_HD double lbp_round_clamp(double v, double lo, double hi) {
@@ -58,12 +37,12 @@ RB_HD double lbp_round_clamp(double v, double lo, double hi) {
 
 RB_HD double lbp_cast(double v, int dt) {
   switch (dt) {
-    case LBP_F64: return v;
-    case LBP_F32: return (double)(float)v;
-    case LBP_I16: return lbp_round_clamp(v, -32768.0, 32767.0);
-    case LBP_I32: return lbp_round_clamp(v, -2147483648.0, 2147483647.0);
-    case LBP_U8: return lbp_round_clamp(v, 0.0, 255.0);
-    case LBP_U16: return lbp_round_clamp(v, 0.0, 65535.0);
+    case RB_DT_FLOAT64: return v;
+    case RB_DT_FLOAT32: return (double)(float)v;
+    case RB_DT_INT16: return lbp_round_clamp(v, -32768.0, 32767.0);
+    case RB_DT_INT32: return lbp_round_clamp(v, -2147483648.0, 2147483647.0);
+    case RB_DT_UINT8: return lbp_round_clamp(v, 0.0, 255.0);
+    case RB_DT_UINT16: return lbp_round_clamp(v, 0.0, 65535.0);
     default: return lbp_round_clamp(v, -9223372036854775808.0, 9223372036854774784.0);
   }
 }
@@ -121,7 +100,7 @@ RB_HD double lbp_re_csqrt(double re, double im) {
 RB_HD void lbp3d_voxel(const double* __restrict__ coef, const void* __restrict__ img, int img_dt, int Z, int Y, int X, int z,
                        int y, int x, const Lbp3dTables& T, double* __restrict__ out, long long ostride) {
   const int nv = T.nv, L = T.levels;
-  const double centre = lbp_load(img, img_dt, ((long long)z * Y + y) * X + x);
+  const double centre = load_f64(img, img_dt, ((long long)z * Y + y) * X + x);
   double f[LBP_MAX_NV];
   double sum = 0.0;
   for (int v = 0; v < nv; v++) {
@@ -141,7 +120,7 @@ RB_HD void lbp3d_voxel(const double* __restrict__ coef, const void* __restrict__
   }
   m2 /= nv;
   m4 /= nv;
-  const double eps = T.sample_dt == LBP_F32 ? 1.1920928955078125e-07 : 2.220446049250313e-16;
+  const double eps = T.sample_dt == RB_DT_FLOAT32 ? 1.1920928955078125e-07 : 2.220446049250313e-16;
   const double zero = eps * mean;
   out[(long long)L * ostride] = m2 <= zero * zero ? (double)NAN : m4 / (m2 * m2) - 3.0;
 

@@ -10,6 +10,7 @@
 //                              ITK's ResampleImageFilter (pinned: the reference's `_resampling` baselines are reproduced
 //                              exactly with truncation, not with rounding).
 #include "common.cuh"
+#include "pixel.cuh"
 
 namespace rb {
 
@@ -88,28 +89,16 @@ __device__ __forceinline__ int mirror(int i, int n) {
 }
 
 enum { RS_NEAREST = 0, RS_LINEAR = 1, RS_BSPLINE3 = 3 };
-enum { PT_I16 = 0, PT_I32 = 1, PT_F32 = 2, PT_F64 = 3, PT_U8 = 4, PT_U16 = 5, PT_I64 = 6 };
 
-__device__ __forceinline__ double src_value(const void* p, int dt, long long i) {
-  switch (dt) {
-    case PT_I16: return (double)((const int16_t*)p)[i];
-    case PT_I32: return (double)((const int32_t*)p)[i];
-    case PT_F32: return (double)((const float*)p)[i];
-    case PT_F64: return ((const double*)p)[i];
-    case PT_U8: return (double)((const uint8_t*)p)[i];
-    case PT_U16: return (double)((const uint16_t*)p)[i];
-    default: return (double)((const long long*)p)[i];
-  }
-}
 // ITK ResampleImageFilter::CastPixelWithBoundsChecking: clamp to the pixel range, then static_cast (truncation)
 __device__ __forceinline__ void store_value(void* p, int dt, long long i, double v) {
   switch (dt) {
-    case PT_I16: ((int16_t*)p)[i] = (int16_t)(v < -32768.0 ? -32768.0 : v > 32767.0 ? 32767.0 : v); break;
-    case PT_I32: ((int32_t*)p)[i] = (int32_t)(v < -2147483648.0 ? -2147483648.0 : v > 2147483647.0 ? 2147483647.0 : v); break;
-    case PT_F32: ((float*)p)[i] = (float)v; break;
-    case PT_F64: ((double*)p)[i] = v; break;
-    case PT_U8: ((uint8_t*)p)[i] = (uint8_t)(v < 0.0 ? 0.0 : v > 255.0 ? 255.0 : v); break;
-    case PT_U16: ((uint16_t*)p)[i] = (uint16_t)(v < 0.0 ? 0.0 : v > 65535.0 ? 65535.0 : v); break;
+    case RB_DT_INT16: ((int16_t*)p)[i] = (int16_t)(v < -32768.0 ? -32768.0 : v > 32767.0 ? 32767.0 : v); break;
+    case RB_DT_INT32: ((int32_t*)p)[i] = (int32_t)(v < -2147483648.0 ? -2147483648.0 : v > 2147483647.0 ? 2147483647.0 : v); break;
+    case RB_DT_FLOAT32: ((float*)p)[i] = (float)v; break;
+    case RB_DT_FLOAT64: ((double*)p)[i] = v; break;
+    case RB_DT_UINT8: ((uint8_t*)p)[i] = (uint8_t)(v < 0.0 ? 0.0 : v > 255.0 ? 255.0 : v); break;
+    case RB_DT_UINT16: ((uint16_t*)p)[i] = (uint16_t)(v < 0.0 ? 0.0 : v > 65535.0 ? 65535.0 : v); break;
     default: ((long long*)p)[i] = (long long)v; break;
   }
 }
@@ -133,14 +122,14 @@ resample_kernel(const void* __restrict__ src, int src_dt, const __grid_constant_
     if (inside) {
       if (interp == RS_NEAREST) {
         const int z = (int)floor(cz + 0.5), y = (int)floor(cy + 0.5), x = (int)floor(cx + 0.5);       // RoundHalfIntegerUp
-        v = src_value(src, src_dt, (long long)min(max(z, 0), G.iz - 1) * iplane + (long long)min(max(y, 0), G.iy - 1) * G.ix + min(max(x, 0), G.ix - 1));
+        v = load_f64(src, src_dt, (long long)min(max(z, 0), G.iz - 1) * iplane + (long long)min(max(y, 0), G.iy - 1) * G.ix + min(max(x, 0), G.ix - 1));
       } else if (interp == RS_LINEAR) {
         const double fz = floor(cz), fy = floor(cy), fx = floor(cx);
         const double wz = cz - fz, wy = cy - fy, wx = cx - fx;
         v = 0;
         for (int dz = 0; dz < 2; dz++) for (int dy = 0; dy < 2; dy++) for (int dx = 0; dx < 2; dx++) {
           const int z = min(max((int)fz + dz, 0), G.iz - 1), y = min(max((int)fy + dy, 0), G.iy - 1), x = min(max((int)fx + dx, 0), G.ix - 1);
-          v += (dz ? wz : 1 - wz) * (dy ? wy : 1 - wy) * (dx ? wx : 1 - wx) * src_value(src, src_dt, (long long)z * iplane + (long long)y * G.ix + x);
+          v += (dz ? wz : 1 - wz) * (dy ? wy : 1 - wy) * (dx ? wx : 1 - wx) * load_f64(src, src_dt, (long long)z * iplane + (long long)y * G.ix + x);
         }
       } else {
         // cubic B-spline over the 4x4x4 neighbourhood starting at floor(c) - 1, mirrored at the borders;
@@ -204,7 +193,7 @@ int bspline_prefilter_launch(double* coeffs, int Z, int Y, int X, cudaStream_t s
 int resample_launch(const void* src, int src_dt, const int* in_size, void* dst, int dst_dt, const int* out_size, const double* start,
                     const double* step, int interp, double default_value, cudaStream_t st) {
   if (interp != RS_NEAREST && interp != RS_LINEAR && interp != RS_BSPLINE3) return fail(RB_ERR_UNSUPPORTED, "interpolator %d (0 nearest, 1 linear, 3 cubic B-spline)", interp);
-  if (interp == RS_BSPLINE3 && src_dt != PT_F64) return fail(RB_ERR_ARG, "the B-spline evaluation reads float64 coefficients");
+  if (interp == RS_BSPLINE3 && src_dt != RB_DT_FLOAT64) return fail(RB_ERR_ARG, "the B-spline evaluation reads float64 coefficients");
   ResampleGeom G;
   G.iz = in_size[0]; G.iy = in_size[1]; G.ix = in_size[2];
   G.oz = out_size[0]; G.oy = out_size[1]; G.ox = out_size[2];

@@ -612,7 +612,6 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
         return [0] * (3 - nd) + rad
 
     def _calculateVoxels(self):
-        import ctypes as C
         img = imageoperations._to_device(self._raw)
         msk = imageoperations._to_device(self.maskArray)
         lev = self._levels_dev
@@ -625,11 +624,11 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
         out = torch.empty((nf, Z, Y, X), dtype=torch.float64, device=img.device)
         vv = float(np.multiply.reduce(self.pixelSpacing))
         idx = [k for k, n in enumerate(self.NAMES) if self.enabledFeatures.get(n)]
-        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
+        ptr = _lib.ptr
         _lib.check(_lib.lib().rb_firstorder_voxel_dev(
-            ptr(img), imageoperations._TORCH_DT[img.dtype], ptr(msk), ptr(centers), ptr(lev), voxel.level_bytes(lev), Z, Y, X,
-            rz, ry, rx, C.c_double(float(self.voxelArrayShift)), C.c_double(vv), C.c_double(float(self.settings.get("initValue", 0))),
-            ptr(out), C.c_longlong(out.stride(0)), 0, Z, 0, C.c_void_p(torch.cuda.current_stream().cuda_stream)), "firstorder")
+            ptr(img), _lib.TORCH_DTYPE_CODE[img.dtype], ptr(msk), ptr(centers), ptr(lev), voxel.level_bytes(lev), Z, Y, X,
+            rz, ry, rx, float(self.voxelArrayShift), vv, float(self.settings.get("initValue", 0)), ptr(out), out.stride(0), 0, Z,
+            0, _lib.stream()), "firstorder")
         if not idx:
             return
         host = torch.empty((len(idx), Z, Y, X), dtype=torch.float64, pin_memory=True)     # enabled maps only

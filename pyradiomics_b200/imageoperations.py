@@ -27,29 +27,17 @@ import numpy as np
 import torch
 
 from . import image as I
-from ._lib import check, lib
+from ._lib import DTYPE_CODE, NP_OF_TORCH, TORCH_DTYPE_CODE, TORCH_OF_NP, check, lib, ptr, stream
 
 logger = logging.getLogger("radiomics.imageoperations")
 
-_DT = {np.dtype("int16"): 0, np.dtype("int32"): 1, np.dtype("float32"): 2, np.dtype("float64"): 3,
-       np.dtype("uint8"): 4, np.dtype("uint16"): 5, np.dtype("int64"): 6}
-_TORCH_DT = {torch.int16: 0, torch.int32: 1, torch.float32: 2, torch.float64: 3, torch.uint8: 4, torch.int64: 6}
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
+# the names this module gave the pointer, stream and pixel-type helpers before _lib held them; existing callers use them
+_ptr, _stream, _DT = ptr, stream, DTYPE_CODE
 
 def _dev():
     return torch.device("cuda", torch.cuda.current_device())
 
 
-_TORCH_OF_NP = {np.int16: torch.int16, np.int32: torch.int32, np.float32: torch.float32, np.float64: torch.float64,
-                np.uint8: torch.uint8, np.int64: torch.int64}
 _STAGE = {"bufs": None, "pool": None}
 _STAGE_CHUNK = 32 << 20
 _STAGE_MIN = 64 << 20
@@ -84,7 +72,7 @@ def _upload_staged(a):
     for e in done:
         if e is not None:
             e.synchronize()                         # the staging blocks are reused by the next upload
-    return out.view(_TORCH_OF_NP[a.dtype.type]).reshape(a.shape)
+    return out.view(TORCH_OF_NP[a.dtype.type]).reshape(a.shape)
 
 
 def _to_device(arr):
@@ -93,7 +81,7 @@ def _to_device(arr):
         t = arr
         if t.dtype == torch.bool:
             t = t.to(torch.uint8)
-        if t.dtype not in _TORCH_DT:
+        if t.dtype not in TORCH_DTYPE_CODE:
             t = t.to(torch.float64)
         return t.to(_dev()).contiguous()
     a = np.asarray(arr)
@@ -101,12 +89,20 @@ def _to_device(arr):
         a = a.view(np.uint8)
     elif a.dtype == np.uint16:
         a = a.astype(np.int32)
-    elif a.dtype not in _DT:
+    elif a.dtype not in DTYPE_CODE:
         a = a.astype(np.float64)
     a = np.ascontiguousarray(a)
-    if a.nbytes >= _STAGE_MIN and a.dtype.type in _TORCH_OF_NP:
+    if a.nbytes >= _STAGE_MIN and a.dtype.type in TORCH_OF_NP:
         return _upload_staged(a)
     return torch.from_numpy(a).to(_dev())
+
+
+def _checked_source(x):
+    """contiguous CUDA tensor of a pixel type the device code reads, or ValueError"""
+    src = x.contiguous()
+    if src.dtype not in TORCH_DTYPE_CODE:
+        raise ValueError(f"unsupported pixel type {src.dtype}")
+    return src
 
 
 def _decode_key(k: int) -> float:
@@ -117,16 +113,12 @@ def _decode_key(k: int) -> float:
 def roi_minmax(img_t: torch.Tensor, mask_t: torch.Tensor | None):
     """(min, max, count) of the ROI, one streaming kernel (replaces builtin min()/max())."""
     keys = torch.tensor([2 ** 63 - 1, -(2 ** 63), 0], dtype=torch.int64, device=img_t.device)
-    check(lib().rb_minmax_dev(_ptr(img_t), _TORCH_DT[img_t.dtype], _ptr(mask_t), C.c_longlong(img_t.numel()), _ptr(keys),
-                              _stream()), "minmax")
+    check(lib().rb_minmax_dev(ptr(img_t), TORCH_DTYPE_CODE[img_t.dtype], ptr(mask_t), img_t.numel(), ptr(keys), stream()),
+          "minmax")
     k = keys.cpu().tolist()
     if k[2] == 0:
         raise ValueError("empty ROI")
     return _decode_key(k[0]), _decode_key(k[1]), k[2]
-
-
-_NP_OF_TORCH = {torch.int16: np.int16, torch.int32: np.int32, torch.float32: np.float32, torch.float64: np.float64,
-                torch.uint8: np.uint8, torch.int64: np.int64}
 
 
 def _edges_from_minmax(minimum, maximum, np_type, **kwargs):
@@ -158,7 +150,7 @@ def getBinEdges(parameterValues, **kwargs):
     """reference signature: 1-D array of the segmented voxel values -> bin edges."""
     t = _to_device(parameterValues).reshape(-1)
     mn, mx, _ = roi_minmax(t, None)
-    return _edges_from_minmax(mn, mx, _NP_OF_TORCH[t.dtype], **kwargs)
+    return _edges_from_minmax(mn, mx, NP_OF_TORCH[t.dtype], **kwargs)
 
 
 def bin_image_device(img_t: torch.Tensor, mask_t: torch.Tensor | None, minmax_reduce=None, **kwargs):
@@ -168,12 +160,12 @@ def bin_image_device(img_t: torch.Tensor, mask_t: torch.Tensor | None, minmax_re
     mn, mx, _ = roi_minmax(img_t, mask_t)
     if minmax_reduce is not None:
         mn, mx = minmax_reduce(mn, mx)
-    edges_native = _edges_from_minmax(mn, mx, _NP_OF_TORCH[img_t.dtype], **kwargs)
+    edges_native = _edges_from_minmax(mn, mx, NP_OF_TORCH[img_t.dtype], **kwargs)
     edges = np.ascontiguousarray(edges_native, dtype=np.float64)
     e_t = torch.from_numpy(edges).to(img_t.device)
     out = torch.empty(img_t.shape, dtype=torch.int32, device=img_t.device)
-    check(lib().rb_digitize_dev(_ptr(img_t), _TORCH_DT[img_t.dtype], _ptr(mask_t), C.c_longlong(img_t.numel()), _ptr(e_t),
-                                int(edges.size), _ptr(out), _stream()), "digitize")
+    check(lib().rb_digitize_dev(ptr(img_t), TORCH_DTYPE_CODE[img_t.dtype], ptr(mask_t), img_t.numel(), ptr(e_t),
+                                int(edges.size), ptr(out), stream()), "digitize")
     return out, edges_native
 
 
@@ -213,8 +205,6 @@ def cropToTumorMask(imageNode, maskNode, boundingBox, **kwargs):
 
 # ------------------------------------------------------------------------------------ resampling
 _INTERPOLATORS = {"sitkNearestNeighbor": 0, "sitkLinear": 1, "sitkBSpline": 3, 1: 0, 2: 1, 3: 3}      # (sitk enum values 1, 2, 3)
-_NP_DT = {np.dtype("int16"): 0, np.dtype("int32"): 1, np.dtype("float32"): 2, np.dtype("float64"): 3, np.dtype("uint8"): 4,
-          np.dtype("int64"): 6}
 
 
 def resample_device(arr_t: torch.Tensor, out_size_zyx, start_zyx, step_zyx, interpolator=3, default_value=0.0, out_dtype=None):
@@ -223,21 +213,21 @@ def resample_device(arr_t: torch.Tensor, out_size_zyx, start_zyx, step_zyx, inte
     clamped and truncated to `out_dtype` (default: the input's) like ITK's ResampleImageFilter"""
     src = arr_t.contiguous()
     out_dtype = out_dtype or src.dtype
-    if out_dtype not in _TORCH_DT:
+    if out_dtype not in TORCH_DTYPE_CODE:
         raise ValueError(f"unsupported pixel type {out_dtype}")
     Z, Y, X = src.shape
     dst = torch.empty(tuple(int(v) for v in out_size_zyx), dtype=out_dtype, device=src.device)
     if interpolator == 3:
         src = src.to(torch.float64).clone()
-        check(lib().rb_bspline_prefilter_dev(_ptr(src), Z, Y, X, _stream()), "bspline prefilter")
-    elif src.dtype not in _TORCH_DT:
+        check(lib().rb_bspline_prefilter_dev(ptr(src), Z, Y, X, stream()), "bspline prefilter")
+    elif src.dtype not in TORCH_DTYPE_CODE:
         src = src.to(torch.float64)
     isz = (C.c_int * 3)(Z, Y, X)
     osz = (C.c_int * 3)(*[int(v) for v in out_size_zyx])
     st = (C.c_double * 3)(*[float(v) for v in start_zyx])
     sp = (C.c_double * 3)(*[float(v) for v in step_zyx])
-    check(lib().rb_resample_dev(_ptr(src), _TORCH_DT[src.dtype], isz, _ptr(dst), _TORCH_DT[out_dtype], osz, st, sp, int(interpolator),
-                                C.c_double(float(default_value)), _stream()), "resample")
+    check(lib().rb_resample_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], isz, ptr(dst), TORCH_DTYPE_CODE[out_dtype], osz, st, sp,
+                                int(interpolator), float(default_value), stream()), "resample")
     return dst
 
 
@@ -337,8 +327,8 @@ def swt_level1_device(x: torch.Tensor, axes, lo, hi, z_range=None):
         x = x.contiguous()
         zb, ze = (0, Z) if z_range is None else (int(z_range[0]), int(z_range[1]))      # slab + halo in, interior planes out
         out = torch.empty((8, ze - zb, Y, X), dtype=torch.float64, device=x.device)
-        check(lib().rb_swt3d_dev(_ptr(x), Z, Y, X, lo.ctypes.data_as(C.c_void_p), hi.ctypes.data_as(C.c_void_p), int(lo.size),
-                                 _ptr(out), C.c_longlong(out.stride(0)), zb, ze, _stream()), "swt3d")
+        check(lib().rb_swt3d_dev(ptr(x), Z, Y, X, ptr(lo), ptr(hi), int(lo.size), ptr(out), out.stride(0), zb, ze, stream()),
+              "swt3d")
         res = {}
         for b in range(8):
             band = {2: b & 1, 1: b >> 1 & 1, 0: b >> 2 & 1}          # axis (0 = z, 1 = y, 2 = x) -> high-pass?
@@ -352,8 +342,8 @@ def swt_level1_device(x: torch.Tensor, axes, lo, hi, z_range=None):
         for key, t in cur.items():
             a = torch.empty_like(t)
             d = torch.empty_like(t)
-            check(lib().rb_swt_axis_dev(_ptr(t), Z, Y, X, int(ax), lo.ctypes.data_as(C.c_void_p), hi.ctypes.data_as(C.c_void_p),
-                                        int(lo.size), _ptr(a), _ptr(d), _stream()), "swt")
+            check(lib().rb_swt_axis_dev(ptr(t), Z, Y, X, int(ax), ptr(lo), ptr(hi), int(lo.size), ptr(a), ptr(d), stream()),
+                  "swt")
             nxt[key + "a"], nxt[key + "d"] = a, d
         cur = nxt
     return cur
@@ -474,9 +464,8 @@ def _rg_pass(src: torch.Tensor, axis: int, sigma_vox: float, order: int, out: to
         out = torch.empty((Z, Y, X), dtype=torch.float32, device=src.device)
     scratch = torch.empty((Z, Y, X), dtype=torch.float64, device=src.device)
     coef = recursive_gaussian_coefficients(sigma_vox, order)
-    check(lib().rb_recursive_gaussian_axis_dev(_ptr(src), int(src.dtype == torch.float32), Z, Y, X, int(axis),
-                                               coef.ctypes.data_as(C.c_void_p), _ptr(out), _ptr(scratch), C.c_double(scale),
-                                               int(accumulate), _stream()), "LoG")
+    check(lib().rb_recursive_gaussian_axis_dev(ptr(src), int(src.dtype == torch.float32), Z, Y, X, int(axis),
+                                               ptr(coef), ptr(out), ptr(scratch), scale, int(accumulate), stream()), "LoG")
     return out
 
 
@@ -561,14 +550,12 @@ def pointwise_image_device(x: torch.Tensor, kind: str, max_abs=None):
     image; None reduces it here (a caller that makes several of these types passes one image_max_abs to all)."""
     if kind not in POINTWISE_KINDS:
         raise ValueError(f"unknown image type {kind!r} (one of {sorted(POINTWISE_KINDS)})")
-    src = x.contiguous()
-    if src.dtype not in _TORCH_DT:
-        raise ValueError(f"unsupported pixel type {src.dtype}")
+    src = _checked_source(x)
     if max_abs is None:
         max_abs = image_max_abs(src)
     out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
-    check(lib().rb_pointwise_image_dev(_ptr(src), _TORCH_DT[src.dtype], C.c_longlong(src.numel()), POINTWISE_KINDS[kind],
-                                       C.c_double(pointwise_scalar(kind, max_abs)), _ptr(out), _stream()), kind)
+    check(lib().rb_pointwise_image_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], src.numel(), POINTWISE_KINDS[kind],
+                                       pointwise_scalar(kind, max_abs), ptr(out), stream()), kind)
     return out
 
 
@@ -576,11 +563,9 @@ def gradient_magnitude_device(x: torch.Tensor, spacing_zyx=None):
     """gradient magnitude (sitk.GradientMagnitudeImageFilter, getGradientImage) of a CUDA volume (Z,Y,X) or plane (Y,X)
     -> float64 CUDA tensor of that shape (rb_gradient_magnitude_dev).  `spacing_zyx`: one spacing per axis that the
     differences are divided by (gradientUseSpacing=True); None = unit weights.  A zero spacing raises ValueError."""
-    src = x.contiguous()
+    src = _checked_source(x)
     if src.dim() not in (2, 3):
         raise ValueError(f"gradient: 2-D or 3-D image expected, got {src.dim()}-D")
-    if src.dtype not in _TORCH_DT:
-        raise ValueError(f"unsupported pixel type {src.dtype}")
     w = [1.0] * 3
     if spacing_zyx is not None:
         sp = [float(s) for s in spacing_zyx]
@@ -591,8 +576,8 @@ def gradient_magnitude_device(x: torch.Tensor, spacing_zyx=None):
         w[3 - len(sp):] = [1.0 / s for s in sp]
     Z, Y, X = (1,) * (3 - src.dim()) + tuple(src.shape)
     out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
-    check(lib().rb_gradient_magnitude_dev(_ptr(src), _TORCH_DT[src.dtype], Z, Y, X, (C.c_double * 3)(*w), _ptr(out),
-                                          _stream()), "gradient")
+    check(lib().rb_gradient_magnitude_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], Z, Y, X, (C.c_double * 3)(*w), ptr(out),
+                                          stream()), "gradient")
     return out
 
 
@@ -640,19 +625,12 @@ _MOMENTS_SCRATCH_BYTES = 40960                     # RB_MOMENTS_SCRATCH_BYTES
 RESEGMENT_MODES = ("absolute", "relative", "sigma")
 
 
-def _checked_source(x):
-    src = x.contiguous()
-    if src.dtype not in _TORCH_DT:
-        raise ValueError(f"unsupported pixel type {src.dtype}")
-    return src
-
-
 def _roi_moments(src, roi_u8, passes):
     """rb_roi_moments_dev -> [n, n_nan, sum, max, sum of (x - mean)^2] on the host (one 40-byte copy)"""
     scratch = torch.empty(_MOMENTS_SCRATCH_BYTES, dtype=torch.uint8, device=src.device)
     res = torch.empty(5, dtype=torch.float64, device=src.device)
-    check(lib().rb_roi_moments_dev(_ptr(src), _TORCH_DT[src.dtype], _ptr(roi_u8), C.c_longlong(src.numel()), passes,
-                                   _ptr(scratch), _ptr(res), _stream()), "roi moments")
+    check(lib().rb_roi_moments_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], ptr(roi_u8), src.numel(), passes,
+                                   ptr(scratch), ptr(res), stream()), "roi moments")
     return res.cpu().tolist()
 
 
@@ -682,10 +660,9 @@ def normalize_image_device(x: torch.Tensor, scale=1, outliers=None, stats=None):
     else:
         mean, std = (float(v) for v in stats)
     out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
-    check(lib().rb_normalize_dev(_ptr(src), _TORCH_DT[src.dtype], C.c_longlong(src.numel()), C.c_double(mean),
-                                 C.c_double(std), int(outliers is not None),
-                                 C.c_double(float(outliers) if outliers is not None else 0.0), C.c_double(float(scale)),
-                                 _ptr(out), _stream()), "normalize")
+    check(lib().rb_normalize_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], src.numel(), mean, std, int(outliers is not None),
+                                 float(outliers) if outliers is not None else 0.0, float(scale), ptr(out), stream()),
+          "normalize")
     return out
 
 
@@ -732,7 +709,7 @@ def resegment_mask_device(img_t: torch.Tensor, mask_t: torch.Tensor, resegmentRa
         raise ValueError(f"Length {len(resegmentRange)} is not allowed for resegmentRange")
     logger.debug(f"Resegmenting mask (range {resegmentRange}, mode {resegmentMode})")
     src = _checked_source(img_t)
-    np_type = _NP_OF_TORCH[src.dtype]
+    np_type = NP_OF_TORCH[src.dtype]
     roi = (mask_t == label).to(torch.uint8).contiguous()
     if roi.shape != src.shape:
         raise ValueError(f"mask shape {tuple(roi.shape)} differs from image shape {tuple(src.shape)}")
@@ -756,9 +733,8 @@ def resegment_mask_device(img_t: torch.Tensor, mask_t: torch.Tensor, resegmentRa
         logger.debug(f"Applying upper threshold ({thresholds[1]})")
     out = torch.empty(src.shape, dtype=torch.uint8, device=src.device)
     counts = torch.empty(2, dtype=torch.int64, device=src.device)
-    check(lib().rb_resegment_dev(_ptr(src), _TORCH_DT[src.dtype], _ptr(roi), C.c_longlong(src.numel()),
-                                 C.c_double(cmp[0]), C.c_double(cmp[-1]), len(cmp), _ptr(out), _ptr(counts), _stream()),
-          "resegment")
+    check(lib().rb_resegment_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], ptr(roi), src.numel(), cmp[0], cmp[-1], len(cmp),
+                                 ptr(out), ptr(counts), stream()), "resegment")
     oldSize, roiSize = counts.cpu().tolist()
     if roiSize <= 1:
         raise ValueError(f"Resegmentation excluded too many voxels with label {label} "
@@ -875,11 +851,9 @@ def lbp3d_device(img_t: torch.Tensor, roi_t: torch.Tensor, levels=2, radius=1.0,
     samples are rounded and clamped to (default: img_t's; a uint16 image reaches the device as int32)."""
     verts, harm = _lbp3d_tables(levels, radius, subdivision)
     levels = int(levels)
-    src = img_t.contiguous()
-    if src.dtype not in _TORCH_DT:
-        raise ValueError(f"unsupported pixel type {src.dtype}")
-    dtype = np.dtype(dtype) if dtype is not None else np.dtype(_NP_OF_TORCH[src.dtype])
-    if dtype not in _DT:
+    src = _checked_source(img_t)
+    dtype = np.dtype(dtype) if dtype is not None else np.dtype(NP_OF_TORCH[src.dtype])
+    if dtype not in DTYPE_CODE:
         raise ValueError(f"unsupported pixel type {dtype}")
     roi = (roi_t != 0).to(torch.uint8).contiguous()
     if src.dim() != 3 or tuple(roi.shape) != tuple(src.shape):
@@ -887,9 +861,8 @@ def lbp3d_device(img_t: torch.Tensor, roi_t: torch.Tensor, levels=2, radius=1.0,
     Z, Yn, X = src.shape
     scratch = torch.empty((Z, Yn, X), dtype=torch.float64, device=src.device)
     out = torch.empty((levels + 1, Z, Yn, X), dtype=torch.float64, device=src.device)
-    check(lib().rb_lbp3d_dev(_ptr(src), _TORCH_DT[src.dtype], _DT[dtype], _ptr(roi), Z, Yn, X,
-                             verts.ctypes.data_as(C.c_void_p), int(len(verts)), harm.ctypes.data_as(C.c_void_p), levels,
-                             _ptr(scratch), _ptr(out), _stream()), "lbp3d")
+    check(lib().rb_lbp3d_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], DTYPE_CODE[dtype], ptr(roi), Z, Yn, X, ptr(verts),
+                             int(len(verts)), ptr(harm), levels, ptr(scratch), ptr(out), stream()), "lbp3d")
     return out
 
 
@@ -945,11 +918,9 @@ def lbp2d_device(img_t: torch.Tensor, axis=0, samples=8, radius=1, method="unifo
     2 -> (y, z)), or of a CUDA plane (Y,X) -> float64 CUDA tensor of the input's shape (rb_lbp2d_dev).  No cast to the
     image's dtype: getLBP2DImage does that on the host, as the reference does."""
     P, code, rp, cp = _lbp2d_params(samples, radius, method)
-    src = img_t.contiguous()
+    src = _checked_source(img_t)
     if src.dim() not in (2, 3):
         raise ValueError(f"LBP 2D: 2-D or 3-D image expected, got {src.dim()}-D")
-    if src.dtype not in _TORCH_DT:
-        raise ValueError(f"unsupported pixel type {src.dtype}")
     if src.dim() == 2:
         axis = 0
     elif isinstance(axis, (int, np.integer)) and -3 <= axis <= 2:
@@ -958,8 +929,8 @@ def lbp2d_device(img_t: torch.Tensor, axis=0, samples=8, radius=1, method="unifo
         raise ValueError(f"LBP 2D: force2Ddimension {axis!r} (0, 1 or 2)")
     Z, Y, X = (1,) * (3 - src.dim()) + tuple(src.shape)
     out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
-    check(lib().rb_lbp2d_dev(_ptr(src), _TORCH_DT[src.dtype], Z, Y, X, int(axis), P, rp.ctypes.data_as(C.c_void_p),
-                             cp.ctypes.data_as(C.c_void_p), code, _ptr(out), _stream()), "lbp2d")
+    check(lib().rb_lbp2d_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], Z, Y, X, int(axis), P, ptr(rp), ptr(cp), code, ptr(out),
+                             stream()), "lbp2d")
     return out
 
 

@@ -12,15 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import CLASS_ID, CLASSES, check, lib
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+from ._lib import CLASS_ID, CLASSES, check, lib, ptr, stream
 
 
 def pack_levels(image: torch.Tensor, mask: torch.Tensor, Ng: int):
@@ -34,8 +26,8 @@ def pack_levels(image: torch.Tensor, mask: torch.Tensor, Ng: int):
     lev = torch.empty(image.shape, dtype=torch.uint8 if lb == 1 else torch.int16, device=image.device)
     presence = torch.zeros(int(Ng), dtype=torch.int32, device=image.device)
     status = torch.zeros(1, dtype=torch.int32, device=image.device)
-    check(lib().rb_pack_levels_dev(_ptr(image), _ptr(mask), C.c_longlong(image.numel()), int(Ng), _ptr(lev),
-                                   _ptr(presence), _ptr(status), _stream()), "pack_levels")
+    check(lib().rb_pack_levels_dev(ptr(image), ptr(mask), image.numel(), int(Ng), ptr(lev), ptr(presence), ptr(status),
+                                   stream()), "pack_levels")
     if int(status.item()) & 1:
         raise IndexError("gray level outside 1..Ng inside the mask")
     return lev, presence
@@ -48,8 +40,8 @@ def level_bytes(lev: torch.Tensor) -> int:
 def glcm_alive_angles(lev, settings, centers=None):
     Z, Y, X = lev.shape
     alive = torch.zeros(_lib.ALIVE_WORDS, dtype=torch.int32, device=lev.device)
-    check(lib().rb_glcm_alive_angles_dev(_ptr(lev), level_bytes(lev), _ptr(centers), Z, Y, X, C.byref(settings),
-                                         _ptr(alive), _stream()), "glcm_alive_angles")
+    check(lib().rb_glcm_alive_angles_dev(ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, C.byref(settings), ptr(alive),
+                                         stream()), "glcm_alive_angles")
     return alive.cpu().numpy().view(np.uint32).copy()
 
 
@@ -71,10 +63,9 @@ def voxel_features(cls: str, lev: torch.Tensor, settings, *, centers=None, z0=0,
         alive = glcm_alive_angles(lev, settings, centers)
     if status is None:
         status = torch.zeros(1, dtype=torch.int32, device=lev.device)
-    alive_p = alive.ctypes.data_as(C.c_void_p) if alive is not None else None
-    check(lib().rb_voxel_features_dev(cid, _ptr(lev), level_bytes(lev), _ptr(centers), Z, Y, X, int(z0), int(z1),
-                                      C.byref(settings), alive_p, _ptr(out), 0, C.c_longlong(out.stride(0)),
-                                      int(out_z0), _ptr(status), _stream()), cls)
+    check(lib().rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(z0), int(z1),
+                                      C.byref(settings), ptr(alive), ptr(out), 0, out.stride(0), int(out_z0), ptr(status),
+                                      stream()), cls)
     return out
 
 
@@ -139,7 +130,6 @@ def class_maps_to_host(cls: str, lev: torch.Tensor, settings, feature_idx=None, 
         alive = glcm_alive_angles(lev, settings, centers)
     if status is None:
         status = torch.zeros(1, dtype=torch.int32, device=dev)
-    alive_p = alive.ctypes.data_as(C.c_void_p) if alive is not None else None
     cur = torch.cuda.current_stream(dev)
     copy_stream = copy_stream or torch.cuda.Stream(device=dev)
     zc = max(1, min(int(zchunk), nz))
@@ -157,32 +147,28 @@ def class_maps_to_host(cls: str, lev: torch.Tensor, settings, feature_idx=None, 
         if copied[slot] is not None:
             cur.wait_event(copied[slot])                 # the DMA of the chunk that used this slot has finished
         buf = ring[slot]
-        check(L.rb_voxel_features_dev(cid, _ptr(lev), level_bytes(lev), _ptr(centers), Z, Y, X, int(za), int(zb),
-                                      C.byref(settings), alive_p, _ptr(buf), 0, C.c_longlong(buf.stride(0)), int(za),
-                                      _ptr(status), C.c_void_p(cur.cuda_stream)), cls)
+        check(L.rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(za), int(zb),
+                                      C.byref(settings), ptr(alive), ptr(buf), 0, buf.stride(0), int(za), ptr(status),
+                                      cur.cuda_stream), cls)
         width = (zb - za) * plane
         if f32:
             for first, count, pos in _runs(idx):
-                check(L.rb_maps_to_f32_dev(C.c_void_p(buf.data_ptr() + first * buf.stride(0) * 8), C.c_longlong(buf.stride(0)),
-                                           C.c_void_p(ring32[slot].data_ptr() + pos * ring32[slot].stride(0) * 4),
-                                           C.c_longlong(ring32[slot].stride(0)), C.c_longlong(width), C.c_longlong(count),
-                                           C.c_void_p(cur.cuda_stream)), "maps_to_f32")
+                check(L.rb_maps_to_f32_dev(buf.data_ptr() + first * buf.stride(0) * 8, buf.stride(0),
+                                           ring32[slot].data_ptr() + pos * ring32[slot].stride(0) * 4, ring32[slot].stride(0),
+                                           width, count, cur.cuda_stream), "maps_to_f32")
         done = torch.cuda.Event()
         done.record(cur)
         copy_stream.wait_event(done)
         off = (za - int(z0)) * plane
         if f32:
             src = ring32[slot]
-            check(L.rb_memcpy2d_async(C.c_void_p(host.data_ptr() + off * 4), C.c_ulonglong(host.stride(0) * 4), _ptr(src),
-                                      C.c_ulonglong(src.stride(0) * 4), C.c_ulonglong(width * 4), C.c_ulonglong(len(idx)), 2,
-                                      C.c_void_p(copy_stream.cuda_stream)), "memcpy2d")
+            check(L.rb_memcpy2d_async(host.data_ptr() + off * 4, host.stride(0) * 4, ptr(src), src.stride(0) * 4, width * 4,
+                                      len(idx), 2, copy_stream.cuda_stream), "memcpy2d")
         else:
             for first, count, pos in _runs(idx):
-                check(L.rb_memcpy2d_async(C.c_void_p(host.data_ptr() + (pos * host.stride(0) + off) * 8),
-                                          C.c_ulonglong(host.stride(0) * 8),
-                                          C.c_void_p(buf.data_ptr() + first * buf.stride(0) * 8),
-                                          C.c_ulonglong(buf.stride(0) * 8), C.c_ulonglong(width * 8), C.c_ulonglong(count), 2,
-                                          C.c_void_p(copy_stream.cuda_stream)), "memcpy2d")
+                check(L.rb_memcpy2d_async(host.data_ptr() + (pos * host.stride(0) + off) * 8, host.stride(0) * 8,
+                                          buf.data_ptr() + first * buf.stride(0) * 8, buf.stride(0) * 8, width * 8, count, 2,
+                                          copy_stream.cuda_stream), "memcpy2d")
         ev = torch.cuda.Event()
         ev.record(copy_stream)
         copied[slot] = ev

@@ -111,26 +111,26 @@ def test_entry_points_reject_bad_arguments():
     L = _lib.lib()
     x = torch.zeros((4, 5, 6), dtype=torch.int16, device="cuda")
     out = torch.empty((4, 5, 6), dtype=torch.float64, device="cuda")
-    s, n = IO._stream(), C.c_longlong(x.numel())
+    s, n = _lib.stream(), C.c_longlong(x.numel())
     c = C.c_double(1.0)
     w = (C.c_double * 3)(1.0, 1.0, 1.0)
     pw = L.rb_pointwise_image_dev
-    assert pw(IO._ptr(x), 0, n, 0, c, IO._ptr(out), s) == _lib.RB_OK
-    assert pw(None, 0, n, 0, c, IO._ptr(out), s) == _lib.RB_ERR_ARG
-    assert pw(IO._ptr(x), 0, n, 0, c, None, s) == _lib.RB_ERR_ARG
-    assert pw(IO._ptr(x), 7, n, 0, c, IO._ptr(out), s) == _lib.RB_ERR_ARG
-    assert pw(IO._ptr(x), -1, n, 0, c, IO._ptr(out), s) == _lib.RB_ERR_ARG
-    assert pw(IO._ptr(x), 0, n, 4, c, IO._ptr(out), s) == _lib.RB_ERR_ARG
-    assert pw(IO._ptr(x), 0, n, -1, c, IO._ptr(out), s) == _lib.RB_ERR_ARG
-    assert pw(IO._ptr(x), 0, C.c_longlong(0), 0, c, IO._ptr(out), s) == _lib.RB_ERR_ARG
+    assert pw(_lib.ptr(x), 0, n, 0, c, _lib.ptr(out), s) == _lib.RB_OK
+    assert pw(None, 0, n, 0, c, _lib.ptr(out), s) == _lib.RB_ERR_ARG
+    assert pw(_lib.ptr(x), 0, n, 0, c, None, s) == _lib.RB_ERR_ARG
+    assert pw(_lib.ptr(x), 7, n, 0, c, _lib.ptr(out), s) == _lib.RB_ERR_ARG
+    assert pw(_lib.ptr(x), -1, n, 0, c, _lib.ptr(out), s) == _lib.RB_ERR_ARG
+    assert pw(_lib.ptr(x), 0, n, 4, c, _lib.ptr(out), s) == _lib.RB_ERR_ARG
+    assert pw(_lib.ptr(x), 0, n, -1, c, _lib.ptr(out), s) == _lib.RB_ERR_ARG
+    assert pw(_lib.ptr(x), 0, C.c_longlong(0), 0, c, _lib.ptr(out), s) == _lib.RB_ERR_ARG
     gm = L.rb_gradient_magnitude_dev
-    assert gm(IO._ptr(x), 0, 4, 5, 6, w, IO._ptr(out), s) == _lib.RB_OK
-    assert gm(None, 0, 4, 5, 6, w, IO._ptr(out), s) == _lib.RB_ERR_ARG
-    assert gm(IO._ptr(x), 0, 4, 5, 6, None, IO._ptr(out), s) == _lib.RB_ERR_ARG
-    assert gm(IO._ptr(x), 0, 4, 5, 6, w, None, s) == _lib.RB_ERR_ARG
-    assert gm(IO._ptr(x), 7, 4, 5, 6, w, IO._ptr(out), s) == _lib.RB_ERR_ARG
+    assert gm(_lib.ptr(x), 0, 4, 5, 6, w, _lib.ptr(out), s) == _lib.RB_OK
+    assert gm(None, 0, 4, 5, 6, w, _lib.ptr(out), s) == _lib.RB_ERR_ARG
+    assert gm(_lib.ptr(x), 0, 4, 5, 6, None, _lib.ptr(out), s) == _lib.RB_ERR_ARG
+    assert gm(_lib.ptr(x), 0, 4, 5, 6, w, None, s) == _lib.RB_ERR_ARG
+    assert gm(_lib.ptr(x), 7, 4, 5, 6, w, _lib.ptr(out), s) == _lib.RB_ERR_ARG
     for Z, Y, X in ((0, 5, 6), (4, 0, 6), (4, 5, -1)):
-        assert gm(IO._ptr(x), 0, Z, Y, X, w, IO._ptr(out), s) == _lib.RB_ERR_ARG
+        assert gm(_lib.ptr(x), 0, Z, Y, X, w, _lib.ptr(out), s) == _lib.RB_ERR_ARG
     torch.cuda.synchronize()
 
 

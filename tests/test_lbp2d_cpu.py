@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 
 import lbp2d_np
-from pyradiomics_b200 import imageoperations as IO
+from pyradiomics_b200 import _lib, imageoperations as IO
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = sorted(glob.glob(os.path.join(HERE, "golden", "lbp2d_*.npz")))
@@ -222,7 +222,7 @@ def run_emul(lib, img, P, R, method, axis):
     P, code, rp, cp = IO._lbp2d_params(P, R, method)
     Z, Y, X = (1,) * (3 - img.ndim) + img.shape
     out = np.empty(img.shape, np.float64)
-    rc = lib.lbp2d_emul(img.ctypes.data, IO._DT[img.dtype], Z, Y, X, axis % 3 if img.ndim == 3 else 0, P, rp.ctypes.data,
+    rc = lib.lbp2d_emul(img.ctypes.data, _lib.DTYPE_CODE[img.dtype], Z, Y, X, axis % 3 if img.ndim == 3 else 0, P, rp.ctypes.data,
                         cp.ctypes.data, code, out.ctypes.data)
     assert rc == 0
     return out

@@ -88,8 +88,8 @@ def test_library_rejects_32_samples():
     cp = np.ones(P)
     t = torch.zeros((2, 4, 4), dtype=torch.int16, device="cuda")
     out = torch.empty((2, 4, 4), dtype=torch.float64, device="cuda")
-    rc = _lib.lib().rb_lbp2d_dev(IO._ptr(t), 0, 2, 4, 4, 0, P, rp.ctypes.data_as(C.c_void_p), cp.ctypes.data_as(C.c_void_p),
-                                 IO.LBP2D_METHODS["default"], IO._ptr(out), IO._stream())
+    rc = _lib.lib().rb_lbp2d_dev(_lib.ptr(t), 0, 2, 4, 4, 0, P, rp.ctypes.data_as(C.c_void_p), cp.ctypes.data_as(C.c_void_p),
+                                 IO.LBP2D_METHODS["default"], _lib.ptr(out), _lib.stream())
     assert rc == _lib.RB_ERR_UNSUPPORTED
 
 

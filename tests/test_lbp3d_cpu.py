@@ -14,7 +14,7 @@ from scipy import ndimage
 from scipy.special import sph_harm_y
 
 import lbp3d_np
-from pyradiomics_b200 import imageoperations as IO
+from pyradiomics_b200 import _lib, imageoperations as IO
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = sorted(glob.glob(os.path.join(HERE, "golden", "lbp3d_*.npz")))
@@ -130,8 +130,8 @@ def run_emul(lib, img, mask, levels, radius, sub, sample_dtype=None):
     coords = np.ascontiguousarray(np.array(np.nonzero(mask)), dtype=np.int64)
     verts, harm = IO._lbp3d_tables(levels, radius, sub)
     out = np.empty((levels + 1, coords.shape[1]))
-    dt = IO._DT[np.dtype(sample_dtype or img.dtype)]
-    rc = lib.lbp3d_emul(coef.ctypes.data, img.ctypes.data, IO._DT[img.dtype], dt, *img.shape, coords.ctypes.data,
+    dt = _lib.DTYPE_CODE[np.dtype(sample_dtype or img.dtype)]
+    rc = lib.lbp3d_emul(coef.ctypes.data, img.ctypes.data, _lib.DTYPE_CODE[img.dtype], dt, *img.shape, coords.ctypes.data,
                         coords.shape[1], verts.ctypes.data, len(verts), harm.ctypes.data, levels, out.ctypes.data)
     assert rc == 0
     return out

@@ -72,8 +72,8 @@ def test_kernel_range_is_enforced_by_the_library():
     scratch = torch.empty((4, 4, 4), dtype=torch.float64, device="cuda")
     out = torch.empty((3, 4, 4, 4), dtype=torch.float64, device="cuda")
     import ctypes as C
-    rc = _lib.lib().rb_lbp3d_dev(IO._ptr(t), 0, 0, IO._ptr(roi), 4, 4, 4, verts.ctypes.data_as(C.c_void_p), len(verts),
-                                 harm.ctypes.data_as(C.c_void_p), 2, IO._ptr(scratch), IO._ptr(out), IO._stream())
+    rc = _lib.lib().rb_lbp3d_dev(_lib.ptr(t), 0, 0, _lib.ptr(roi), 4, 4, 4, verts.ctypes.data_as(C.c_void_p), len(verts),
+                                 harm.ctypes.data_as(C.c_void_p), 2, _lib.ptr(scratch), _lib.ptr(out), _lib.stream())
     assert rc == _lib.RB_ERR_UNSUPPORTED
 
 

@@ -269,8 +269,8 @@ def test_entry_points_reject_bad_arguments():
     res = torch.empty(5, dtype=torch.float64, device="cuda")
     counts = torch.empty(2, dtype=torch.int64, device="cuda")
     scratch = torch.empty(IO._MOMENTS_SCRATCH_BYTES, dtype=torch.uint8, device="cuda")
-    s, n, z = IO._stream(), C.c_longlong(x.numel()), C.c_longlong(0)
-    p, d = IO._ptr, C.c_double
+    s, n, z = _lib.stream(), C.c_longlong(x.numel()), C.c_longlong(0)
+    p, d = _lib.ptr, C.c_double
     mo = L.rb_roi_moments_dev
     assert mo(p(x), 0, p(m), n, 2, p(scratch), p(res), s) == _lib.RB_OK
     assert mo(p(x), 0, None, n, 1, p(scratch), p(res), s) == _lib.RB_OK
