@@ -28,16 +28,7 @@ def _stale():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build_variant(name: str, defines: list[str]) -> str:
-    """developer tool: the same library compiled with extra -D flags -> pyradiomics_b200/variants/lib<name>.so
-    (load it with B200_RADIOMICS_LIB=<path>); used to A/B kernel variants inside one GPU session."""
-    out = os.path.join(HERE, "variants", f"lib{name}.so")
-    os.makedirs(os.path.dirname(out), exist_ok=True)
-    _compile_and_link(out, [f"-D{d}" for d in defines], os.path.join(HERE, "variants", f"obj_{name}"))
-    return out
-
-
-def _compile_and_link(out: str, extra: list[str], objdir: str, verbose: bool = False) -> None:
+def _compile_and_link(out: str, objdir: str, verbose: bool = False) -> None:
     """one nvcc per .cu in parallel (the translation units are independent: no relocatable device code), then link"""
     from concurrent.futures import ThreadPoolExecutor
 
@@ -46,7 +37,7 @@ def _compile_and_link(out: str, extra: list[str], objdir: str, verbose: bool = F
     jobs = []
     for src in sources():
         obj = os.path.join(objdir, os.path.basename(src)[:-3] + ".o")
-        jobs.append((src, obj, [nvcc, *NVCC_FLAGS, *extra, *(["-Xptxas", "-v"] if verbose else []), "-c", src, "-o", obj]))
+        jobs.append((src, obj, [nvcc, *NVCC_FLAGS, *(["-Xptxas", "-v"] if verbose else []), "-c", src, "-o", obj]))
     with ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 4)) as ex:
         for rc in ex.map(lambda j: subprocess.call(j[2], cwd=CSRC), jobs):
             if rc:
@@ -62,15 +53,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if os.path.exists(LIB):
             return LIB
         raise RuntimeError("nvcc not found and libb200radiomics.so is not built")
-    _compile_and_link(LIB, [], os.path.join(HERE, "build"), verbose)
+    _compile_and_link(LIB, os.path.join(HERE, "build"), verbose)
     return LIB
 
 
 if __name__ == "__main__":
     import sys
 
-    if "--variant" in sys.argv:      # python -m pyradiomics_b200.build --variant NAME DEF1=V DEF2=V ...
-        i = sys.argv.index("--variant")
-        print(build_variant(sys.argv[i + 1], sys.argv[i + 2:]))
-    else:
-        print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -38,15 +38,7 @@ namespace rb {
 constexpr int GF_NA = 13;
 constexpr int GF_LOGT = 40;       // log2 table covers 0..2*18+1
 constexpr int GF_KT = 256;        // |a-b| tables
-#ifndef GF_DENSE_SMALL
-#define GF_DENSE_SMALL 1
-#endif
-#ifndef GF_DENSE_MAX_CLS
-#define GF_DENSE_MAX_CLS 10     // n <= 12 solved densely in registers
-#endif
-#ifndef GF_BREAKDOWN
-#define GF_BREAKDOWN 1e-10
-#endif
+constexpr int GF_DENSE_MAX_CLS = 10;   // n <= 12 solved densely in registers
 
 struct GlcmFastTables {
   // per angle (in processing order: 3 axis, 6 face-diagonal, 4 body-diagonal)
@@ -465,8 +457,7 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
     }
     bool bipartite = false;
     if (comp == all && !selfpair) {
-      // 2-colouring by a breadth-first sweep over class masks (<= 2 nlev closure steps; round 1 swept the pair list
-      // instead -- 18 % of this kernel's instructions -- and had moved the test into the solver thread for that reason)
+      // 2-colouring by a breadth-first sweep over class masks (<= 2 nlev closure steps)
       bool connected;
       glcm_graph_scan(eq, es, EA, dsh, EA | EB, false, &connected, &bipartite, true);
     }

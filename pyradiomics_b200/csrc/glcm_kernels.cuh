@@ -35,30 +35,12 @@ struct GlcmTask {
 // Phase B.  KIND 0: tasks with n <= 8 levels, KIND 1: 9..12 (dense register solves, see glcm_small_solve),
 // KIND 2: larger level graphs (register Lanczos, glcm_lanczos.cuh; dynamic shared memory = LZ_NARR * 18 doubles per
 // thread).  Each is its own kernel because the three want very different register budgets.
-#ifndef GF_DENSE_SYNC
-#define GF_DENSE_SYNC 1
-#endif
-#ifndef GF_SOLVE_MINB_S
-#define GF_SOLVE_MINB_S 4
-#endif
-#ifndef GF_SOLVE_MINB_L
-#define GF_SOLVE_MINB_L 2
-#endif
-#ifndef GF_LZ_TOPUP
-#define GF_LZ_TOPUP 0              // 1: a size group's last batch is topped up with tasks of the next smaller group (needs
-                                   // LZ_EIG_EXACT_STATIC = 0 for reproducible bits)
-#endif
-static_assert(!(GF_LZ_TOPUP && LZ_EIG_EXACT_STATIC), "topped-up batches need the task-sized eigenvalue search (LZ_EIG_EXACT_STATIC=0): "
-                                                      "otherwise a task's bits depend on the template that happens to solve it");
-#ifndef GF_SOLVE_TILE
-#define GF_SOLVE_TILE 4096
-#endif
 constexpr int GF_LZ_SMEM_BYTES = LZ_NARR * 18 * 128 * (int)sizeof(double);
 constexpr int glcm_phaseA_smem_bytes(int nt) { return 27 * nt * (int)(sizeof(uint32_t) + sizeof(uint8_t)); }
 template <int KIND> struct SolveKind;
-template <> struct SolveKind<0> { static constexpr int lo = 0, hi = 6, minb = GF_SOLVE_MINB_S; };
+template <> struct SolveKind<0> { static constexpr int lo = 0, hi = 6, minb = 4; };
 template <> struct SolveKind<1> { static constexpr int lo = 7, hi = GF_DENSE_MAX_CLS, minb = 2; };
-template <> struct SolveKind<2> { static constexpr int lo = GF_DENSE_MAX_CLS + 1, hi = GF_NCLS - 1, minb = GF_SOLVE_MINB_L; };
+template <> struct SolveKind<2> { static constexpr int lo = GF_DENSE_MAX_CLS + 1, hi = GF_NCLS - 1, minb = 2; };
 
 // the 27 window levels of the voxel with linear index vi (zeros if !live)
 __device__ __forceinline__ void glcm_task_window(const uint8_t* __restrict__ lev, const VoxParams& P, long long vi, bool live,
@@ -82,7 +64,7 @@ __device__ __forceinline__ void solve_group(const uint8_t* __restrict__ lev, con
     uint32_t W7[7];
     glcm_pack_window(w, 1, W7);
     bool ok;
-    const double r = glcm_small_solve<N, GF_DENSE_SYNC != 0>(w, 1, W7, T, e.slot, &ok, live);
+    const double r = glcm_small_solve<N, true>(w, 1, W7, T, e.slot, &ok, live);
     if (live) res[k] = ok ? r : NAN;
   }
 }
@@ -117,11 +99,10 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
   if (threadIdx.x == 0) glcm_solve_tables_from(*Tg, T);
   __syncthreads();
   const unsigned n = *qcount;
-  // Tiles of GF_SOLVE_TILE (4096) consecutive tasks are counting-sorted by size class in shared memory, so the
-  // lanes of a warp run solves of the same size (otherwise a third of the lanes stay active).  The sort is STABLE and
-  // atomic-free (per-thread counts, one serial scan per class), so the position of a task -- and with it the batch and,
-  // for topped-up Lanczos batches, the size template that solves it -- is the same in every run: bit-reproducible maps.
-  constexpr int TILE = GF_SOLVE_TILE;
+  // Tiles of 4096 consecutive tasks are counting-sorted by size class in shared memory, so the lanes of a warp run
+  // solves of the same size (otherwise a third of the lanes stay active).  The sort is STABLE and atomic-free (per-thread
+  // counts, one serial scan per class), so a task's position is the same in every run.
+  constexpr int TILE = 4096;
   constexpr int LO = SolveKind<KIND>::lo, KC = SolveKind<KIND>::hi - SolveKind<KIND>::lo + 1;
   __shared__ uint16_t order[TILE];
   __shared__ int bucket[GF_NCLS];                 // end position of each class of this kind in `order`
@@ -168,18 +149,11 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
     __syncthreads();
     if (KIND == 2) {
       RB_DYN_SHARED(double, lz_scratch);                 // [LZ_NARR * 18][128]
-      // size groups from the top; a group's last batch is topped up with tasks of the next smaller group (a larger N
-      // solves them as well: padded nodes), so a tile has ONE partially filled batch instead of three
+      // size groups from the top: a task's size class fixes the template that solves it
       const int e14 = bucket[12], e16 = bucket[14], e18 = bucket[15];
-      int s18 = GF_LZ_TOPUP ? e18 - (e18 - e16 + 127) / 128 * 128 : e16;
-      if (s18 < 0) s18 = 0;
-      const int e16b = s18 < e16 ? s18 : e16;
-      int s16 = !GF_LZ_TOPUP ? e14 : e16b > e14 ? e16b - (e16b - e14 + 127) / 128 * 128 : e16b;
-      if (s16 < 0) s16 = 0;
-      const int e14b = s16 < e14 ? s16 : e14;
-      if (!only || only == 18) lanczos_group<18>(lev, P, T, queue, res, order, base, s18, e18, lz_scratch);
-      if (!only || only == 16) lanczos_group<16>(lev, P, T, queue, res, order, base, s16, e16b, lz_scratch);
-      if (!only || only == 14) lanczos_group<14>(lev, P, T, queue, res, order, base, 0, e14b, lz_scratch);
+      if (!only || only == 18) lanczos_group<18>(lev, P, T, queue, res, order, base, e16, e18, lz_scratch);
+      if (!only || only == 16) lanczos_group<16>(lev, P, T, queue, res, order, base, e14, e16, lz_scratch);
+      if (!only || only == 14) lanczos_group<14>(lev, P, T, queue, res, order, base, 0, e14, lz_scratch);
     } else {
       // dense solves: one template size at a time, block-uniform (idle threads run on an empty window), so the
       // barriers inside glcm_small_solve keep the warps on the same code (free-running warps stall on instruction

@@ -1,10 +1,6 @@
 // MCC eigen-tasks of large level graphs (13..18 nodes; only the three axis angles have enough pairs for
 // that): second largest |eigenvalue| of M = D^-1/2 A D^-1/2, A = co-occurrence counts of ONE angle whose
 // level graph is connected and not bipartite (phase A filters those), D = diag(row sums R).
-//
-// Replaces round 1's glcm_fast_solve_task for these tasks.  That solver kept ~0.7 KB of float Lanczos
-// scratch per thread in local memory with dynamic indexing everywhere: long-scoreboard stalls, divergent
-// lanes and the scratch written back to DRAM.  Here:
 //   * the window is loaded PERMUTED so that the angle axis is the fastest window coordinate: the 18 pairs
 //     are the static position pairs (p, p+1), p % 3 < 2 -- no per-slot tables, all pair code is unrolled;
 //   * level classes are 27-bit position masks (__vcmpeq4 on the packed window), node i = i-th class in
@@ -19,8 +15,9 @@
 //   * every loop has a compile-time trip count (N = 14 / 16 / 18 by size class): a warp's lanes never
 //     diverge; a breakdown (invariant subspace) just continues with zero vectors, which leaves decoupled
 //     zero eigenvalues in the tridiagonal -- harmless for max(|hi|, |lo|).  Padded nodes (n < N) contribute exact zeros
-//     to every sum and the eigenvalue search looks at the leading (n-1) x (n-1) block only, so a task's result is
-//     bit-identical whichever size template solves it.
+//     to every sum, and the eigenvalue search runs over the template's whole (N-1) x (N-1) tridiagonal.  A task's size
+//     class fixes its template, so its bits are reproducible; results from different templates agree to rounding, not
+//     to the bit.
 // __host__ __device__: tests/host_emul checks the arithmetic against LAPACK on the CPU box (test-only).
 #pragma once
 // (included from the middle of glcm_fast.cuh: needs GlcmSolveTables, glcm_eq_positions, tridiag_extreme_pair_static)
@@ -28,99 +25,11 @@
 namespace rb {
 
 constexpr uint32_t LZ_LOW = 0x36DB6DBu;       // window positions p (a*9 + b*3 + c) with c < 2: lower ends of the pairs (p, p+1)
-#ifndef LZ_ACC_N
-#define LZ_ACC_N 3
-#endif
-#ifndef LZ_EIG_EXACT_STATIC
-#define LZ_EIG_EXACT_STATIC 2      // 2: always the fully static eigenvalue search of the template's (N-1) x (N-1) tridiagonal (default,
-                                   // with GF_LZ_TOPUP = 0); 0: search sized by the task (template-independent bits: needed when
-                                   // batches are topped up across size groups).  (A mixed mode -- static only for tasks that fill
-                                   // their template -- measured slower: divergent lanes run both searches.)
-#endif
-#ifndef LZ_SEGSUM
-#define LZ_SEGSUM 0                // 1: neighbour sums by a segmented scan over node-sorted endpoint lists (no smem read-modify-write
-                                   // chain; bit-identical).  Slower: the unrolled 36-entry scan pushes the kernel out of the
-                                   // instruction cache
-#endif
-constexpr int LZ_ACC = LZ_ACC_N;               // interleaved partial sums per reduction
+constexpr int LZ_ACC = 3;                     // interleaved partial sums per reduction
 constexpr int LZ_NARR = 5;                    // per-thread shared arrays: U, S, IR, D, E (N doubles each)
+constexpr double GF_BREAKDOWN = 1e-10;        // Lanczos breakdown: residual norms at or below this continue with zeros
 
 RB_HD constexpr int lz_smem_doubles(int N) { return LZ_NARR * N; }
-
-// Both extreme eigenvalues of the leading m x m block of a symmetric tridiagonal held in registers (d[0..NMAX-1],
-// e[1..NMAX-1]); the loops have the compile-time bound NMAX and rows >= m are predicated off, so that the SAME task gives
-// bit-identical results whichever size template (NMAX >= m) happens to solve it -- the maps do not depend on how the
-// eigen-task queue was filled.  Laguerre from outside the spectrum for both ends in one loop, Sturm bisection for an end
-// that has not settled (as tridiag_extreme_pair_static).
-template <int NMAX>
-RB_HD double tridiag_bisect_dyn(const double* d, const double* e, int m, double lo, double hi, int k) {
-  for (int it = 0; it < 36; it++) {
-    const double xm = 0.5 * (lo + hi);
-    double pm2 = 1.0, pm1 = d[0] - xm;
-    int cnt = pm1 <= 0;
-#pragma unroll
-    for (int i = 1; i < NMAX; i++) {
-      if (i < m) {
-        const double e2 = e[i] * e[i];
-        if (e2 == 0) { pm2 = 1.0; pm1 = d[i] - xm; cnt += pm1 <= 0; }
-        else {
-          const double p = (d[i] - xm) * pm1 - e2 * pm2;
-          const bool neg_prev = pm1 < 0 || (pm1 == 0 && pm2 > 0);
-          const bool neg_cur = p < 0 || (p == 0 && !neg_prev);
-          cnt += neg_cur != neg_prev;
-          pm2 = pm1; pm1 = p;
-        }
-      }
-    }
-    if (cnt > k) hi = xm; else lo = xm;
-  }
-  return 0.5 * (lo + hi);
-}
-template <int NMAX>
-RB_HD void tridiag_extreme_pair_dyn(const double* d, const double* e, int m, double* hi_out, double* lo_out, bool live) {
-  double lo = d[0], hi = d[0];
-#pragma unroll
-  for (int i = 0; i < NMAX; i++) {
-    if (i < m) {
-      const double r = (i > 0 ? fabs(e[i]) : 0.0) + ((i + 1 < NMAX && i + 1 < m) ? fabs(e[i + 1 < NMAX ? i + 1 : i]) : 0.0);
-      lo = fmin(lo, d[i] - r); hi = fmax(hi, d[i] + r);
-    }
-  }
-  if (m <= 1) { *hi_out = live ? d[0] : 0.0; *lo_out = live ? d[0] : 0.0; return; }
-  double x[2] = {hi + 1e-9, lo - 1e-9};
-  bool done[2] = {!live, !live};
-  const double dm = (double)m;
-  for (int it = 0; it < 24; it++) {
-    if (done[0] && done[1]) break;
-#pragma unroll
-    for (int c = 0; c < 2; c++) {
-      double p0 = 1.0, p1 = d[0] - x[c], q0 = 0.0, q1 = -1.0, r0 = 0.0, r1 = 0.0;   // p, p', p''
-#pragma unroll
-      for (int i = 1; i < NMAX; i++) {
-        if (i < m) {
-          const double a = d[i] - x[c], b = e[i] * e[i];
-          const double p2 = a * p1 - b * p0;
-          const double q2 = a * q1 - p1 - b * q0;
-          const double r2 = a * r1 - 2.0 * q1 - b * r0;
-          p0 = p1; p1 = p2; q0 = q1; q1 = q2; r0 = r1; r1 = r2;
-        }
-      }
-      if (done[c]) continue;
-      if (p1 == 0) { done[c] = true; continue; }
-      const double G = q1 / p1, H = G * G - r1 / p1;
-      const double disc = (dm - 1.0) * (dm * H - G * G);
-      const double sq = sqrt(disc > 0 ? disc : 0.0);
-      const double den = fabs(G + sq) > fabs(G - sq) ? G + sq : G - sq;
-      if (den == 0 || den != den) continue;            // stalls: left to the bisection below
-      const double step = dm / den;
-      x[c] -= step;
-      if (fabs(step) < 1e-10) done[c] = true;
-    }
-  }
-  *hi_out = done[0] ? x[0] : tridiag_bisect_dyn<NMAX>(d, e, m, lo - 1e-9, hi + 1e-9, m - 1);
-  *lo_out = done[1] ? x[1] : tridiag_bisect_dyn<NMAX>(d, e, m, lo - 1e-9, hi + 1e-9, 0);
-  if (!live) { *hi_out = 0; *lo_out = 0; }
-}
 
 // wl: the 27 window levels with the angle axis as the FASTEST coordinate (0 = unmasked / outside);
 // sm: per-thread scratch of LZ_NARR*N doubles with element stride st.
@@ -177,49 +86,6 @@ RB_HD double glcm_lanczos_axis(const int* wl, const TT& T, double* sm, int st, i
     ida[t / 6] |= a << (5 * (t % 6));
     idb[t / 6] |= b << (5 * (t % 6));
   }
-#if LZ_SEGSUM
-  // ---- endpoint lists sorted by owner node (counting sort through shared memory, once per task): entry e of node i's
-  // run [off_i, off_i + R_i) holds the node at the other end of one of i's pairs, in pair order.  The Lanczos loop then
-  // gathers U[adj_e] with 36 INDEPENDENT loads and sums each run in registers; the former S[a] += U[b] form was a chain
-  // of 36 shared-memory read-modify-writes per step that the compiler must keep in order (a and b may alias): ~1.4k
-  // cycles of exposed latency per step with two warps per scheduler.  Same terms in the same order: bit-identical sums.
-  uint32_t adjw[6];                                        // 6 entries of 5 bits per word
-  uint64_t firstm = 0, lastm = 0;                          // bit e: entry e opens / closes a run
-  const int cnt = 2 * RB_POPC(VL);
-  {
-    int off = 0;
-#pragma unroll
-    for (int i = 0; i < N; i++) {
-      const int Ri = (int)Rd[i];
-      *reinterpret_cast<int*>(&S[(size_t)i * st]) = off;   // cursor of node i
-      if (Ri) { firstm |= 1ull << off; lastm |= 1ull << (off + Ri - 1); }
-      off += Ri;
-    }
-    int* const ADJ = reinterpret_cast<int*>(D);            // D and E are contiguous: 4N >= 36 ints per thread, int e at
-#define LZ_ADJ(e) ADJ[(size_t)((e) >> 1) * st * 2 + ((e) & 1)]   /* double slot e/2, half e%2 */
-#pragma unroll
-    for (int t = 0; t < 18; t++) {
-      const int p = (t / 2) * 3 + (t % 2);
-      if (VL >> p & 1u) {
-        const int a = (ida[t / 6] >> (5 * (t % 6))) & 31u, b = (idb[t / 6] >> (5 * (t % 6))) & 31u;
-        int* const ca = reinterpret_cast<int*>(&S[(size_t)a * st]);
-        const int sa = *ca; *ca = sa + 1; LZ_ADJ(sa) = b;
-        int* const cb = reinterpret_cast<int*>(&S[(size_t)b * st]);
-        const int sb = *cb; *cb = sb + 1; LZ_ADJ(sb) = a;
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < 6; k++) adjw[k] = 0;
-#pragma unroll
-    for (int e = 0; e < 36; e++) {
-      const int v = e < cnt ? LZ_ADJ(e) : 0;
-      adjw[e / 6] |= (uint32_t)v << (5 * (e % 6));
-    }
-#undef LZ_ADJ
-#pragma unroll
-    for (int i = 0; i < N; i++) S[(size_t)i * st] = 0.0;   // nodes >= n own no run: their sum stays 0
-  }
-#endif
   // ---- start vector (generic fixed components), D-orthogonal to the constant vector, D-normalised
   double y0[N], y1[N];
   double Ssum = 0, dot = 0;
@@ -246,22 +112,6 @@ RB_HD double glcm_lanczos_axis(const int* wl, const TT& T, double* sm, int st, i
   E[0] = 0;
   // ---- N-1 Lanczos steps (the deflated space has n-1 <= N-1 dimensions; see the file header for breakdowns)
   for (int j = 0; j < N - 1; j++) {
-#if LZ_SEGSUM
-#pragma unroll
-    for (int i = 0; i < N; i++) U[(size_t)i * st] = y1[i];
-    {
-      double acc = 0.0;
-      int r = -1;                                          // run index = owner node (every node < n owns one run)
-#pragma unroll
-      for (int e = 0; e < 36; e++) {
-        const double g = U[(size_t)((adjw[e / 6] >> (5 * (e % 6))) & 31u) * st];
-        const bool fst = firstm >> e & 1ull;
-        r += fst;
-        acc = fma(acc, fst ? 0.0 : 1.0, g);                // acc + g inside a run, g at its first entry (exact either way)
-        if (lastm >> e & 1ull) S[(size_t)r * st] = acc;
-      }
-    }
-#else
 #pragma unroll
     for (int i = 0; i < N; i++) { U[(size_t)i * st] = y1[i]; S[(size_t)i * st] = 0.0; }
     // neighbour sums: S[a] += y[b], S[b] += y[a] for every valid pair (a self pair adds 2 y[a])
@@ -275,7 +125,6 @@ RB_HD double glcm_lanczos_axis(const int* wl, const TT& T, double* sm, int st, i
         S[b] += ua;
       }
     }
-#endif
     // z = W y1 - beta y0 (kept in y0's registers); alpha = <y1, W y1>_D = sum y1_i s_i.  Every reduction below runs
     // on LZ_ACC interleaved partial sums: with two warps per scheduler a single 18-long DFMA chain is exposed latency.
     double al[LZ_ACC];
@@ -331,13 +180,8 @@ RB_HD double glcm_lanczos_axis(const int* wl, const TT& T, double* sm, int st, i
 #pragma unroll
   for (int i = 0; i < N - 1; i++) { d[i] = D[(size_t)i * st]; e[i] = E[(size_t)i * st]; }
   double hi, lo;
-#if LZ_EIG_EXACT_STATIC == 2
-  // always the full static search: padded / broken-down rows are decoupled zero eigenvalues, harmless for max(|hi|,|lo|).
-  // Template-dependent bits: only with GF_LZ_TOPUP=0 (a task's size class then fixes its template)
+  // padded / broken-down rows are decoupled zero eigenvalues, harmless for max(|hi|,|lo|)
   tridiag_extreme_pair_static<N - 1, false>(d, e, &hi, &lo, live && n >= 2);
-#else
-  tridiag_extreme_pair_dyn<N - 1>(d, e, n - 1, &hi, &lo, live && n >= 2);      // the deflated space has n - 1 dimensions
-#endif
   return fmax(fabs(hi), fabs(lo));
 }
 

@@ -180,19 +180,11 @@ struct NgtdmGeneralDiff {
 
 // scr_pk / scr_ns: per-thread scratch of 27 entries each, element stride st (device: shared memory laid out
 // [entry][thread]).  FULL: wl must be a full window (all 27 levels non-zero).
-// NGTDM_ABLATE (developer A/B builds, -D): stop the body early and store stand-in values, to time its stages --
-// 1 after the window sums, 2 after the equality masks, diffs and class sums, 3 after the compaction, 4 after the sort
-#ifndef NGTDM_ABLATE
-#define NGTDM_ABLATE 0
-#endif
-#define NGTDM_ABLATE_AT(STAGE, V0, V1) \
-  if (NGTDM_ABLATE == STAGE) { for (int _k = 0; _k < NGTDM_NF; _k++) out[_k] = (double)(V0) + (double)(V1); return; }
 template <bool FULL>
 RB_HD void ngtdm_fast_body(const int* wl, const SmallFastTables& T, double* out, int* scr_pk, double* scr_ns, int st) {
   int B = 0, C = 0;
 #pragma unroll
   for (int v = 0; v < 27; v++) { B += wl[v] * wl[v]; C += wl[v]; }
-  NGTDM_ABLATE_AT(1, B, C)
   uint32_t eq[27];
   RB_EQMASKS_27(wl, eq);
   int Nvp = 27, SE = 0;                          // FULL: sum_v diff_v * L
@@ -235,7 +227,6 @@ RB_HD void ngtdm_fast_body(const int* wl, const SmallFastTables& T, double* out,
     ForPos<0, 27>::go(p1);
     ssum = p1.ssum;
   }
-  NGTDM_ABLATE_AT(2, SE + ssum, scr_pk[st] + scr_ns[st])
   // compact the classes: entry nl <= v is already read.  Non-representatives write a dead entry at nl (overwritten by
   // the next representative, or past the end).
   int nl = 0, SL = 0, SL2 = 0;
@@ -251,12 +242,10 @@ RB_HD void ngtdm_fast_body(const int* wl, const SmallFastTables& T, double* out,
     X[v] = rep ? g * n : 0;
     if (rep) { nl++; SL += g; SL2 += g * g; pw += ns; }
   }
-  NGTDM_ABLATE_AT(3, nl + SL + X[5] + X[20], pw)
   RB_NGTDM_SORT27(X);
   int bd = 0;                                    // sum_{a<b} |i_a n_a - i_b n_b|
 #pragma unroll
   for (int k = 0; k < 27; k++) bd += (2 * k - 53 + nl) * X[k];
-  NGTDM_ABLATE_AT(4, bd + SL2, pw)
   const double cpx = ngtdm_complexity_pairs(scr_pk, scr_ns, st, nl, T);
   // u = the unit of the diffs (FULL: L); p_i = n_i / Nvp
   const double u = FULL ? (double)NGTDM_L : 1.0, N = (double)Nvp;

@@ -230,19 +230,7 @@ def _adversarial_windows():
     return [np.ascontiguousarray(np.clip(w, 0, 32), dtype=np.uint8) for w in out]
 
 
-@pytest.fixture(scope="module")
-def emul_dyn():
-    """the same device math with the task-sized eigenvalue search (LZ_EIG_EXACT_STATIC=0)"""
-    so = os.path.join(HERE, "host_emul", "libemul_dyn.so")
-    src = os.path.join(HERE, "host_emul", "emul.cpp")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-Wno-unknown-pragmas", "-DLZ_EIG_EXACT_STATIC=0", "-o", so + ".%d" % os.getpid(), src])
-    os.replace(so + ".%d" % os.getpid(), so)
-    lib = C.CDLL(so)
-    lib.emul_glcm_lanczos_axis.restype = C.c_double
-    return lib
-
-
-def test_eigen_task_solvers_against_lapack(emul, emul_dyn):
+def test_eigen_task_solvers_against_lapack(emul):
     """the dense register solve (n <= 12 levels) and the register Lanczos solve (13..18 levels, per-thread shared vectors)
     on random / structured / holed / adversarial windows, against numpy's eigvalsh -- both in fp64 throughout: 1e-9"""
     emul.emul_glcm_solve_window_cls.restype = C.c_double
@@ -277,12 +265,9 @@ def test_eigen_task_solvers_against_lapack(emul, emul_dyn):
                 assert nout.value == n
                 if n > 12:
                     assert lz == d                                          # layout-independent, same code as the dispatcher
-                for N2 in (16, 18):                                         # a larger size template: same value (a task's size
-                    if N2 > N:                                              # class fixes its template on the device: no top-up)
+                for N2 in (16, 18):                                         # a larger size template: same value to rounding
+                    if N2 > N:                                              # (a task's size class fixes its template)
                         assert abs(emul.emul_glcm_lanczos_axis(wp.ctypes.data_as(C.c_void_p), N2, 1, 0, C.byref(nout)) - lz) < 1e-12
-                        # ... and the SAME BITS in the task-sized build that topped-up batches would need
-                        assert emul_dyn.emul_glcm_lanczos_axis(wp.ctypes.data_as(C.c_void_p), N2, 1, 0, C.byref(nout)) == \
-                            emul_dyn.emul_glcm_lanczos_axis(wp.ctypes.data_as(C.c_void_p), N, 128, 77, C.byref(nout))
                 worst["lanczos_small"] = max(worst["lanczos_small"], abs(lz - ref)); count["lanczos_small"] += 1
     assert count["dense"] > 3000 and count["lanczos"] > 150 and count["lanczos_small"] > 1000, count
     assert worst["dense"] < 1e-9, worst

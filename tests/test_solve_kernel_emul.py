@@ -17,20 +17,20 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 _LIBS = {}
 
 
-def _build(tag, defs):
-    if tag in _LIBS:                       # never overwrite a library this process has loaded
-        return _LIBS[tag]
-    so = os.path.join(HERE, "host_emul", f"libsolve_emul_{tag}.so")
+def _solve_lib():
+    if "solve" in _LIBS:                   # never overwrite a library this process has loaded
+        return _LIBS["solve"]
+    so = os.path.join(HERE, "host_emul", "libsolve_emul.so")
     src = os.path.join(HERE, "host_emul", "solve_kernel_emul.cpp")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-pthread", "-Wno-unknown-pragmas", *defs, "-shared", "-fPIC", "-o", so + ".%d" % os.getpid(), src])
+    subprocess.check_call(["g++", "-O1", "-std=c++17", "-pthread", "-Wno-unknown-pragmas", "-shared", "-fPIC", "-o", so + ".%d" % os.getpid(), src])
     os.replace(so + ".%d" % os.getpid(), so)
-    _LIBS[tag] = C.CDLL(so)
-    return _LIBS[tag]
+    _LIBS["solve"] = C.CDLL(so)
+    return _LIBS["solve"]
 
 
 @pytest.mark.parametrize("kind,n", [("smooth", 12), ("uniform", 16)])
 def test_emulated_solve_kernels_process_every_task_once(kind, n):
-    lib = _build("local", [])
+    lib = _solve_lib()
     lev = np.ascontiguousarray(bench.synth_volume(40, kind)[:n, :n, :n].astype(np.uint8))
     cap = 100000
     rk, rd, cls = np.zeros(cap), np.zeros(cap), np.zeros(cap, np.int32)
@@ -40,8 +40,7 @@ def test_emulated_solve_kernels_process_every_task_once(kind, n):
     rk, rd, cls = rk[:nt], rd[:nt], cls[:nt]
     assert not (rk == -12345.0).any(), "a queued task was not picked up by any solve kernel"
     assert not np.isnan(rk).any()
-    # bit-identical to the direct solve -- also for the large tasks that were topped up into a batch of the next larger
-    # Lanczos size template (padded nodes add exact zeros; the eigenvalue search is sized by the task, not the template)
+    # bit-identical to the direct solve: both solve a task with the size template its class fixes
     assert np.array_equal(rk, rd)
     hist = np.bincount(cls, minlength=16)
     assert hist[:7].sum() and hist[7:11].sum() and hist[11:].sum()      # all three kernels had work
@@ -53,7 +52,7 @@ def test_emulated_glcm_pipeline_equals_per_voxel_math(kind, n):
     kernel, in plane chunks like glcm_fast_launch, against the single-thread composition of the same math
     (emul_glcm_fast, itself pinned on the reference's voxel-mode maps in test_host_emul.py)"""
     from pyradiomics_b200 import _lib
-    pipe = _build("local", [])
+    pipe = _solve_lib()
     pipe.emul_glcm_pipeline.restype = C.c_longlong
     so = os.path.join(HERE, "host_emul", "libemul_pipe.so")          # own copy: test_host_emul.py rebuilds libemul.so
     if "emul" not in _LIBS:
