@@ -76,6 +76,34 @@ def recursive_gaussian_axis(x, coef, axis):
     return np.moveaxis(out, 0, axis)
 
 
+def log_restatement(x, sigma_mm, spacing_zyx, in_dtype=None, coefficients=None, return_terms=False):
+    """sigma^2-normalised LoG exactly as the CUDA path computes it (imageoperations.log_filter_device): a float64 input
+    stays float64 for the first pass, every other input is rounded to float32.  Every pass is the float64 recursion
+    (causal + anti-causal) times its scale, rounded to float32; per direction d the two smoothing passes run in the
+    kernel's order (d = z: y then x; d = y: z then x; d = x: z then y), the derivative pass is scaled by sigma_d^2, and
+    the three terms are added in float32 in the order z, y, x.  `coefficients(sigma_vox, order)` defaults to the host's
+    recursive_gaussian_coefficients.  Returns the float32 image (and the terms T_z, T_y, T_x when asked)."""
+    if coefficients is None:
+        from pyradiomics_b200.imageoperations import recursive_gaussian_coefficients as coefficients
+    in_dtype = np.dtype(in_dtype if in_dtype is not None else np.asarray(x).dtype)
+    src = np.asarray(x).astype(np.float64 if in_dtype == np.float64 else np.float32).astype(np.float64)
+    s = [sigma_mm / float(v) for v in spacing_zyx]
+
+    def rg(v, axis, order, scale=1.0):
+        return (recursive_gaussian_axis(v, coefficients(s[axis], order), axis) * scale).astype(np.float32)
+
+    def f64(v):
+        return v.astype(np.float64)
+
+    gz = f64(rg(src, 0, 0))
+    terms = [rg(f64(rg(f64(rg(src, 1, 0)), 2, 0)), 0, 2, s[0] * s[0]),
+             rg(f64(rg(gz, 2, 0)), 1, 2, s[1] * s[1]),
+             rg(f64(rg(gz, 1, 0)), 2, 2, s[2] * s[2])]
+    out = terms[0] + terms[1]
+    out = out + terms[2]
+    return (out, terms) if return_terms else out
+
+
 def swt3_levels(x, lo, hi, axes, level=1, start_level=0):
     """restatement of the reference's _swt3 (radiomics/imageoperations.py:899-970) around swtn_level1: the odd axes are
     wrap-padded by one sample ONCE (:914-919), every level is a level-1 transform of the previous (still padded)

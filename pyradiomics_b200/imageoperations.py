@@ -231,6 +231,19 @@ def resample_device(arr_t: torch.Tensor, out_size_zyx, start_zyx, step_zyx, inte
     return dst
 
 
+def _clamp_truncate(v, dtype):
+    """float64 values -> `dtype` like ITK's CastPixelWithBoundsChecking: clamp to the type's range, then truncate
+    (floats are rounded)"""
+    dtype = np.dtype(dtype)
+    if not np.issubdtype(dtype, np.integer):
+        return v.astype(dtype)
+    info = np.iinfo(dtype)
+    hi = float(info.max)
+    if hi > info.max:                       # 2^63 / 2^64 are not representable: the largest double below them
+        hi = np.nextafter(hi, 0.0)
+    return np.trunc(np.clip(v, float(info.min), hi)).astype(dtype)
+
+
 def resampleImage(imageNode, maskNode, **kwargs):
     """reference signature (radiomics/imageoperations.py:448-612): resample image (B-spline by default) and mask (nearest
     neighbour) to `resampledPixelSpacing`, cropped to the ROI's bounding box grown by `padDistance` new-grid voxels; the
@@ -284,10 +297,15 @@ def resampleImage(imageNode, maskNode, **kwargs):
     osz = pad3 + tuple(int(v) for v in newSize[::-1])
     st3 = (0.0,) * (3 - nd) + tuple(start[::-1])
     sp3 = (1.0,) * (3 - nd) + tuple(step[::-1])
-    out_img = resample_device(img_t, osz, st3, sp3, _INTERPOLATORS[interpolator])
+    # a pixel type the device does not carry (uint16 travels as int32; int8, uint32, uint64 as float64) is resampled into
+    # float64 and clamped + truncated to its own range here: a plain astype would wrap a B-spline overshoot below 0 of a
+    # uint16 image to ~65535 where ITK clamps it to 0
+    native = NP_OF_TORCH.get(img_t.dtype) == img.dtype.type
+    out_img = resample_device(img_t, osz, st3, sp3, _INTERPOLATORS[interpolator], out_dtype=None if native else torch.float64)
     out_msk = resample_device(msk_t, osz, st3, sp3, 0)
     origin = np.array(I.origin_xyz(maskNode), dtype=np.float64) + start * maskSpacing      # TransformContinuousIndexToPhysicalPoint (:557)
-    a_img = out_img.cpu().numpy().reshape(osz[3 - nd:]).astype(img.dtype, copy=False)
+    a_img = out_img.cpu().numpy().reshape(osz[3 - nd:])
+    a_img = a_img.astype(img.dtype, copy=False) if native else _clamp_truncate(a_img, img.dtype)
     a_msk = out_msk.cpu().numpy().reshape(osz[3 - nd:]).astype(msk.dtype if msk.dtype != np.bool_ else np.uint8, copy=False)
     return I.ArrayImage(a_img, tuple(newSp), tuple(origin)), I.ArrayImage(a_msk, tuple(newSp), tuple(origin))
 

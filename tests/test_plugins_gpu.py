@@ -10,7 +10,7 @@ import torch
 
 import filters_np as FN
 import pipeline as PL
-from helpers import GOLDEN, assert_maps_close, ref_map, voxel_goldens
+from helpers import GOLDEN, assert_maps_close, log_bound, ref_map, voxel_goldens
 from pyradiomics_b200 import featureclasses as FC, image as I, imageoperations as IO
 
 pytestmark = pytest.mark.gpu
@@ -142,16 +142,9 @@ def test_log_matches_restatement_and_analytic_gaussian_laplace():
     for sigma in (1.0, 2.0, 3.0):
         out = [I.as_array(im) for im, n, _ in IO.getLoGImage(I.ArrayImage(x.astype(np.float32), sp), None, sigma=[sigma])][0]
         assert out.dtype == np.float32
-        # restatement (float64 recursion of the same coefficients)
-        ref = np.zeros(x.shape)
-        xf = x.astype(np.float32).astype(np.float64)
-        for d in range(3):
-            cur = xf
-            for e in range(3):
-                if e != d:
-                    cur = FN.recursive_gaussian_axis(cur, IO.recursive_gaussian_coefficients(sigma, 0), e).astype(np.float32).astype(np.float64)
-            ref += (FN.recursive_gaussian_axis(cur, IO.recursive_gaussian_coefficients(sigma, 2), d) * sigma ** 2).astype(np.float32)
-        assert np.allclose(out, ref, rtol=2e-4, atol=2e-4 * np.abs(ref).max())
+        # restatement of the same passes, roundings and float32 sum (oracle/filters_np.py): per-voxel rounding bound
+        ref, terms = FN.log_restatement(x.astype(np.float32), sigma, sp, return_terms=True)
+        assert (np.abs(out.astype(np.float64) - ref) <= log_bound(terms, x.astype(np.float32))).all()
         # analytic sigma^2-normalised Gaussian Laplacian (truncated FIR), interior only
         ana = ndi.gaussian_laplace(x, sigma, mode="nearest", truncate=6.0) * sigma ** 2
         c = slice(12, -12)
@@ -419,15 +412,8 @@ def test_log_x_axis_tiles_match_restatement_on_ragged_sizes():
     rng = np.random.default_rng(5)
     x = rng.normal(size=(5, 7, 45)).astype(np.float32) * 50
     out = [I.as_array(im) for im, n, _ in IO.getLoGImage(I.ArrayImage(x, (1.0, 1.0, 1.0)), None, sigma=[1.5])][0]
-    ref = np.zeros(x.shape)
-    xf = x.astype(np.float64)
-    for d in range(3):
-        cur = xf
-        for e in range(3):
-            if e != d:
-                cur = FN.recursive_gaussian_axis(cur, IO.recursive_gaussian_coefficients(1.5, 0), e).astype(np.float32).astype(np.float64)
-        ref += (FN.recursive_gaussian_axis(cur, IO.recursive_gaussian_coefficients(1.5, 2), d) * 1.5 ** 2).astype(np.float32)
-    assert np.allclose(out, ref, rtol=2e-4, atol=2e-4 * np.abs(ref).max())
+    ref, terms = FN.log_restatement(x, 1.5, (1.0, 1.0, 1.0), return_terms=True)
+    assert (np.abs(out.astype(np.float64) - ref) <= log_bound(terms, x)).all()
 
 
 @pytest.mark.gpu
