@@ -188,8 +188,10 @@ typedef enum {
   RB_DT_INT16 = 0, RB_DT_INT32 = 1, RB_DT_FLOAT32 = 2, RB_DT_FLOAT64 = 3, RB_DT_UINT8 = 4, RB_DT_UINT16 = 5, RB_DT_INT64 = 6
 } rb_dtype;
 /* rb_minmax_dev: ROI minimum / maximum (mask_dev may be NULL = all voxels) as order-preserving
- *   int64 keys in keys_dev[0..1] plus the voxel count in keys_dev[2]; initialise keys_dev to
- *   {INT64_MAX, INT64_MIN, 0}; decode a key k with  bits = k >= 0 ? k : k ^ INT64_MAX.
+ *   int64 keys in keys_dev[0..1], the voxel count in keys_dev[2] and the count of NaN voxels in
+ *   keys_dev[3] (NaN voxels are counted in [2] but take no part in the minimum / maximum);
+ *   initialise keys_dev to {INT64_MAX, INT64_MIN, 0, 0}; decode a key k with
+ *   bits = k >= 0 ? k : k ^ INT64_MAX.
  *   Replaces the Python-level min()/max() of getBinEdges (radiomics/imageoperations.py:128-129).
  * rb_digitize_dev: out[i] = number of edges <= image[i] inside the mask, 0 outside: np.digitize
  *   on the masked voxels as binImage does (radiomics/imageoperations.py:156-174); comparisons are

@@ -24,23 +24,26 @@ __device__ __forceinline__ long long f64_key(double v) {
 
 __global__ void __launch_bounds__(256)
 minmax_kernel(const void* __restrict__ img, int dt, const uint8_t* __restrict__ mask, long long n,
-              long long* __restrict__ keys /* [0]=min key, [1]=max key, [2]=count */) {
+              long long* __restrict__ keys /* [0]=min key, [1]=max key, [2]=count, [3]=NaN count */) {
   double lo = 1.0 / 0.0, hi = -1.0 / 0.0;
-  long long cnt = 0;
+  long long cnt = 0, nans = 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     if (mask && !mask[i]) continue;
     const double v = load_f64(img, dt, i);
-    lo = v < lo ? v : lo; hi = v > hi ? v : hi; cnt++;
+    lo = v < lo ? v : lo; hi = v > hi ? v : hi; cnt++;      // NaN compares false: counted, not in min / max
+    nans += v != v;
   }
   for (int o = 16; o; o >>= 1) {
     const double l2 = __shfl_xor_sync(0xffffffffu, lo, o), h2 = __shfl_xor_sync(0xffffffffu, hi, o);
     lo = l2 < lo ? l2 : lo; hi = h2 > hi ? h2 : hi;
     cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    nans += __shfl_xor_sync(0xffffffffu, nans, o);
   }
   if ((threadIdx.x & 31) == 0 && cnt) {
     atomicMin(&keys[0], f64_key(lo));
     atomicMax(&keys[1], f64_key(hi));
     atomicAdd((unsigned long long*)&keys[2], (unsigned long long)cnt);
+    if (nans) atomicAdd((unsigned long long*)&keys[3], (unsigned long long)nans);
   }
 }
 

@@ -32,13 +32,15 @@ RB_HD void firstorder_voxel(double* x, int n, const uint16_t* w, int wn, double 
   }
   double sum = 0, en = 0;
   for (int i = 0; i < n; i++) { sum += x[i]; const double s = x[i] + shift; en += s * s; }
-  const double inv = 1.0 / n, mean = sum * inv;
+  // means divide by n as np.mean does: sum * (1 / n) misses a constant window's value by an ulp for some n, and then
+  // Variance / Skewness / Kurtosis of a flat window come out as ~1e-30 / +-1 / 1 instead of 0
+  const double mean = sum / n;
   double mad = 0, m2 = 0, m3 = 0, m4 = 0;
   for (int i = 0; i < n; i++) {
     const double d = x[i] - mean, d2 = d * d;
     mad += fabs(d); m2 += d2; m3 += d2 * d; m4 += d2 * d2;
   }
-  m2 *= inv; m3 *= inv; m4 *= inv;
+  m2 /= n; m3 /= n; m4 /= n;
   const double p10 = fo_percentile(x, n, 10.0), p90 = fo_percentile(x, n, 90.0);
   double ks = 0; int kn = 0;
   for (int i = 0; i < n; i++) if (!(x[i] < p10) && !(x[i] > p90)) { ks += x[i]; kn++; }
@@ -58,8 +60,8 @@ RB_HD void firstorder_voxel(double* x, int n, const uint16_t* w, int wn, double 
   out[F_P10] = p10; out[F_P90] = p90; out[F_Energy] = en; out[F_Entropy] = ent;
   out[F_IQR] = fo_percentile(x, n, 75.0) - fo_percentile(x, n, 25.0);
   out[F_Kurtosis] = m4 / (m2s * m2s);
-  out[F_Maximum] = x[n - 1]; out[F_MAD] = mad * inv; out[F_Mean] = mean; out[F_Median] = fo_percentile(x, n, 50.0);
-  out[F_Minimum] = x[0]; out[F_Range] = x[n - 1] - x[0]; out[F_RMAD] = rmad / kn; out[F_RMS] = sqrt(en * inv);
+  out[F_Maximum] = x[n - 1]; out[F_MAD] = mad / n; out[F_Mean] = mean; out[F_Median] = fo_percentile(x, n, 50.0);
+  out[F_Minimum] = x[0]; out[F_Range] = x[n - 1] - x[0]; out[F_RMAD] = rmad / kn; out[F_RMS] = sqrt(en / n);
   out[F_Skewness] = m3 / (m2s * sqrt(m2s)); out[F_TotalEnergy] = en * voxel_volume; out[F_Uniformity] = uni;
   out[F_Variance] = m2;
 }

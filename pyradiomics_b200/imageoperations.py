@@ -110,23 +110,59 @@ def _decode_key(k: int) -> float:
     return float(np.array([bits], dtype=np.int64).view(np.float64)[0])
 
 
-def roi_minmax(img_t: torch.Tensor, mask_t: torch.Tensor | None):
-    """(min, max, count) of the ROI, one streaming kernel (replaces builtin min()/max())."""
-    keys = torch.tensor([2 ** 63 - 1, -(2 ** 63), 0], dtype=torch.int64, device=img_t.device)
+def roi_extent(img_t: torch.Tensor, mask_t: torch.Tensor | None):
+    """(min, max, count, NaN count) of the ROI, one streaming kernel (replaces builtin min()/max()).  NaN voxels are
+    counted but take no part in min / max; an empty ROI gives (+inf, -inf, 0, 0)."""
+    keys = torch.tensor([2 ** 63 - 1, -(2 ** 63), 0, 0], dtype=torch.int64, device=img_t.device)
     check(lib().rb_minmax_dev(ptr(img_t), TORCH_DTYPE_CODE[img_t.dtype], ptr(mask_t), img_t.numel(), ptr(keys), stream()),
           "minmax")
     k = keys.cpu().tolist()
     if k[2] == 0:
+        return math.inf, -math.inf, 0, 0
+    return _decode_key(k[0]), _decode_key(k[1]), k[2], k[3]
+
+
+def roi_minmax(img_t: torch.Tensor, mask_t: torch.Tensor | None):
+    """(min, max, count) of the ROI, NaN voxels left out of min / max; ValueError for an empty ROI."""
+    mn, mx, n, _ = roi_extent(img_t, mask_t)
+    if n == 0:
         raise ValueError("empty ROI")
-    return _decode_key(k[0]), _decode_key(k[1]), k[2]
+    return mn, mx, n
+
+
+def _binning_range(img_t: torch.Tensor, mask_t: torch.Tensor | None, minmax_reduce=None):
+    """(min, max) the bin edges are built from: (NaN, NaN) when a ROI voxel is NaN, as the reference's min() / max() see
+    it (its getBinEdges then raises).  With `minmax_reduce` every caller reduces, also one whose part of the ROI is empty
+    (it passes +inf, -inf, which leaves the others' range as it is) or holds a NaN (it passes -inf, +inf, so every
+    caller refuses the range); only a ROI that is empty after the reduction raises here."""
+    mn, mx, _, nans = roi_extent(img_t, mask_t)
+    if minmax_reduce is not None:
+        mn, mx = minmax_reduce(-math.inf if nans else mn, math.inf if nans else mx)
+    if nans:
+        return math.nan, math.nan
+    if mn > mx:
+        raise ValueError("empty ROI")
+    return mn, mx
 
 
 def _edges_from_minmax(minimum, maximum, np_type, **kwargs):
-    """reference getBinEdges arithmetic (imageoperations.py:119-149) on the scalars min / max, carried
-    out in the image's own NumPy scalar type so that float32 / integer inputs round exactly as
-    `min(values) - (min(values) % binWidth)`, np.arange and np.histogram do in the reference."""
+    """reference getBinEdges arithmetic (imageoperations.py:119-149) on the scalars min / max.  Floating-point images
+    compute in their own NumPy scalar type, so float32 inputs round exactly as `min(values) - (min(values) % binWidth)`,
+    np.arange and np.histogram do in the reference.  Integer images compute with exact integers: the reference's
+    `maximum + 2 * binWidth` in the image's own type wraps under NumPy 2 (a uint8 maximum >= 206, an int16 maximum
+    >= 32718 at binWidth 25), which NumPy 1 promoted away -- the edges here are NumPy 1's (DESIGN.md section 5).
+    A NaN or infinite minimum / maximum raises ValueError, as np.histogram and np.arange do in the reference."""
     binWidth = kwargs.get("binWidth", 25)
     binCount = kwargs.get("binCount")
+    if not (math.isfinite(minimum) and math.isfinite(maximum)):
+        raise ValueError(f"autodetected range of [{minimum}, {maximum}] is not finite")
+    if np.issubdtype(np_type, np.integer) and binCount is None:
+        minimum, maximum = int(minimum), int(maximum)
+        lowBound = minimum - (minimum % binWidth)
+        e = np.arange(lowBound, maximum + 2 * binWidth, binWidth)
+        if len(e) == 1:
+            e = np.array([e[0] - 0.5, e[0] + 0.5])
+        return e
     minimum, maximum = np_type(minimum), np_type(maximum)
     if binCount is not None:
         # np.histogram(values, binCount)[1]: linspace(min, max, binCount + 1) in the result type of
@@ -149,17 +185,16 @@ def _edges_from_minmax(minimum, maximum, np_type, **kwargs):
 def getBinEdges(parameterValues, **kwargs):
     """reference signature: 1-D array of the segmented voxel values -> bin edges."""
     t = _to_device(parameterValues).reshape(-1)
-    mn, mx, _ = roi_minmax(t, None)
+    mn, mx = _binning_range(t, None)
     return _edges_from_minmax(mn, mx, NP_OF_TORCH[t.dtype], **kwargs)
 
 
 def bin_image_device(img_t: torch.Tensor, mask_t: torch.Tensor | None, minmax_reduce=None, **kwargs):
     """device tensors in -> (int32 levels tensor (0 outside the mask), edges ndarray).  `minmax_reduce(mn, mx)` turns a
     slab's ROI minimum / maximum into the whole ROI's (multi-GPU: all-reduce MIN / MAX), so every rank bins with the
-    same edges."""
-    mn, mx, _ = roi_minmax(img_t, mask_t)
-    if minmax_reduce is not None:
-        mn, mx = minmax_reduce(mn, mx)
+    same edges; a slab without ROI voxels takes part and gets all zeros.  ValueError for an empty ROI and, before
+    anything is binned, for a ROI holding NaN or +-inf (the reference's np.histogram / np.arange refuse those too)."""
+    mn, mx = _binning_range(img_t, mask_t, minmax_reduce)
     edges_native = _edges_from_minmax(mn, mx, NP_OF_TORCH[img_t.dtype], **kwargs)
     edges = np.ascontiguousarray(edges_native, dtype=np.float64)
     e_t = torch.from_numpy(edges).to(img_t.device)

@@ -113,7 +113,7 @@ def main():
         "unit": "voxels/s", "n_gpus": 1, "gpu": gpu_info(0), "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": step_ms, "ms_all_steps": total, "higher_is_better": True, "dtype": "f64",
         "config": {"volume": f"raw_from_levels(synth_volume({n}, 'smooth')), int16", "spacing_zyx": SPACING_ZYX,
-                   "step": "imageoperations.image_max_abs (one rb_minmax_dev + a 24-byte copy to the host), then "
+                   "step": "imageoperations.image_max_abs (one rb_minmax_dev + a 32-byte copy to the host), then "
                            "pointwise_image_device x 4 and gradient_magnitude_device -> five float64 images"},
         "per_type": per_type,
         "bytes_per_step": all_bytes, "achieved_GBps": all_bytes / (step_ms * 1e-3) / 1e9,

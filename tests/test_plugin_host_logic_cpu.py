@@ -350,14 +350,15 @@ def test_plugin_log_generator_checks_and_names(monkeypatch):
     assert list(IO.getLoGImage(img, None)) == []                                                               # no sigma given
 
 
-def test_bin_edges_from_min_max_equal_the_reference_arithmetic_for_every_dtype():
+def test_bin_edges_from_min_max_equal_the_reference_arithmetic_in_int64_for_every_dtype():
     """imageoperations._edges_from_minmax (the host half of binImage: the GPU only reduces min / max and digitizes) against
     the reference's getBinEdges arithmetic on the ROI vector (oracle/pipeline.bin_edges = imageoperations.py:119-149), in the
-    image's own scalar type: float32 images round differently from float64 ones, integers promote in np.arange"""
+    image's own scalar type: float32 images round differently from float64 ones.  Integer images compute as under NumPy 1,
+    i.e. in int64, where `maximum + 2 * binWidth` cannot wrap (DESIGN.md section 5)"""
     from pyradiomics_b200 import imageoperations as IO
     rng = np.random.default_rng(17)
     n = 0
-    for dt in (np.int16, np.int32, np.float32, np.float64):
+    for dt in (np.int16, np.int32, np.float32, np.float64, np.uint8, np.int64):
         for trial in range(120):
             scale = [1, 7, 300, 4000][trial % 4]
             v = rng.normal(rng.uniform(-scale, scale), scale, 50)
@@ -368,15 +369,102 @@ def test_bin_edges_from_min_max_equal_the_reference_arithmetic_for_every_dtype()
                        dict(binCount=8), dict(binCount=64), dict(binCount=1)):
                 if np.issubdtype(dt, np.integer) and kw.get("binWidth") == 0.1 and scale == 4000:
                     continue                                       # (tens of thousands of edges: nothing new)
-                with np.errstate(over="ignore"):                   # int16 + 2 * 5000 wraps in NumPy scalar arithmetic -- in both
-                    ref = PL.bin_edges(v, kw.get("binWidth", 25), kw.get("binCount"))
-                    got = IO._edges_from_minmax(v.min(), v.max(), dt, **kw)
+                ref = PL.bin_edges(v.astype(np.int64) if np.issubdtype(dt, np.integer) else v, kw.get("binWidth", 25),
+                                   kw.get("binCount"))
+                got = IO._edges_from_minmax(v.min(), v.max(), dt, **kw)
                 assert np.asarray(got).shape == np.asarray(ref).shape, (dt, kw, v.min(), v.max())
                 assert np.array_equal(np.asarray(got, np.float64), np.asarray(ref, np.float64)), (dt, kw, v.min(), v.max())
                 # ... and digitizing with them gives the reference's levels
                 assert np.array_equal(np.digitize(v, np.asarray(got, np.float64)), np.digitize(v, ref))
                 n += 1
     assert n > 3500
+
+
+# the pixel type each NumPy input type reaches the device as (imageoperations._to_device)
+DEVICE_TYPE = {np.int8: np.float64, np.uint8: np.uint8, np.int16: np.int16, np.uint16: np.int32, np.int32: np.int32,
+               np.uint32: np.float64, np.int64: np.int64, np.uint64: np.float64, np.float32: np.float32, np.float64: np.float64}
+
+
+@pytest.mark.parametrize("dt", list(DEVICE_TYPE), ids=lambda t: np.dtype(t).name)
+def test_bin_edges_of_integer_images_do_not_wrap_at_the_type_limit(dt):
+    """ROI maxima within 2 binWidth of the type's limit: under NumPy 2 the reference's `maximum + 2 * binWidth` wraps in
+    uint8 / int16 scalars (a uint8 maximum 240 at binWidth 25 gives edges [0, 25] and every voxel above 25 level 2); the
+    edges here are the ones of the same values in int64 -- NumPy 1's promotion -- for every input type (float images:
+    the reference's own arithmetic)"""
+    from pyradiomics_b200 import imageoperations as IO
+    info = np.iinfo(dt) if np.issubdtype(dt, np.integer) else None
+    # (64-bit types: 2^40, where float64 still spaces binWidth 0.1 edges apart -- the digitiser compares in float64)
+    hi = min(int(info.max), 2 ** 40) if info else 3.0e5
+    for bw in (25, 3.5, 0.1, 7):
+        for top in range(0, int(2 * bw) + 2, max(1, int(bw) // 4)):
+            for span in (0, 1, 17, 200):
+                mx = hi - top
+                v = np.array([mx - span, mx - span // 2, mx]).astype(dt)
+                ref = PL.bin_edges(v.astype(np.int64) if info else v, binWidth=bw)
+                got = IO._edges_from_minmax(DEVICE_TYPE[dt](v.min()), DEVICE_TYPE[dt](v.max()), DEVICE_TYPE[dt], binWidth=bw)
+                assert np.array_equal(np.asarray(got, np.float64), np.asarray(ref, np.float64)), (bw, v)
+                if info:
+                    lv = np.digitize(v.astype(np.float64), np.asarray(got, np.float64))
+                    assert lv.min() >= 1 and lv.max() < len(got), (bw, v, got)     # every voxel inside the edges
+    if info and info.min < 0 and info.bits <= 32:                                   # ... and at the lower limit
+        v = np.array([info.min, info.min + 3]).astype(dt)
+        got = IO._edges_from_minmax(DEVICE_TYPE[dt](v.min()), DEVICE_TYPE[dt](v.max()), DEVICE_TYPE[dt], binWidth=25)
+        assert np.array_equal(np.asarray(got, np.float64), np.asarray(PL.bin_edges(v.astype(np.int64), 25), np.float64))
+
+
+def test_reference_numpy2_wraps_where_the_product_does_not():
+    """what the deviation is about: the oracle (the reference's arithmetic under NumPy 2) loses the top of the range"""
+    from pyradiomics_b200 import imageoperations as IO
+    v = np.array([3, 120, 240], np.uint8)
+    with np.errstate(over="ignore"):
+        assert list(PL.bin_edges(v, 25)) == [0, 25]
+        assert np.digitize(v, PL.bin_edges(v, 25)).tolist() == [1, 2, 2]
+        assert len(PL.bin_edges(np.array([0, 32718], np.int16), 25)) == 0
+    assert list(IO._edges_from_minmax(3, 240, np.uint8, binWidth=25)) == list(range(0, 276, 25))
+    assert IO._edges_from_minmax(0, 32718, np.int16, binWidth=25)[-1] == 32750
+
+
+@pytest.mark.parametrize("lo,hi", [(np.nan, np.nan), (1.0, np.inf), (-np.inf, 1.0), (-np.inf, np.inf)])
+@pytest.mark.parametrize("kw", [dict(binWidth=25), dict(binWidth=0.1), dict(binCount=1), dict(binCount=64)])
+@pytest.mark.parametrize("dt", [np.float32, np.float64])
+def test_non_finite_roi_range_raises_value_error_like_the_reference(lo, hi, kw, dt):
+    from pyradiomics_b200 import imageoperations as IO
+    v = np.array([lo, 5.0, hi], dt)
+    with pytest.raises(ValueError), np.errstate(invalid="ignore"):
+        PL.bin_edges(v, kw.get("binWidth", 25), kw.get("binCount"))
+    # NaN voxels do not enter the device's min / max: the caller hands NaN, NaN on when the ROI holds one
+    mn, mx = (np.nan, np.nan) if np.isnan(lo) else (lo, hi)
+    with pytest.raises(ValueError, match="not finite"):
+        IO._edges_from_minmax(dt(mn), dt(mx), dt, **kw)
+
+
+def test_binning_range_reduces_empty_and_nan_slabs_without_raising_first(monkeypatch):
+    """bin_image_device's (min, max) with a reducer (the multi-GPU all-reduce): a slab without ROI voxels or with a NaN
+    still takes part in the reduction -- raising before it would leave the other ranks waiting in the collective"""
+    from pyradiomics_b200 import imageoperations as IO
+    seen = []
+
+    def reducer(others):
+        def f(mn, mx):
+            seen.append((mn, mx))
+            return min(mn, others[0]), max(mx, others[1])
+        return f
+
+    ext = {}
+    monkeypatch.setattr(IO, "roi_extent", lambda img, msk: ext["v"])
+    ext["v"] = (np.inf, -np.inf, 0, 0)                                      # empty slab
+    assert IO._binning_range(None, None, reducer((-5.0, 40.0))) == (-5.0, 40.0)
+    assert seen[-1] == (np.inf, -np.inf)
+    with pytest.raises(ValueError, match="empty ROI"):                      # empty everywhere
+        IO._binning_range(None, None, reducer((np.inf, -np.inf)))
+    with pytest.raises(ValueError, match="empty ROI"):                      # empty, no reducer
+        IO._binning_range(None, None)
+    ext["v"] = (1.0, 3.0, 7, 2)                                             # two NaN among 7 voxels
+    mn, mx = IO._binning_range(None, None, reducer((-5.0, 40.0)))
+    assert np.isnan(mn) and np.isnan(mx) and seen[-1] == (-np.inf, np.inf)  # every rank gets a non-finite range
+    ext["v"] = (1.0, 3.0, 7, 0)
+    assert IO._binning_range(None, None, reducer((-5.0, 40.0))) == (-5.0, 40.0)
+    assert IO._binning_range(None, None) == (1.0, 3.0)
 
 
 # ---- cmatrices: argument errors are raised on the host, before anything touches the device, with the reference's exception
