@@ -143,9 +143,12 @@ def check(rc, what=""):
 
 
 def feature_names(cls):
+    """the map order of a voxel class's kernel: one of CLASSES (or its id) or "firstorder\""""
+    L = lib()
+    if cls == "firstorder":
+        return [L.rb_firstorder_feature_name(i).decode() for i in range(L.rb_firstorder_num_features())]
     cid = CLASS_ID[cls] if isinstance(cls, str) else cls
-    n = lib().rb_num_features(cid)
-    return [lib().rb_feature_name(cid, i).decode() for i in range(n)]
+    return [L.rb_feature_name(cid, i).decode() for i in range(L.rb_num_features(cid))]
 
 
 def make_settings(Ng, n_roi_levels, **kw):

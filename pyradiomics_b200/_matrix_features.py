@@ -4,7 +4,9 @@ work, exactly the layer the reference keeps in Python (radiomics/glcm.py:208-887
 glszm.py:108-434, gldm.py:103-430, ngtdm.py:116-287).  Voxel-based extraction does NOT come through
 here -- there the features are fused into the CUDA kernels (csrc/vox_features.cuh, glcm_fast.cuh).
 
-Each function takes the processed matrix of ONE ROI (no voxel axis) and returns {feature: float}.
+Each *_features function takes the processed matrix of ONE ROI (no voxel axis) and returns {feature: float}; the
+<CLASS>_NAMES tables name the features (GLCM / GLRLM / NGTDM in the order of the voxel kernels' maps,
+_lib.feature_names; GLSZM / GLDM map the shared size-matrix formulas to the class's names).
 """
 from __future__ import annotations
 
@@ -24,31 +26,34 @@ def _entropy(p):
 
 
 # ---------------------------------------------------------------------------------- GLCM
+GLCM_NAMES = ("Autocorrelation", "ClusterProminence", "ClusterShade", "ClusterTendency", "Contrast", "Correlation",
+              "DifferenceAverage", "DifferenceEntropy", "DifferenceVariance", "Id", "Idm", "Idmn", "Idn", "Imc1", "Imc2",
+              "InverseVariance", "JointAverage", "JointEnergy", "JointEntropy", "MCC", "MaximumProbability", "SumAverage",
+              "SumEntropy", "SumSquares")
+
+
 def glcm_process(P, levels, symmetrical=True, weights=None):
-    """raw counts [Ng,Ng,Na] -> normalised [n,n,A] restricted to the present levels, with the
-    reference's symmetrisation / weighting / empty-angle removal (glcm.py:149-205)."""
+    """raw counts [B,Ng,Ng,Na] of a batch of B matrices -> normalised [B,n,n,A] restricted to the present levels, with
+    the reference's symmetrisation / weighting / removal of the angles that are empty for EVERY matrix of the batch
+    (glcm.py:149-205): one common angle axis, so the batch stacks."""
     idx = np.asarray(levels, int) - 1
-    P = P[np.ix_(idx, idx)].astype(float)
+    P = P[:, idx][:, :, idx].astype(float)
     if symmetrical:
-        P = P + P.transpose(1, 0, 2)
+        P = P + P.transpose(0, 2, 1, 3)
     if weights is not None:
-        P = (P * weights[None, None, :]).sum(2, keepdims=True)
-    tot = P.sum((0, 1))
-    if P.shape[2] > 1:
-        keep = tot != 0
-        P, tot = P[:, :, keep], tot[keep]
+        P = (P * weights[None, None, None, :]).sum(3, keepdims=True)
+    tot = P.sum((1, 2))
+    if P.shape[3] > 1:
+        keep = tot.sum(0) != 0
+        P, tot = P[..., keep], tot[:, keep]
     tot = np.where(tot == 0, np.nan, tot)
-    return P / tot[None, None, :]
+    return P / tot[:, None, None, :]
 
 
 def glcm_features(p, levels, Ng):
     lv = np.asarray(levels, float)
     n, A = lv.size, p.shape[2]
-    per_angle = {k: np.full(A, np.nan) for k in (
-        "Autocorrelation", "ClusterProminence", "ClusterShade", "ClusterTendency", "Contrast", "Correlation",
-        "DifferenceAverage", "DifferenceEntropy", "DifferenceVariance", "Id", "Idm", "Idmn", "Idn", "Imc1", "Imc2",
-        "InverseVariance", "JointEnergy", "JointEntropy", "MCC", "MaximumProbability", "SumAverage", "SumEntropy",
-        "SumSquares")}
+    per_angle = {k: np.full(A, np.nan) for k in GLCM_NAMES if k != "JointAverage"}
     ux_all = np.full(A, np.nan)
     li = lv.astype(int)
     kd = np.abs(li[:, None] - li[None, :])
@@ -109,6 +114,12 @@ def glcm_features(p, levels, Ng):
 
 
 # ---------------------------------------------------------------------------------- GLRLM
+GLRLM_NAMES = ("GrayLevelNonUniformity", "GrayLevelNonUniformityNormalized", "GrayLevelVariance", "HighGrayLevelRunEmphasis",
+               "LongRunEmphasis", "LongRunHighGrayLevelEmphasis", "LongRunLowGrayLevelEmphasis", "LowGrayLevelRunEmphasis",
+               "RunEntropy", "RunLengthNonUniformity", "RunLengthNonUniformityNormalized", "RunPercentage", "RunVariance",
+               "ShortRunEmphasis", "ShortRunHighGrayLevelEmphasis", "ShortRunLowGrayLevelEmphasis")
+
+
 def glrlm_process(P, levels, weights=None):
     """raw [Ng,Nr,Na] -> [n,R,A] with absent levels, empty angles and empty run lengths removed
     (glrlm.py:120-127,153-170,184-188).  Returns (P, run_lengths, runs_per_angle)."""
@@ -128,12 +139,7 @@ def glrlm_process(P, levels, weights=None):
 def glrlm_features(P, j, Nr, levels):
     i = np.asarray(levels, float)
     A = P.shape[2]
-    names = ("ShortRunEmphasis", "LongRunEmphasis", "GrayLevelNonUniformity", "GrayLevelNonUniformityNormalized",
-             "RunLengthNonUniformity", "RunLengthNonUniformityNormalized", "RunPercentage", "GrayLevelVariance",
-             "RunVariance", "RunEntropy", "LowGrayLevelRunEmphasis", "HighGrayLevelRunEmphasis",
-             "ShortRunLowGrayLevelEmphasis", "ShortRunHighGrayLevelEmphasis", "LongRunLowGrayLevelEmphasis",
-             "LongRunHighGrayLevelEmphasis")
-    r = {k: np.full(A, np.nan) for k in names}
+    r = {k: np.full(A, np.nan) for k in GLRLM_NAMES}
     i2, j2 = i[:, None] ** 2, j[None, :] ** 2
     for a in range(A):
         if np.isnan(Nr[a]):
@@ -217,6 +223,9 @@ def size_matrix_process(P, levels):
 
 
 # ---------------------------------------------------------------------------------- NGTDM
+NGTDM_NAMES = ("Busyness", "Coarseness", "Complexity", "Contrast", "Strength")
+
+
 def ngtdm_features(P):
     """P [n,3] = (n_i, s_i, i) for the levels with n_i > 0."""
     n, s, i = P[:, 0].astype(float), P[:, 1].astype(float), P[:, 2].astype(float)

@@ -113,19 +113,15 @@ def _fingerprint(a):
 
 
 class DeviceImage:
-    """One (image, ROI mask, binning) discretised ONCE on the GPU: rb_minmax_dev -> rb_digitize_dev ->
-    rb_pack_levels_dev (reference: binImage in every class constructor, base.py:119-125, i.e. 5x per image)."""
+    """One (image, ROI mask, binning) discretised ONCE on the GPU (voxel.discretize; reference: binImage in every class
+    constructor, base.py:119-125, i.e. 5x per image)."""
 
     def __init__(self, imageArray, maskRaw, label, masked, settings):
         img_t = imageoperations._to_device(imageArray)
         # the ROI mask is formed on the device: label compare of the raw mask (or all ones for an unmasked kernel)
         raw_t = imageoperations._to_device(maskRaw)
         msk_t = (raw_t == label).to(torch.uint8) if masked else torch.ones(raw_t.shape, dtype=torch.uint8, device=raw_t.device)
-        lev_t, self.edges = imageoperations.bin_image_device(img_t, msk_t, **settings)
-        Ng = int(lev_t.max().item())
-        self.levels, presence = voxel.pack_levels(lev_t, msk_t, max(Ng, 1))
-        self.grayLevels = (torch.nonzero(presence).flatten() + 1).cpu().numpy().astype(np.int64)
-        self.Ng = int(self.grayLevels.max()) if self.grayLevels.size else 0
+        lev_t, self.edges, self.levels, self.grayLevels, self.Ng = voxel.discretize(img_t, msk_t, **settings)
         self.mask_dev = msk_t
         self._lev32 = lev_t                     # kept until the host copy has been asked for (or never)
         self._binned_host = None
@@ -263,10 +259,6 @@ class RadiomicsFeaturesBase:
     def imageArray(self, value):
         self._imageArray = value
 
-    @property
-    def _levels_dev(self):
-        return self._device.levels
-
     # ---- enabling (reference base.py:127-179)
     def enableFeatureByName(self, featureName, enable=True):
         if featureName not in self.featureNames:
@@ -329,10 +321,19 @@ class RadiomicsFeaturesBase:
         zc = int(self.settings.get("b200_zchunk", 0) or 0)
         return zc if zc > 0 else max(8, min(64, -(-nz // 16)))
 
+    def _voxel_launch(self, lev):
+        """(launch(za, zb, buf) of voxel.maps_to_host, device status word or None) of the class's voxel kernel on the
+        discretised volume `lev`: here the fused texture kernel (voxel.texture_launch)"""
+        settings = self._voxel_settings()
+        centers = self._centers_dev()
+        alive = self._device.glcm_alive(settings, centers) if self.CLASS == "glcm" else None
+        status = torch.zeros(1, dtype=torch.int32, device=lev.device)
+        return voxel.texture_launch(self.CLASS, lev, settings, centers=centers, alive=alive, status=status), status
+
     def _calculateVoxels(self):
-        """The fused kernel of the class in z-chunks; the ENABLED maps stream to page-locked host memory chunk by
-        chunk while the next chunk computes (voxel.class_maps_to_host) -- replaces the voxelBatch loop and the
-        per-voxel assignment of base.py:200-245.  `voxelBatch` is accepted and ignored."""
+        """The class's voxel kernel in z-chunks; the ENABLED maps stream to page-locked host memory chunk by chunk while
+        the next chunk computes (voxel.maps_to_host) -- replaces the voxelBatch loop and the per-voxel assignment of
+        base.py:200-245.  `voxelBatch` is accepted and ignored."""
         lev = self._device.levels3d()
         names = _lib.feature_names(self.CLASS)
         idx = [k for k, n in enumerate(names) if self.enabledFeatures.get(n)]
@@ -341,19 +342,14 @@ class RadiomicsFeaturesBase:
                 self.logger.debug("Feature %s is deprecated / not computed in voxel-based mode", n)
         if not idx:
             return
-        settings = self._voxel_settings()
-        centers = self._centers_dev()
-        alive = self._device.glcm_alive(settings, centers) if self.CLASS == "glcm" else None
-        status = torch.zeros(1, dtype=torch.int32, device=lev.device)
+        launch, status = self._voxel_launch(lev)
         # b200_zrange=(z0, z1): compute and return only these planes (a multi-GPU caller hands every rank the whole image --
         # so that bin edges, gray levels and the GLCM angle set are those of the whole ROI -- and takes one slab per rank)
         z0, z1 = self.settings.get("b200_zrange") or (0, int(lev.shape[0]))
         with self.progressReporter(total=int(z1 - z0), desc="planes") as pbar:
-            host = voxel.class_maps_to_host(self.CLASS, lev, settings, idx, centers=centers, alive=alive, status=status,
-                                            z0=int(z0), z1=int(z1),
-                                            zchunk=self._zchunk(int(z1 - z0)), out_dtype=self._map_dtype(),
-                                            progress=pbar.update)
-        st = int(status.item())
+            host = voxel.maps_to_host(launch, len(names), lev.shape, lev.device, idx, z0=int(z0), z1=int(z1),
+                                      zchunk=self._zchunk(int(z1 - z0)), out_dtype=self._map_dtype(), progress=pbar.update)
+        st = 0 if status is None else int(status.item())
         if st & 2:
             raise _lib.B200Error("weighted GLCM entry list overflow")
         if st & 1:
@@ -388,6 +384,13 @@ class RadiomicsFeaturesBase:
     def _batch_args(self, voxelCoordinates):
         return [self.settings.get("kernelRadius", 1), voxelCoordinates] if voxelCoordinates is not None else []
 
+    def _single_roi(self, P):
+        """the matrix of the one ROI out of the [batch, ...] a matrix builder returns"""
+        if P.shape[0] != 1:
+            raise NotImplementedError(f"{self.MATRIX_ATTR} of a voxel batch: the voxel-based path is fused (no per-voxel "
+                                      f"matrices); use cmatrices.calculate_{self.CLASS} for dense per-voxel matrices")
+        return P[0]
+
     def _value(self, name):
         """single feature (the reference's get<Name>FeatureValue entry points)."""
         if getattr(self, self.MATRIX_ATTR) is None:
@@ -395,21 +398,24 @@ class RadiomicsFeaturesBase:
         return np.float64(self._segment_features()[name])
 
 
-def _add_feature_getters(cls, names, deprecated=()):
+def _add_feature_getters(cls, names, deprecated=(), computable_deprecated=()):
+    """get<Name>FeatureValue for every feature: `names` compute; `deprecated` [(name, why)] raise DeprecationWarning like
+    the reference's; `computable_deprecated` [(name, why)] compute on request, but enableAllFeatures skips them"""
+    def add(n, fn, doc, is_deprecated=False):
+        fn.__name__, fn.__qualname__, fn.__doc__ = f"get{n}FeatureValue", f"{cls.__name__}.get{n}FeatureValue", doc
+        fn._is_deprecated = is_deprecated
+        setattr(cls, fn.__name__, fn)
+
+    kind = cls.CLASS.upper()
     for n in names:
-        def getter(self, _n=n):
-            return self._value(_n)
-        getter.__name__ = f"get{n}FeatureValue"
-        getter.__doc__ = (f"{cls.CLASS.upper()} {n}: same definition as the reference's "
-                          f"Radiomics{cls.CLASS.upper()}.get{n}FeatureValue (see SURVEY.md Appendix C).")
-        setattr(cls, getter.__name__, getter)
+        add(n, lambda self, _n=n: self._value(_n),
+            f"{kind} {n}: same definition as the reference's Radiomics{kind}.get{n}FeatureValue (see SURVEY.md Appendix C).")
+    for n, why in computable_deprecated:
+        add(n, lambda self, _n=n: self._value(_n), f"{kind} {n} (deprecated in the reference: {why}).", True)
     for n, why in deprecated:
         def dep(self, _why=why):
             raise DeprecationWarning(_why)
-        dep.__name__ = f"get{n}FeatureValue"
-        dep.__doc__ = f"DEPRECATED in the reference: {why}"
-        dep._is_deprecated = True
-        setattr(cls, dep.__name__, dep)
+        add(n, dep, f"DEPRECATED in the reference: {why}", True)
 
 
 class RadiomicsGLCM(RadiomicsFeaturesBase):
@@ -428,35 +434,18 @@ class RadiomicsGLCM(RadiomicsFeaturesBase):
         else:
             P, angles = cmatrices.calculate_glcm(self.imageArray, self.maskArray, np.array(self.settings.get("distances", [1])),
                                                  self.coefficients["Ng"], f2, f2d, *self._batch_args(voxelCoordinates))
-        w = _weights(angles, self._spacing_zyx(), self.weightingNorm, "glcm")
-        # symmetrise / weight / drop the angles that are empty for EVERY voxel of the batch (glcm.py:149-205): one
-        # common angle axis, so the batch stacks
-        idx = np.asarray(self.coefficients["grayLevels"], int) - 1
-        P = P[:, idx][:, :, idx].astype(float)
-        if self.symmetricalGLCM:
-            P = P + P.transpose(0, 2, 1, 3)
-        if w is not None:
-            P = (P * w[None, None, None, :]).sum(3, keepdims=True)
-        tot = P.sum((1, 2))
-        if P.shape[3] > 1:
-            keep = tot.sum(0) != 0
-            P, tot = P[..., keep], tot[:, keep]
-        tot = np.where(tot == 0, np.nan, tot)
-        return P / tot[:, None, None, :]
+        return MF.glcm_process(P, self.coefficients["grayLevels"], self.symmetricalGLCM,
+                               _weights(angles, self._spacing_zyx(), self.weightingNorm, "glcm"))
 
     def _segment_features(self):
         return MF.glcm_features(self.P_glcm[0], self.coefficients["grayLevels"], self.coefficients["Ng"])
 
 
-_add_feature_getters(RadiomicsGLCM, _lib_names := [
-    "Autocorrelation", "ClusterProminence", "ClusterShade", "ClusterTendency", "Contrast", "Correlation",
-    "DifferenceAverage", "DifferenceEntropy", "DifferenceVariance", "Id", "Idm", "Idmn", "Idn", "Imc1", "Imc2",
-    "InverseVariance", "JointAverage", "JointEnergy", "JointEntropy", "MCC", "MaximumProbability", "SumAverage",
-    "SumEntropy", "SumSquares"],
-    deprecated=[("Dissimilarity", "mathematically equal to Difference Average"),
-                ("Homogeneity1", "mathematically equal to Inverse Difference"),
-                ("Homogeneity2", "mathematically equal to Inverse Difference Moment"),
-                ("SumVariance", "mathematically equal to Cluster Tendency")])
+_add_feature_getters(RadiomicsGLCM, MF.GLCM_NAMES,
+                     deprecated=[("Dissimilarity", "mathematically equal to Difference Average"),
+                                 ("Homogeneity1", "mathematically equal to Inverse Difference"),
+                                 ("Homogeneity2", "mathematically equal to Inverse Difference Moment"),
+                                 ("SumVariance", "mathematically equal to Cluster Tendency")])
 
 
 class RadiomicsGLRLM(RadiomicsFeaturesBase):
@@ -476,10 +465,7 @@ class RadiomicsGLRLM(RadiomicsFeaturesBase):
             P, angles = cmatrices.calculate_glrlm(self.imageArray, self.maskArray, self.coefficients["Ng"],
                                                   int(np.max(self.imageArray.shape)), f2, f2d, *self._batch_args(voxelCoordinates))
         w = _weights(angles, self._spacing_zyx(), self.weightingNorm, "glrlm")
-        if P.shape[0] != 1:
-            raise NotImplementedError("P_glrlm of a voxel batch: the voxel-based path is fused (no per-voxel matrices); "
-                                      "use cmatrices.calculate_glrlm for dense per-voxel matrices")
-        M, j, Nr = MF.glrlm_process(P[0], self.coefficients["grayLevels"], w)
+        M, j, Nr = MF.glrlm_process(self._single_roi(P), self.coefficients["grayLevels"], w)
         self.coefficients["jvector"], self.coefficients["Nr"] = j, Nr
         return M[None]
 
@@ -487,11 +473,7 @@ class RadiomicsGLRLM(RadiomicsFeaturesBase):
         return MF.glrlm_features(self.P_glrlm[0], self.coefficients["jvector"], self.coefficients["Nr"], self.coefficients["grayLevels"])
 
 
-_add_feature_getters(RadiomicsGLRLM, [
-    "GrayLevelNonUniformity", "GrayLevelNonUniformityNormalized", "GrayLevelVariance", "HighGrayLevelRunEmphasis",
-    "LongRunEmphasis", "LongRunHighGrayLevelEmphasis", "LongRunLowGrayLevelEmphasis", "LowGrayLevelRunEmphasis",
-    "RunEntropy", "RunLengthNonUniformity", "RunLengthNonUniformityNormalized", "RunPercentage", "RunVariance",
-    "ShortRunEmphasis", "ShortRunHighGrayLevelEmphasis", "ShortRunLowGrayLevelEmphasis"])
+_add_feature_getters(RadiomicsGLRLM, MF.GLRLM_NAMES)
 
 
 class _SizeMatrixClass(RadiomicsFeaturesBase):
@@ -513,9 +495,7 @@ class RadiomicsGLSZM(_SizeMatrixClass):
         else:
             P = cmatrices.calculate_glszm(self.imageArray, self.maskArray, self.coefficients["Ng"], int(np.sum(self.maskArray)),
                                           f2, f2d, *self._batch_args(voxelCoordinates))
-        if P.shape[0] != 1:
-            raise NotImplementedError("P_glszm of a voxel batch: use cmatrices.calculate_glszm for dense per-voxel matrices")
-        M, j = MF.size_matrix_process(P[0], self.coefficients["grayLevels"])
+        M, j = MF.size_matrix_process(self._single_roi(P), self.coefficients["grayLevels"])
         self.coefficients["jvector"] = j
         return M[None]
 
@@ -538,9 +518,7 @@ class RadiomicsGLDM(_SizeMatrixClass):
         else:
             P = cmatrices.calculate_gldm(self.imageArray, self.maskArray, np.array(self.settings.get("distances", [1])),
                                          self.coefficients["Ng"], self.gldm_a, f2, f2d, *self._batch_args(voxelCoordinates))
-        if P.shape[0] != 1:
-            raise NotImplementedError("P_gldm of a voxel batch: use cmatrices.calculate_gldm for dense per-voxel matrices")
-        M, j = MF.size_matrix_process(P[0], self.coefficients["grayLevels"])
+        M, j = MF.size_matrix_process(self._single_roi(P), self.coefficients["grayLevels"])
         self.coefficients["jvector"] = j
         return M[None]
 
@@ -568,7 +546,8 @@ class RadiomicsNGTDM(RadiomicsFeaturesBase):
         return MF.ngtdm_features(self.P_ngtdm[0])
 
 
-_add_feature_getters(RadiomicsNGTDM, ["Busyness", "Coarseness", "Complexity", "Contrast", "Strength"])
+_add_feature_getters(RadiomicsNGTDM, MF.NGTDM_NAMES)
+
 
 class RadiomicsFirstOrder(RadiomicsFeaturesBase):
     """First-order statistics (reference radiomics/firstorder.py; SURVEY.md section 8f rank 2).  Voxel-
@@ -586,9 +565,8 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
     def __init__(self, inputImage, inputMask, **kwargs):
         self.voxelArrayShift = kwargs.get("voxelArrayShift", 0)
         self.pixelSpacing = I.spacing_xyz(inputImage)
-        self._raw = I.as_array(inputImage)
         super().__init__(inputImage, inputMask, **kwargs)
-        self._imageArray = self._raw          # like the reference, imageArray stays the raw intensities here
+        self._imageArray = self._rawImageArray      # like the reference, imageArray stays the raw intensities here
 
     @property
     def discretizedImageArray(self):
@@ -596,7 +574,7 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
 
     def _window_radii(self):
         r = int(self.settings.get("kernelRadius", 1))
-        nd = self._raw.ndim
+        nd = self._rawImageArray.ndim
         if self.masked:
             m = self._centerMask
             size = []
@@ -605,46 +583,37 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
                 size.append(int(on[-1] - on[0] + 1))
             size = np.array(size)
         else:
-            size = np.array(self._raw.shape)
+            size = np.array(self._rawImageArray.shape)
         rad = [int(min(r, s - 1)) for s in size]
         if self.settings.get("force2D", False):
             rad[self.settings.get("force2Ddimension", 0)] = 0
         return [0] * (3 - nd) + rad
 
-    def _calculateVoxels(self):
-        img = imageoperations._to_device(self._raw)
+    def _voxel_launch(self, lev):
+        """rb_firstorder_voxel_dev on the raw intensities (uploaded once), a chunk of planes per launch: every window reads
+        the whole volume, so a chunk's maps are those of one whole-volume launch"""
+        img = imageoperations._to_device(self._rawImageArray)
         msk = imageoperations._to_device(self.maskArray)
-        lev = self._levels_dev
         if img.ndim == 2:
-            img, msk, lev = img[None], msk[None], lev[None]
-        centers = None if self.masked else imageoperations._to_device(self._centerMask if self._centerMask.ndim == 3 else self._centerMask[None])
+            img, msk = img[None], msk[None]
+        centers = self._centers_dev()
         Z, Y, X = img.shape
         rz, ry, rx = self._window_radii()
-        nf = _lib.lib().rb_firstorder_num_features()
-        out = torch.empty((nf, Z, Y, X), dtype=torch.float64, device=img.device)
         vv = float(np.multiply.reduce(self.pixelSpacing))
-        idx = [k for k, n in enumerate(self.NAMES) if self.enabledFeatures.get(n)]
         ptr = _lib.ptr
-        _lib.check(_lib.lib().rb_firstorder_voxel_dev(
-            ptr(img), _lib.TORCH_DTYPE_CODE[img.dtype], ptr(msk), ptr(centers), ptr(lev), voxel.level_bytes(lev), Z, Y, X,
-            rz, ry, rx, float(self.voxelArrayShift), vv, float(self.settings.get("initValue", 0)), ptr(out), out.stride(0), 0, Z,
-            0, _lib.stream()), "firstorder")
-        if not idx:
-            return
-        host = torch.empty((len(idx), Z, Y, X), dtype=torch.float64, pin_memory=True)     # enabled maps only
-        for pos, k in enumerate(idx):
-            host[pos].copy_(out[k], non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        arrs = host.numpy()
-        for pos, k in enumerate(idx):
-            arr = arrs[pos] if self._raw.ndim == 3 else arrs[pos][0]
-            self.featureValues[self.NAMES[k]] = I.like(self.inputImage, arr)
+
+        def launch(za, zb, buf):
+            _lib.check(_lib.lib().rb_firstorder_voxel_dev(
+                ptr(img), _lib.TORCH_DTYPE_CODE[img.dtype], ptr(msk), ptr(centers), ptr(lev), voxel.level_bytes(lev), Z, Y, X,
+                rz, ry, rx, float(self.voxelArrayShift), vv, float(self.settings.get("initValue", 0)), ptr(buf), buf.stride(0),
+                za, zb, za, _lib.stream()), "firstorder")
+        return launch, None
 
     def _initCalculation(self, voxelCoordinates=None):
         pass
 
     def _segment_features(self):
-        x = np.sort(self._raw[self.maskArray].astype(np.float64))
+        x = np.sort(self._rawImageArray[self.maskArray].astype(np.float64))
         n = x.size
         sh = x + self.voxelArrayShift
         en = float(np.sum(sh ** 2))
@@ -674,29 +643,44 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
 _add_feature_getters(RadiomicsFirstOrder, RadiomicsFirstOrder.NAMES,
                      deprecated=[("StandardDeviation", "the square root of Variance")])
 
-class RadiomicsShape(RadiomicsFeaturesBase):
+
+class _ShapeClass(RadiomicsFeaturesBase):
+    """what RadiomicsShape and RadiomicsShape2D share: segment-based only (the reference raises while constructing,
+    shape.py:50-52 via base.py:66), no binning (shape ignores intensities), coefficients computed on first use"""
+    MATRIX_ATTR = "_unused_matrix"
+    VOXEL_BASED_ERROR = None
+
+    def __init__(self, inputImage, inputMask, **kwargs):
+        if kwargs.get("voxelBased", False):
+            raise NotImplementedError(self.VOXEL_BASED_ERROR)
+        super().__init__(inputImage, inputMask, **kwargs)
+
+    def _initBinning(self):
+        self._imageArray = self._rawImageArray
+
+    def _calculateVoxels(self):
+        raise NotImplementedError(self.VOXEL_BASED_ERROR)
+
+    def _value(self, name):
+        if not hasattr(self, "eigenValues"):          # the last thing _initCalculation sets
+            self._initCalculation()
+        return np.float64(self._segment_features()[name])
+
+
+class RadiomicsShape(_ShapeClass):
     """3-D shape descriptors of the ROI (reference radiomics/shape.py; SURVEY.md section 8f rank 4): mesh
     surface area / volume / maximum diameters from the CUDA marching-cubes + all-pairs kernels
     (rb_shape_coefficients_dev), axis lengths from exact integer voxel moments (rb_shape_moments_dev).
     Segment-based only, like the reference (shape.py:50-52); independent of gray values (no binning)."""
-    CLASS, MATRIX_ATTR = "shape", "_unused_matrix"
+    CLASS, VOXEL_BASED_ERROR = "shape", "Shape features are not available in voxel-based mode"
     NAMES = ["MeshVolume", "VoxelVolume", "SurfaceArea", "SurfaceVolumeRatio", "Sphericity", "Maximum3DDiameter",
              "Maximum2DDiameterSlice", "Maximum2DDiameterColumn", "Maximum2DDiameterRow", "MajorAxisLength",
              "MinorAxisLength", "LeastAxisLength", "Elongation", "Flatness"]
-    DEPRECATED = ["Compactness1", "Compactness2", "SphericalDisproportion"]
 
     def __init__(self, inputImage, inputMask, **kwargs):
         if np.ndim(I.as_array(inputMask)) != 3:
             raise AssertionError("Shape features are only available in 3D. If 2D, use shape2D instead")
-        if kwargs.get("voxelBased", False):      # the reference raises while constructing (shape.py:50-52 via base.py:66)
-            raise NotImplementedError("Shape features are not available in voxel-based mode")
         super().__init__(inputImage, inputMask, **kwargs)
-
-    def _initBinning(self):                   # shape ignores intensities
-        self._imageArray = self._rawImageArray
-
-    def _calculateVoxels(self):
-        raise NotImplementedError("Shape features are not available in voxel-based mode")
 
     def _initCalculation(self, voxelCoordinates=None):
         from . import cshape
@@ -726,44 +710,20 @@ class RadiomicsShape(RadiomicsFeaturesBase):
             f["Flatness"] = np.nan if (ev[0] < 0 or ev[2] < 0) else np.sqrt(ev[0] / ev[2])
         return f
 
-    def _value(self, name):
-        if not hasattr(self, "SurfaceArea"):
-            self._initCalculation()
-        return np.float64(self._segment_features()[name])
+
+# the deprecated ones are still computable on request, skipped by enableAllFeatures (shape.py:203-273)
+_add_feature_getters(RadiomicsShape, RadiomicsShape.NAMES,
+                     computable_deprecated=[(n, "correlated to Sphericity")
+                                            for n in ("Compactness1", "Compactness2", "SphericalDisproportion")])
 
 
-def _add_shape_getters():
-    _add_feature_getters(RadiomicsShape, RadiomicsShape.NAMES)
-    for n in RadiomicsShape.DEPRECATED:       # still computable on request, skipped by enableAllFeatures (shape.py:203-273)
-        def getter(self, _n=n):
-            return self._value(_n)
-        getter.__name__ = f"get{n}FeatureValue"
-        getter.__doc__ = f"SHAPE {n} (deprecated in the reference: correlated to Sphericity)."
-        getter._is_deprecated = True
-        setattr(RadiomicsShape, getter.__name__, getter)
-
-
-_add_shape_getters()
-
-class RadiomicsShape2D(RadiomicsFeaturesBase):
+class RadiomicsShape2D(_ShapeClass):
     """2-D shape descriptors of a single-slice ROI (reference radiomics/shape2D.py): perimeter, mesh surface and maximum
     diameter from the CUDA marching-squares + all-pairs kernels (rb_calculate_coefficients2D), axis lengths from the pixel
     covariance.  Segment-based only; needs a 2-D mask or a 3-D one with force2D and size 1 in force2Ddimension."""
-    CLASS, MATRIX_ATTR = "shape2D", "_unused_matrix"
+    CLASS, VOXEL_BASED_ERROR = "shape2D", "Shape features are not available in pixel-based mode"
     NAMES = ["MeshSurface", "PixelSurface", "Perimeter", "PerimeterSurfaceRatio", "Sphericity", "MaximumDiameter",
              "MajorAxisLength", "MinorAxisLength", "Elongation"]
-    DEPRECATED = ["SphericalDisproportion"]
-
-    def __init__(self, inputImage, inputMask, **kwargs):
-        if kwargs.get("voxelBased", False):
-            raise NotImplementedError("Shape features are not available in pixel-based mode")
-        super().__init__(inputImage, inputMask, **kwargs)
-
-    def _initBinning(self):                   # shape ignores intensities
-        self._imageArray = self._rawImageArray
-
-    def _calculateVoxels(self):
-        raise NotImplementedError("Shape features are not available in pixel-based mode")
 
     def _initCalculation(self, voxelCoordinates=None):
         from . import cshape
@@ -803,24 +763,10 @@ class RadiomicsShape2D(RadiomicsFeaturesBase):
                  "Elongation": np.nan if (ev[0] < 0 or ev[1] < 0) else np.sqrt(ev[0] / ev[1])}
         return f
 
-    def _value(self, name):
-        if not hasattr(self, "Surface"):
-            self._initCalculation()
-        return np.float64(self._segment_features()[name])
 
+_add_feature_getters(RadiomicsShape2D, RadiomicsShape2D.NAMES,
+                     computable_deprecated=[("SphericalDisproportion", "the inverse of Sphericity")])
 
-def _add_shape2d_getters():
-    _add_feature_getters(RadiomicsShape2D, RadiomicsShape2D.NAMES)
-    for n in RadiomicsShape2D.DEPRECATED:
-        def getter(self, _n=n):
-            return self._value(_n)
-        getter.__name__ = f"get{n}FeatureValue"
-        getter.__doc__ = f"SHAPE2D {n} (deprecated in the reference: the inverse of Sphericity)."
-        getter._is_deprecated = True
-        setattr(RadiomicsShape2D, getter.__name__, getter)
-
-
-_add_shape2d_getters()
 
 FEATURE_CLASSES = {"glcm": RadiomicsGLCM, "glrlm": RadiomicsGLRLM, "glszm": RadiomicsGLSZM, "gldm": RadiomicsGLDM,
                    "ngtdm": RadiomicsNGTDM}

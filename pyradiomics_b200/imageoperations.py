@@ -31,8 +31,6 @@ from ._lib import DTYPE_CODE, NP_OF_TORCH, TORCH_DTYPE_CODE, TORCH_OF_NP, check,
 
 logger = logging.getLogger("radiomics.imageoperations")
 
-# the names this module gave the pointer, stream and pixel-type helpers before _lib held them; existing callers use them
-_ptr, _stream, _DT = ptr, stream, DTYPE_CODE
 
 def _dev():
     return torch.device("cuda", torch.cuda.current_device())

@@ -83,10 +83,8 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
     info = []
     for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=msk, image_types=image_types,
                                     gradient_use_spacing=gradient_use_spacing):
-        lev32, _ = IO.bin_image_device(img.contiguous(), msk, **kw)
-        Ng = int(lev32.max().item())
-        lev, presence = voxel.pack_levels(lev32, msk, Ng)
-        nlev = int((presence > 0).sum().item())
+        _, _, lev, levels, Ng = voxel.discretize(img.contiguous(), msk, **kw)
+        nlev = len(levels)
         s = _lib.make_settings(Ng, nlev, spacing_zyx=spacing_zyx, **kw)
         for c in classes:
             nf = _lib.lib().rb_num_features(_lib.CLASS_ID[c])
@@ -172,27 +170,11 @@ def voxel_suite_with_filters_slab(own: torch.Tensor, own_mask: torch.Tensor, Z: 
     msk = (own_mask != 0).to(torch.uint8).contiguous()
     dev = own.device
     r = int(kw.get("kernelRadius", 1))
-
-    def reduce_minmax(mn, mx):
-        if world == 1:
-            return mn, mx
-        t = torch.tensor([-mn, mx], dtype=torch.float64, device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        return -float(t[0].item()), float(t[1].item())
-
     info, outs = [], {}
     nz = own.shape[0]
     for name, img in derived_images_slab(own, Z, rank, world, spacing_zyx, wavelet, sigmas):
-        lev32, _ = IO.bin_image_device(img.contiguous(), msk, minmax_reduce=reduce_minmax, **kw)
-        ngt = lev32.max().to(torch.int64).reshape(1)
-        if world > 1:
-            dist.all_reduce(ngt, op=dist.ReduceOp.MAX)
-        Ng = int(ngt.item())
-        lev, presence = voxel.pack_levels(lev32, msk, Ng)
-        pres = presence.to(torch.int64)
-        if world > 1:
-            dist.all_reduce(pres, op=dist.ReduceOp.SUM)
-        nlev = int((pres > 0).sum().item())
+        _, _, lev, levels, Ng = voxel.discretize(img.contiguous(), msk, all_reduce=dist.all_reduce if world > 1 else None, **kw)
+        nlev = len(levels)
         s = _lib.make_settings(Ng, nlev, spacing_zyx=spacing_zyx, **kw)
         slab = D.SlabHalo(lev, r, rank, world)
         slab.exchange()

@@ -11,7 +11,7 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, imageoperations
 from ._lib import CLASS_ID, CLASSES, check, lib, ptr, stream
 
 
@@ -31,6 +31,35 @@ def pack_levels(image: torch.Tensor, mask: torch.Tensor, Ng: int):
     if int(status.item()) & 1:
         raise IndexError("gray level outside 1..Ng inside the mask")
     return lev, presence
+
+
+def discretize(image: torch.Tensor, mask: torch.Tensor, /, all_reduce=None, **binning):
+    """One image's gray-level discretisation on the device (the reference's binImage + the levels present in the ROI):
+    bin (imageoperations.bin_image_device, binWidth / binCount in `binning`) -> Ng, the largest level -> pack_levels ->
+    the gray levels that occur in the ROI.  `all_reduce` (torch.distributed.all_reduce's signature) makes a z-slab of a
+    volume sharded over ranks use the whole ROI's min / max, Ng and levels.
+    Returns (int32 levels, bin edges, packed levels, gray levels present as an int64 ndarray, Ng)."""
+    minmax_reduce = None
+    if all_reduce is not None:
+        from torch.distributed import ReduceOp
+
+        def minmax_reduce(mn, mx):                      # MIN of the minima as MAX of their negatives: one collective
+            t = torch.tensor([-mn, mx], dtype=torch.float64, device=image.device)
+            all_reduce(t, op=ReduceOp.MAX)
+            neg_mn, mx = t.tolist()
+            return -neg_mn, mx
+    lev32, edges = imageoperations.bin_image_device(image, mask, minmax_reduce=minmax_reduce, **binning)
+    Ng = lev32.max()
+    if all_reduce is not None:
+        Ng = Ng.to(torch.int64).reshape(1)
+        all_reduce(Ng, op=ReduceOp.MAX)
+    Ng = int(Ng.item())
+    lev, presence = pack_levels(lev32, mask, max(Ng, 1))
+    if all_reduce is not None:
+        presence = presence.to(torch.int64)
+        all_reduce(presence, op=ReduceOp.SUM)
+    gray_levels = (torch.nonzero(presence).flatten() + 1).cpu().numpy().astype(np.int64)
+    return lev32, edges, lev, gray_levels, Ng
 
 
 def level_bytes(lev: torch.Tensor) -> int:
@@ -103,33 +132,53 @@ def _runs(idx):
     return out
 
 
+def texture_launch(cls: str, lev: torch.Tensor, settings, *, centers=None, alive=None, status=None):
+    """the `launch(za, zb, buf)` of maps_to_host for the fused kernel of one texture class: planes [za,zb) of `lev` into
+    `buf` [F, >= zb-za, Y, X] (plane za at buf[:, 0]) on the current stream"""
+    cid = CLASS_ID[cls]
+    Z, Y, X = lev.shape
+    if cls == "glcm" and alive is None:
+        alive = glcm_alive_angles(lev, settings, centers)
+    if status is None:
+        status = torch.zeros(1, dtype=torch.int32, device=lev.device)
+
+    def launch(za, zb, buf):
+        check(lib().rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(za), int(zb),
+                                          C.byref(settings), ptr(alive), ptr(buf), 0, buf.stride(0), int(za), ptr(status),
+                                          torch.cuda.current_stream(lev.device).cuda_stream), cls)
+    return launch
+
+
 def class_maps_to_host(cls: str, lev: torch.Tensor, settings, feature_idx=None, *, centers=None, alive=None, z0=0, z1=None,
                        zchunk=64, out_dtype=torch.float64, host=None, copy_stream=None, status=None, progress=None, sync=True):
-    """Output assembly of one class (the reference's per-batch `featureMaps[tuple(voxelCoords)] = ...`,
-    radiomics/base.py:205-209,232-234, without the batch loop): the fused kernel runs over planes [z0,z1) in z-chunks
-    into a two-slot device ring; every finished chunk leaves for the host on `copy_stream` -- ONE strided DMA per run
-    of consecutive selected features (rb_memcpy2d_async) -- while the next chunk computes.  Only the maps in
+    """Output assembly of one texture class (the reference's per-batch `featureMaps[tuple(voxelCoords)] = ...`,
+    radiomics/base.py:205-209,232-234, without the batch loop): maps_to_host over the class's fused kernel
+    (texture_launch)."""
+    launch = texture_launch(cls, lev, settings, centers=centers, alive=alive, status=status)
+    return maps_to_host(launch, lib().rb_num_features(CLASS_ID[cls]), lev.shape, lev.device, feature_idx, z0=z0, z1=z1,
+                        zchunk=zchunk, out_dtype=out_dtype, host=host, copy_stream=copy_stream, progress=progress, sync=sync)
+
+
+def maps_to_host(launch, nf, shape, dev, feature_idx=None, *, z0=0, z1=None, zchunk=64, out_dtype=torch.float64,
+                 host=None, copy_stream=None, progress=None, sync=True):
+    """The voxel-map driver of every voxel class: `launch(za, zb, buf)` enqueues the `nf` maps of planes [za,zb) of a
+    (Z,Y,X) = `shape` volume into `buf` [nf, >= zb-za, Y, X] on the current stream of device `dev`.  Planes [z0,z1) run
+    in z-chunks into a two-slot device ring; every finished chunk leaves for the host on `copy_stream` -- ONE strided DMA
+    per run of consecutive selected features (rb_memcpy2d_async) -- while the next chunk computes.  Only the maps in
     `feature_idx` (default: all) are copied.  `out_dtype` float32 converts on the device first (half the PCIe bytes).
     Returns the page-locked host tensor [len(feature_idx), z1-z0, Y, X] (allocated from torch's caching pinned
     allocator when `host` is None: the caller owns it, dropping it recycles the block).  sync=False returns without
     waiting for the last copies (the caller synchronises `copy_stream` before touching `host`), so a following class
     starts computing while this one's tail is still on the wire."""
-    cid = CLASS_ID[cls]
-    Z, Y, X = lev.shape
+    Z, Y, X = shape
     z1 = Z if z1 is None else int(z1)
     nz = z1 - int(z0)
-    nf = lib().rb_num_features(cid)
     idx = list(range(nf)) if feature_idx is None else [int(k) for k in feature_idx]
-    dev = lev.device
     if host is None:
         host = torch.empty((len(idx), nz, Y, X), dtype=out_dtype, pin_memory=True)
     assert host.shape == (len(idx), nz, Y, X) and host.dtype == out_dtype and host.is_contiguous()
     if not idx or nz <= 0:
         return host
-    if cls == "glcm" and alive is None:
-        alive = glcm_alive_angles(lev, settings, centers)
-    if status is None:
-        status = torch.zeros(1, dtype=torch.int32, device=dev)
     cur = torch.cuda.current_stream(dev)
     copy_stream = copy_stream or torch.cuda.Stream(device=dev)
     zc = max(1, min(int(zchunk), nz))
@@ -147,9 +196,7 @@ def class_maps_to_host(cls: str, lev: torch.Tensor, settings, feature_idx=None, 
         if copied[slot] is not None:
             cur.wait_event(copied[slot])                 # the DMA of the chunk that used this slot has finished
         buf = ring[slot]
-        check(L.rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(za), int(zb),
-                                      C.byref(settings), ptr(alive), ptr(buf), 0, buf.stride(0), int(za), ptr(status),
-                                      cur.cuda_stream), cls)
+        launch(za, zb, buf)
         width = (zb - za) * plane
         if f32:
             for first, count, pos in _runs(idx):

@@ -38,9 +38,15 @@ def test_settings_struct_layout_matches_header():
 
 
 def test_feature_names(L):
+    from pyradiomics_b200 import _matrix_features as MF, featureclasses as FC
     assert [L.rb_num_features(i) for i in range(5)] == [24, 16, 16, 14, 5]
     assert _lib.feature_names("glcm")[19] == "MCC"
     assert _lib.feature_names("ngtdm") == ["Busyness", "Coarseness", "Complexity", "Contrast", "Strength"]
+    # every Python name table lists the features in the order of the library's maps
+    tables = {"glcm": MF.GLCM_NAMES, "glrlm": MF.GLRLM_NAMES, "glszm": sorted(MF.GLSZM_NAMES.values()),
+              "gldm": sorted(MF.GLDM_NAMES.values()), "ngtdm": MF.NGTDM_NAMES, "firstorder": FC.RadiomicsFirstOrder.NAMES}
+    for cls, names in tables.items():
+        assert list(names) == _lib.feature_names(cls), cls
 
 
 @pytest.mark.parametrize("size", [(5, 5, 5), (1, 6, 7), (2, 2, 9), (3, 1, 4), (6, 7), (1, 5)])

@@ -272,10 +272,10 @@ def test_plugin_shares_one_discretisation_between_the_classes():
     assert np.array_equal(objs[0].coefficients["grayLevels"], levels)
 
 
-@pytest.mark.parametrize("cname", ["glcm", "ngtdm"])
+@pytest.mark.parametrize("cname", ["glcm", "ngtdm", "firstorder"])
 def test_plugin_zrange_and_float32_maps(cname):
     raw, msk = _raw_case(seed=5)
-    cls = FC.FEATURE_CLASSES[cname]
+    cls = {**FC.FEATURE_CLASSES, **FC.NEXT_CLASSES}[cname]
     full = cls(raw, msk, voxelBased=True, binWidth=25, b200_zchunk=7).execute()
     slab = cls(raw, msk, voxelBased=True, binWidth=25, b200_zrange=(6, 15), b200_zchunk=4).execute()
     f32 = cls(raw, msk, voxelBased=True, binWidth=25, b200_map_dtype="float32", b200_zchunk=5).execute()
