@@ -99,10 +99,10 @@ def glcm_features(p, gray_levels, Ng, n_roi_levels=None):
         V, A = p.shape[0], p.shape[3]
         pd = np.zeros((V, Ng, A))
         ps = np.zeros((V, 2 * Ng + 1, A))
-        for a in range(n):
-            for b in range(n):
-                pd[:, kd[a, b], :] += p[:, a, b, :]
-                ps[:, ks[a, b], :] += p[:, a, b, :]
+        # unbuffered adds in (a, b) order: every bin sums its entries in the order of a double loop over (a, b)
+        pf = p.reshape(V, n * n, A)
+        np.add.at(pd, (slice(None), kd.reshape(-1)), pf)
+        np.add.at(ps, (slice(None), ks.reshape(-1)), pf)
         kD = np.arange(Ng, dtype=float)[None, :, None]
         kS = np.arange(2 * Ng + 1, dtype=float)[None, :, None]
         da = (kD * pd).sum(1)

@@ -423,7 +423,19 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
   }
   if (nr > NJCAP) { f[G_MCC] = NAN; if (status) *status |= 1; return true; }
   double A[NJCAP * NJCAP];
+  double dd[NJCAP], ee[NJCAP];
   for (int k = 0; k < nr * nr; k++) A[k] = 0;
+  if (P.symmetric) {
+    // symmetric P (px = py): M = P / sqrt(px_i px_j + eps) is itself symmetric, its singular values are the |eigenvalues|
+    // of M, so MCC is M's second largest |eigenvalue|, solved for directly.  (sqrt of the second eigenvalue of M M^T
+    // squares it first: an absolute rounding of eps in a small eigenvalue of M M^T becomes ~sqrt(eps) in MCC.)
+    for (int e = 0; e < E.n; e++) {
+      const int li = E.key[e] >> 16, lj = E.key[e] & 0xFFFF;
+      A[ridx[li] * nr + ridx[lj]] = ((double)E.w[e] / S) / sqrt(px[li] * px[lj] + EPS);
+    }
+    f[G_MCC] = sym_second_largest_abs(A, nr, nr, dd, ee);
+    return true;
+  }
   for (int e1 = 0; e1 < E.n; e1++) {
     int l1 = E.key[e1] >> 16, c1 = E.key[e1] & 0xFFFF;
     double m1 = ((double)E.w[e1] / S) / sqrt(px[l1] * py[c1] + EPS);
@@ -434,7 +446,6 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
       A[ridx[l1] * nr + ridx[l2]] += m1 * m2;
     }
   }
-  double dd[NJCAP], ee[NJCAP];
   const double l2 = sym_psd_second_largest(A, nr, nr, dd, ee);
   f[G_MCC] = sqrt(l2 > 0 ? l2 : 0.0);
   return true;

@@ -71,8 +71,10 @@ def test_phaseA_full_and_general_bodies_equal_generic_kernel(name, monkeypatch):
     gen = _glcm(lev, centers).cpu().numpy()
     monkeypatch.delenv("B200_RADIOMICS_FORCE_GENERIC")
     for k, f in enumerate(_lib.feature_names("glcm")):
-        atol = 1e-6 if f in ("MCC", "Imc2", "Imc1") else 1e-9
-        ok = np.isclose(fast[k], gen[k], rtol=1e-7, atol=atol, equal_nan=True)
+        # MCC: both solves are within 1e-9 of LAPACK (tests/test_fast_voxel_windows_gpu.py), an absolute bound;
+        # Imc2: 1e-6 stays for the square root of rounding noise the generic kernel can return (see below)
+        rtol, atol = {"MCC": (0, 1e-9), "Imc1": (2e-9, 1e-12), "Imc2": (2e-9, 1e-6)}.get(f, (1e-7, 1e-9))
+        ok = np.isclose(fast[k], gen[k], rtol=rtol, atol=atol, equal_nan=True)
         if f == "Imc2":
             # An angle with exactly independent margins has HXY2 == HXY.  The fast path counts its Imc2 as 0 when the two
             # agree to 1e-12; the generic kernel follows the reference's exact comparison of the rounded entropies and

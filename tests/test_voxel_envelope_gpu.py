@@ -160,7 +160,8 @@ def test_fast_kernels_with_centers_equal_generic_kernel(binned_volume_with_roi, 
     assert (fast[:, ~roi] == -1).all() and (gen[:, ~roi] == -1).all()
     for k, f in enumerate(_lib.feature_names(cname)):
         if cname == "glcm":       # tolerances of the GLCM fast-vs-generic test on 40^3 (tests/test_voxel_gpu.py)
-            ok = np.allclose(fast[k], gen[k], rtol=1e-7, atol=1e-6 if f in ("MCC", "Imc2", "Imc1") else 1e-9, equal_nan=True)
+            rtol, atol = {"MCC": (0, 1e-9), "Imc1": (2e-9, 1e-12), "Imc2": (2e-9, 1e-6)}.get(f, (1e-7, 1e-9))
+            ok = np.allclose(fast[k], gen[k], rtol=rtol, atol=atol, equal_nan=True)
         else:
             ok = np.allclose(fast[k], gen[k], rtol=1e-10, atol=1e-12, equal_nan=True)
         assert ok, (cname, f, np.nanmax(np.abs(fast[k] - gen[k])))

@@ -83,8 +83,13 @@ def test_slab_and_reflection_properties_at_scale(cname):
     flipped = voxel.voxel_features(cname, lev.flip(2).contiguous(), s).flip(3)
     a, b = whole.cpu().numpy(), flipped.cpu().numpy()
     assert np.isfinite(a).all()
-    # MCC eigen-tasks keep their Lanczos vectors in float32: reflection-invariant to ~1e-7 only
-    assert np.allclose(a, b, rtol=2e-6 if cname == "glcm" else 1e-9, atol=1e-12)
+    # the MCC eigen-tasks see a reflected window's levels in another order, so MCC moves by fp64 rounding: each run is
+    # within 1e-9 of LAPACK (tests/test_fast_voxel_windows_gpu.py), an absolute bound whatever the size of MCC
+    if cname == "glcm":
+        k = _lib.feature_names("glcm").index("MCC")
+        assert np.allclose(a[k], b[k], rtol=0, atol=2e-9)
+        a, b = np.delete(a, k, 0), np.delete(b, k, 0)
+    assert np.allclose(a, b, rtol=1e-9, atol=1e-12)
 
 
 def test_tensor_api_matches_host_api():
@@ -109,9 +114,13 @@ def test_glcm_fast_path_equals_generic_kernel(kind, monkeypatch):
     monkeypatch.delenv("B200_RADIOMICS_FORCE_GENERIC")
     names = _lib.feature_names("glcm")
     for k, f in enumerate(names):
-        # MCC / Imc2 of near-degenerate angles are rounding noise in every implementation
-        atol = 1e-6 if f in ("MCC", "Imc2", "Imc1") else 1e-9
-        assert np.allclose(fast[k], gen[k], rtol=1e-7, atol=atol, equal_nan=True), f
+        # MCC: both solves are within 1e-9 of LAPACK (tests/test_fast_voxel_windows_gpu.py), an absolute bound.
+        # Imc2: on an angle of exactly independent margins the generic kernel keeps the reference's exact comparison of two
+        # rounded entropies (NaN, dropped, or the square root of their rounding noise, up to ~1e-7) and the fast path
+        # takes 0 (DESIGN.md section 5), so 1e-6 stays; tests/test_fast_voxel_windows_gpu.py checks both against the
+        # oracle with independence decided exactly.
+        rtol, atol = {"MCC": (0, 1e-9), "Imc1": (2e-9, 1e-12), "Imc2": (2e-9, 1e-6)}.get(f, (1e-7, 1e-9))
+        assert np.allclose(fast[k], gen[k], rtol=rtol, atol=atol, equal_nan=True), f
 
 
 @pytest.mark.parametrize("kind", ["uniform", "smooth"])
