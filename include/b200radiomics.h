@@ -166,21 +166,23 @@ void rb_glszm_release(void *handle);
 
 /* Segment-based matrices straight from a DEVICE-resident packed level volume (rb_pack_levels_dev) -- what the plugin
  * classes call once the image has been discretised on the GPU, instead of shipping it back to the host for the entry
- * points above.  Same matrices / layouts / angle order; results in HOST float64 buffers; synchronous.
+ * points above.  Same matrices / layouts / angle order; results in HOST float64 buffers.  Every launch and copy runs on
+ * `stream`, so the levels may still be in flight on it; each call returns once `stream` has reached its results.
  * rb_segment_texture_dev builds GLCM, GLDM and NGTDM in ONE pass over the volume (NULL = not wanted): a CTA stages a box
  *   of the level volume in shared memory -- through TMA (cp.async.bulk.tensor.3d with hardware zero-fill outside the
  *   volume) when the row pitch is a multiple of 16 bytes, else by cooperative loads -- and accumulates the three
  *   matrices in shared-memory histograms (reference radiomics/src/cmatrices.c:4-92, 660-754, 543-658).  `distances`
  *   drives all three (the GLCM uses the unidirectional half of the offsets).
  * rb_segment_glrlm_dev: every run END walks back to the start of its run (cmatrices.c:299-541).
- * rb_segment_glszm_dev: phase one of GLSZM as rb_calculate_glszm (finish with rb_fill_glszm / rb_glszm_release). */
+ * rb_segment_glszm_dev: phase one of GLSZM as rb_calculate_glszm (finish with rb_fill_glszm / rb_glszm_release); the
+ *   handle keeps `stream`, and rb_fill_glszm runs on it too. */
 int rb_segment_texture_dev(const void *levels_dev, int level_bytes, const int *size, int nd, const int *distances,
                            int ndist, int Ng, int alpha, int force2D, int force2Ddimension, double *glcm, double *gldm,
-                           double *ngtdm, int *angles);
+                           double *ngtdm, int *angles, void *stream);
 int rb_segment_glrlm_dev(const void *levels_dev, int level_bytes, const int *size, int nd, int Ng, int Nr, int force2D,
-                         int force2Ddimension, double *glrlm, int *angles);
+                         int force2Ddimension, double *glrlm, int *angles, void *stream);
 int rb_segment_glszm_dev(const void *levels_dev, int level_bytes, const int *size, int nd, int Ng, int force2D,
-                         int force2Ddimension, int *max_region, void **handle);
+                         int force2Ddimension, int *max_region, void **handle, void *stream);
 
 /* ---- gray-level discretisation and pre-filters (device pointers, asynchronous) --------------
  * Pixel types: every `dtype` argument is an rb_dtype code; any other value gives RB_ERR_ARG. */

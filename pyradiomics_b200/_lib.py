@@ -83,9 +83,9 @@ PROTOTYPES = {
     "rb_calculate_glszm": (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _p, _i, _p, _p]),
     "rb_fill_glszm": (_i, [_p, _i, _i, _p]),
     "rb_glszm_release": (None, [_p]),
-    "rb_segment_texture_dev": (_i, [_p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
-    "rb_segment_glrlm_dev": (_i, [_p, _i, _p, _i, _i, _i, _i, _i, _p, _p]),
-    "rb_segment_glszm_dev": (_i, [_p, _i, _p, _i, _i, _i, _i, _p, _p]),
+    "rb_segment_texture_dev": (_i, [_p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "rb_segment_glrlm_dev": (_i, [_p, _i, _p, _i, _i, _i, _i, _i, _p, _p, _p]),
+    "rb_segment_glszm_dev": (_i, [_p, _i, _p, _i, _i, _i, _i, _p, _p, _p]),
     "rb_minmax_dev": (_i, [_p, _i, _p, _ll, _p, _p]),
     "rb_digitize_dev": (_i, [_p, _i, _p, _ll, _p, _i, _p, _p]),
     "rb_swt_axis_dev": (_i, [_p, _i, _i, _i, _i, _p, _p, _i, _p, _p, _p]),

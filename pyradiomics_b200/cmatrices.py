@@ -10,7 +10,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import check, lib, ptr
+from ._lib import check, lib, ptr, stream
 
 
 def _arrays(image, mask):
@@ -121,7 +121,8 @@ def calculate_gldm(image, mask, distances, Ng, alpha, force2D, force2Ddimension,
 # ---------------------------------------------------------------------------------------------------------------------
 # Device-resident variants: the same matrices from a packed level volume that is already on the GPU (a CUDA tensor from
 # rb_pack_levels_dev) -- what the plugin classes use in segment-based mode, so the discretised image never returns to
-# the host (the reference hands cMatrices the host array it binned in Python, radiomics/glcm.py:145 etc.).
+# the host (the reference hands cMatrices the host array it binned in Python, radiomics/glcm.py:145 etc.).  They run on
+# torch's current stream, the one the levels were written on.
 def _dev_args(levels):
     import torch
     assert isinstance(levels, torch.Tensor) and levels.is_cuda and levels.is_contiguous() and levels.ndim in (2, 3)
@@ -142,7 +143,8 @@ def segment_texture_device(levels, distances, Ng, alpha, force2D, force2Ddimensi
     P_gldm = np.empty((1, Ng, 2 * ang_bi.shape[0] + 1), dtype=np.float64) if gldm else None
     P_ngtdm = np.empty((1, Ng, 3), dtype=np.float64) if ngtdm else None
     check(lib().rb_segment_texture_dev(lev, lb, ptr(size), int(size.size), ptr(d), int(d.size), int(Ng), int(alpha), int(bool(force2D)),
-                                       int(force2Ddimension), ptr(P_glcm), ptr(P_gldm), ptr(P_ngtdm), None), "GLCM/GLDM/NGTDM")
+                                       int(force2Ddimension), ptr(P_glcm), ptr(P_gldm), ptr(P_ngtdm), None, stream()),
+          "GLCM/GLDM/NGTDM")
     if glcm:
         out["glcm"] = (P_glcm, ang)
     if gldm:
@@ -157,7 +159,7 @@ def calculate_glrlm_device(levels, Ng, Nr, force2D, force2Ddimension):
     ang = generate_angles(size, [1], 0, force2D, force2Ddimension)
     out = np.empty((1, Ng, int(Nr), ang.shape[0]), dtype=np.float64)
     check(lib().rb_segment_glrlm_dev(lev, lb, ptr(size), int(size.size), int(Ng), int(Nr), int(bool(force2D)), int(force2Ddimension),
-                                     ptr(out), None), "GLRLM")
+                                     ptr(out), None, stream()), "GLRLM")
     return out, ang
 
 
@@ -167,7 +169,7 @@ def calculate_glszm_device(levels, Ng, force2D, force2Ddimension):
     mx = C.c_int(0)
     handle = C.c_void_p()
     check(lib().rb_segment_glszm_dev(lev, lb, ptr(size), int(size.size), int(Ng), int(bool(force2D)), int(force2Ddimension),
-                                     C.byref(mx), C.byref(handle)), "GLSZM")
+                                     C.byref(mx), C.byref(handle), stream()), "GLSZM")
     max_region = max(1, mx.value)
     out = np.empty((1, Ng, max_region), dtype=np.float64)
     check(lib().rb_fill_glszm(handle, int(Ng), max_region, ptr(out)), "GLSZM")

@@ -53,16 +53,18 @@ static bool force_generic() {
 int calculate_matrix_host(int mode, const int32_t* image, const uint8_t* mask, const int* size, int nd,
                           const int* distances, int ndist, int Ng, int Nr, int alpha, int force2D, int force2Ddimension,
                           int kernelRadius, const int* voxels, int nvox, double* out_host, int* angles_out);
+int upload_levels(const int32_t* image, const uint8_t* mask, long long n, int Ng, DevBuf& lev, int* status_dev);
 int glszm_zones_host(const int32_t* image, const uint8_t* mask, const int* size, int nd, int Ng, int force2D,
                      int force2Ddimension, int kernelRadius, const int* voxels, int nvox, int* max_region_out,
-                     void** handle_out, const void* levels_dev = nullptr);
-int segment_matrices(const void* lev, int level_bytes, int nd, int Z, int Y, int X, const int* distances, int ndist, int Ng,
-                     int alpha, int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
-                     int* angles_out, cudaStream_t st);
-int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X, int Ng, int Nr, int force2D, int force2Ddimension,
-                  double* glrlm_host, int* angles_out, cudaStream_t st);
-int glszm_fill_host(void* handle, int Ng, int max_region, double* out_host);
-void glszm_release(void* handle);
+                     void** handle_out);
+int glszm_fill(void* handle, int Ng, int max_region, double* out_host);
+
+// the arguments every rb_segment_*_dev entry point checks before it touches the device
+static int check_segment_levels(const void* levels_dev, int level_bytes, const int* size, int nd, int Ng) {
+  if (!levels_dev || !size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "levels / size");
+  if (level_bytes != rb_level_bytes(Ng)) return fail(RB_ERR_ARG, "level_bytes does not match Ng");
+  return RB_OK;
+}
 
 int minmax_launch(const void* img, int dt, const uint8_t* mask, long long n, long long* keys, cudaStream_t st);
 int shape_coefficients_dev(const uint8_t* mask_dev, int Z, int Y, int X, long long sz, long long sy, long long sx,
@@ -234,18 +236,13 @@ int rb_voxel_features_host(int cls, const int32_t* image, const uint8_t* mask, i
   const long long n = (long long)Z * Y * X;
   const int nf = kNumFeatures[cls];
   const int lb = rb_level_bytes(settings->Ng);
-  DevBuf img, msk, lev, out, status, alive_dev;
-  RB_CUDA(img.alloc(n * 4));
-  RB_CUDA(msk.alloc(n));
-  RB_CUDA(lev.alloc(n * lb));
+  DevBuf lev, out, status, alive_dev;
   RB_CUDA(out.alloc(sizeof(double) * n * nf));
   RB_CUDA(status.alloc(2 * sizeof(int)));
   RB_CUDA(alive_dev.alloc(RB_ALIVE_WORDS * 4));
   RB_CUDA(cudaMemsetAsync(status.p, 0, 2 * sizeof(int), 0));
   RB_CUDA(cudaMemsetAsync(alive_dev.p, 0, RB_ALIVE_WORDS * 4, 0));
-  RB_CUDA(cudaMemcpyAsync(img.p, image, n * 4, cudaMemcpyHostToDevice, 0));
-  RB_CUDA(cudaMemcpyAsync(msk.p, mask, n, cudaMemcpyHostToDevice, 0));
-  int rc = rb_pack_levels_dev(img.as<int32_t>(), msk.as<uint8_t>(), n, settings->Ng, lev.p, NULL, status.as<int>(), 0);
+  int rc = upload_levels(image, mask, n, settings->Ng, lev, status.as<int>());
   if (rc) return rc;
   uint32_t alive[RB_ALIVE_WORDS];
   if (cls == RB_GLCM) {
@@ -290,24 +287,22 @@ int rb_calculate_ngtdm(const int32_t* image, const uint8_t* mask, const int* siz
 // ---- segment-mode matrices from a device-resident packed level volume (no host round trip of the image)
 int rb_segment_texture_dev(const void* levels_dev, int level_bytes, const int* size, int nd, const int* distances, int ndist,
                            int Ng, int alpha, int force2D, int force2Ddimension, double* glcm, double* gldm, double* ngtdm,
-                           int* angles) {
-  if (!levels_dev || !size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "levels / size");
-  if (level_bytes != rb_level_bytes(Ng)) return fail(RB_ERR_ARG, "level_bytes does not match Ng");
-  return segment_matrices(levels_dev, level_bytes, nd, nd == 3 ? size[0] : 1, size[nd - 2], size[nd - 1], distances, ndist, Ng,
-                          alpha, force2D, force2Ddimension, glcm, gldm, ngtdm, angles, 0);
+                           int* angles, void* stream) {
+  if (int rc = check_segment_levels(levels_dev, level_bytes, size, nd, Ng)) return rc;
+  return segment_matrices(levels_dev, level_bytes, size, nd, distances, ndist, Ng, alpha, force2D, force2Ddimension, glcm,
+                          gldm, ngtdm, angles, (cudaStream_t)stream);
 }
 int rb_segment_glrlm_dev(const void* levels_dev, int level_bytes, const int* size, int nd, int Ng, int Nr, int force2D,
-                         int force2Ddimension, double* glrlm, int* angles) {
-  if (!levels_dev || !size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "levels / size");
-  if (level_bytes != rb_level_bytes(Ng)) return fail(RB_ERR_ARG, "level_bytes does not match Ng");
-  return segment_glrlm(levels_dev, level_bytes, nd, nd == 3 ? size[0] : 1, size[nd - 2], size[nd - 1], Ng, Nr, force2D,
-                       force2Ddimension, glrlm, angles, 0);
+                         int force2Ddimension, double* glrlm, int* angles, void* stream) {
+  if (int rc = check_segment_levels(levels_dev, level_bytes, size, nd, Ng)) return rc;
+  return segment_glrlm(levels_dev, level_bytes, size, nd, Ng, Nr, force2D, force2Ddimension, glrlm, angles,
+                       (cudaStream_t)stream);
 }
 int rb_segment_glszm_dev(const void* levels_dev, int level_bytes, const int* size, int nd, int Ng, int force2D,
-                         int force2Ddimension, int* max_region, void** handle) {
-  if (!levels_dev || !size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "levels / size");
-  if (level_bytes != rb_level_bytes(Ng)) return fail(RB_ERR_ARG, "level_bytes does not match Ng");
-  return glszm_zones_host(NULL, NULL, size, nd, Ng, force2D, force2Ddimension, 0, NULL, 1, max_region, handle, levels_dev);
+                         int force2Ddimension, int* max_region, void** handle, void* stream) {
+  if (int rc = check_segment_levels(levels_dev, level_bytes, size, nd, Ng)) return rc;
+  return segment_glszm(levels_dev, level_bytes, size, nd, Ng, force2D, force2Ddimension, max_region, handle,
+                       (cudaStream_t)stream);
 }
 
 int rb_calculate_glszm(const int32_t* image, const uint8_t* mask, const int* size, int nd, int Ng, int force2D,
@@ -317,8 +312,8 @@ int rb_calculate_glszm(const int32_t* image, const uint8_t* mask, const int* siz
   return glszm_zones_host(image, mask, size, nd, Ng, force2D, force2Ddimension, kernelRadius, voxels, nvox, max_region,
                           handle);
 }
-int rb_fill_glszm(void* handle, int Ng, int max_region, double* glszm) { return glszm_fill_host(handle, Ng, max_region, glszm); }
-void rb_glszm_release(void* handle) { glszm_release(handle); }
+int rb_fill_glszm(void* handle, int Ng, int max_region, double* glszm) { return glszm_fill(handle, Ng, max_region, glszm); }
+void rb_glszm_release(void* handle) { delete (GlszmHandle*)handle; }
 
 int rb_minmax_dev(const void* image_dev, int dtype, const uint8_t* mask_dev, long long nvoxels, long long* keys_dev,
                   void* stream) {

@@ -60,6 +60,27 @@ struct DevBuf {
   template <typename U> U* as() const { return (U*)p; }
 };
 
+// The opaque handle between GLSZM's two phases: the zones as (gray, size) int pairs, and the stream phase one ran on,
+// where the fill (matrix_kernels.cu glszm_fill) runs too.
+struct GlszmHandle {
+  bool batch = false;
+  cudaStream_t st = 0;
+  int nvox = 1, wcap = 0;
+  unsigned nzones = 0;
+  DevBuf zones;   // segment: int[2*nzones]; batch: int[nvox][2*wcap]
+  DevBuf nz;      // batch: int[nvox]
+};
+
+// Segment-mode builders (segment_kernels.cu): one ROI's matrices from packed levels (uint8 or uint16, size[nd], nd = 2
+// or 3) into HOST float64 buffers, or GLSZM's zones into a new handle; every launch and copy runs on `st`.
+int segment_matrices(const void* lev, int level_bytes, const int* size, int nd, const int* distances, int ndist, int Ng,
+                     int alpha, int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
+                     int* angles_out, cudaStream_t st);
+int segment_glrlm(const void* lev, int level_bytes, const int* size, int nd, int Ng, int Nr, int force2D, int force2Ddimension,
+                  double* glrlm_host, int* angles_out, cudaStream_t st);
+int segment_glszm(const void* lev, int level_bytes, const int* size, int nd, int Ng, int force2D, int force2Ddimension,
+                  int* max_region, void** handle, cudaStream_t st);
+
 // SM count of the current device (132 if it cannot be queried)
 inline int sm_count() {
   int dev = 0, sms = 132;

@@ -54,6 +54,19 @@ struct AngleSet {
   int8_t a[NA_MAX][3];
 };
 
+// The front end every segment-mode builder starts from (segment_geometry, segment_kernels.cu): the volume as Z x Y x X
+// (a 2-D image is one plane) and its offsets as (dz, dy, dx) rows.
+struct SegmentGeometry {
+  int Z, Y, X;
+  long long n;   // Z * Y * X, 1..2^31-1
+  AngleSet A;
+  int H;         // largest |offset component|
+};
+// Checks Ng (1..65535), the voxel count and the offset count (at most na_max; "more than NA_MAX angles" counts both
+// directions); angles_out (may be NULL) receives the offsets as the reference returns them, Na x nd.
+int segment_geometry(const int* size, int nd, const int* distances, int ndist, bool bidirectional, int force2D,
+                     int force2Ddimension, int Ng, int na_max, int* angles_out, SegmentGeometry& G);
+
 enum Weighting { W_NONE = 0, W_INFINITY = 1, W_EUCLIDEAN = 2, W_MANHATTAN = 3, W_NO_WEIGHTING = 4 };
 enum TexClass { C_GLCM = 0, C_GLRLM = 1, C_GLSZM = 2, C_GLDM = 3, C_NGTDM = 4 };
 static const int kNumFeatures[5] = {GLCM_NF, GLRLM_NF, GLSZM_NF, GLDM_NF, NGTDM_NF};

@@ -1,85 +1,21 @@
 // Texture-MATRIX builders of the cMatrices API surface (what reference radiomics/src/cmatrices.c computes) from host
 // image + mask: prepare() uploads and packs the levels (range check), then
 //
-//   segment mode : GLCM / GLDM / NGTDM / GLRLM go to segment_matrices / segment_glrlm (segment_kernels.cu); GLSZM is
-//                  here: union-find connected-component labelling (26-neighbourhood, equal gray level) + zone-size
-//                  histogram.
+//   segment mode : segment_matrices / segment_glrlm / segment_glszm (segment_kernels.cu), on the default stream.
 //   voxel batch  : one thread per listed voxel writes its private dense matrix (no atomics, reference
 //                  radiomics/src/_cmatrices.c:203-207 etc.); this is the API-compatibility path -- the product's
 //                  voxel-based features never materialise these (see voxel_kernels.cu / voxel_fast.cu).
+// GLSZM is two-phase in both modes: phase one leaves its zones in a GlszmHandle, glszm_fill turns them into the matrix.
 #include "common.cuh"
 #include "host_common.hpp"
 #include "vox_features.cuh"
 
 namespace rb {
 
-struct Vol {
-  int Z, Y, X;
-  __host__ __device__ long long n() const { return (long long)Z * Y * X; }
-  __device__ bool in(int z, int y, int x) const { return z >= 0 && z < Z && y >= 0 && y < Y && x >= 0 && x < X; }
-  __device__ long long idx(int z, int y, int x) const { return ((long long)z * Y + y) * X + x; }
-};
-
 // u32 counts -> float64 (segment_kernels.cu)
 __global__ void u32_to_f64_kernel(const unsigned* __restrict__ hist, long long n, double* __restrict__ out);
 
-// ---- GLSZM (segment): union-find connected components over equal-level 26/8-neighbours -----
-__device__ __forceinline__ int uf_find(int* L, int i) {
-  int p = L[i];
-  while (p != i) { i = p; p = L[i]; }
-  return i;
-}
-__device__ __forceinline__ void uf_union(int* L, int a, int b) {
-  while (true) {
-    a = uf_find(L, a); b = uf_find(L, b);
-    if (a == b) return;
-    if (a < b) { const int t = a; a = b; b = t; }
-    const int old = atomicMin(&L[a], b);
-    if (old == a) return;
-    a = old;
-  }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) ccl_init_kernel(const T* __restrict__ lev, long long n, int* __restrict__ L) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    L[i] = lev[i] ? (int)i : -1;
-}
-template <typename T>
-__global__ void __launch_bounds__(256)
-ccl_merge_kernel(const T* __restrict__ lev, Vol V, const __grid_constant__ AngleSet A, int* __restrict__ L) {
-  const long long n = V.n(), plane = (long long)V.Y * V.X;
-  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x) {
-    const int g = lev[t];
-    if (!g) continue;
-    const int z = (int)(t / plane), rem = (int)(t % plane), y = rem / V.X, x = rem % V.X;
-    for (int a = 0; a < A.na; a++) {       // unidirectional half of the neighbourhood is enough
-      const int z2 = z + A.a[a][0], y2 = y + A.a[a][1], x2 = x + A.a[a][2];
-      if (!V.in(z2, y2, x2)) continue;
-      const long long j = V.idx(z2, y2, x2);
-      if (lev[j] == g) uf_union(L, (int)t, (int)j);
-    }
-  }
-}
-__global__ void __launch_bounds__(256) ccl_count_kernel(int* __restrict__ L, long long n, unsigned* __restrict__ size) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    if (L[i] < 0) continue;
-    const int r = uf_find(L, (int)i);
-    atomicAdd(&size[r], 1u);
-  }
-}
-template <typename T>
-__global__ void __launch_bounds__(256)
-ccl_zones_kernel(const T* __restrict__ lev, const int* __restrict__ L, const unsigned* __restrict__ size, long long n,
-                 int* __restrict__ zones, unsigned* __restrict__ nzones, unsigned* __restrict__ max_region) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    if (L[i] != (int)i) continue;            // roots only
-    const unsigned k = atomicAdd(nzones, 1u);
-    zones[2 * (size_t)k] = lev[i];
-    zones[2 * (size_t)k + 1] = (int)size[i];
-    atomicMax(max_region, size[i]);
-  }
-}
+// GLSZM (segment) phase two: the (gray, size) pairs of segment_glszm -> u32 histogram [Ng][max_region]
 __global__ void __launch_bounds__(256)
 zones_fill_kernel(const int* __restrict__ zones, unsigned nzones, int Ng, int max_region, unsigned* __restrict__ hist,
                   int* __restrict__ status) {
@@ -225,52 +161,44 @@ batch_glszm_fill_kernel(const int* __restrict__ zones, const int* __restrict__ n
 int pack_levels(const int32_t* image, const uint8_t* mask, long long n, int Ng, void* lev, uint32_t* presence,
                 int* status, cudaStream_t st);
 
+// Host image + mask -> packed levels in `lev` (1 byte per voxel when Ng <= 255, else 2) on the default stream; a gray
+// level outside 1..Ng inside the mask sets bit 0 of *status_dev (zeroed by the caller).
+int upload_levels(const int32_t* image, const uint8_t* mask, long long n, int Ng, DevBuf& lev, int* status_dev) {
+  DevBuf dimg, dmsk;
+  RB_CUDA(dimg.alloc(n * 4));
+  RB_CUDA(dmsk.alloc(n));
+  RB_CUDA(lev.alloc(n * (Ng <= 255 ? 1 : 2)));
+  RB_CUDA(cudaMemcpyAsync(dimg.p, image, n * 4, cudaMemcpyHostToDevice, 0));
+  RB_CUDA(cudaMemcpyAsync(dmsk.p, mask, n, cudaMemcpyHostToDevice, 0));
+  const int rc = pack_levels(dimg.as<int32_t>(), dmsk.as<uint8_t>(), n, Ng, lev.p, nullptr, status_dev, 0);
+  if (rc) return rc;
+  RB_CUDA(cudaStreamSynchronize(0));     // dimg / dmsk go out of scope
+  return RB_OK;
+}
+
 struct Prepared {
-  int nd, Z, Y, X, f2, lb;
-  long long n;
-  const void* lev = nullptr;   // own_lev.p, or the caller's device-resident packed levels (borrowed, not freed)
-  DevBuf own_lev, status, vox;
-  AngleSet A;
-  int na;
-  std::vector<int> ang_nd;   // Na x nd, as the reference returns them
+  SegmentGeometry G;
+  int nd, f2, lb;
+  DevBuf lev, status, vox;
 };
 
-// common front end: shapes, angles, upload + pack (range check), optional voxel list upload
+// common front end of the host-pointer API: segment geometry (angles_out, may be NULL, gets the offsets), upload + pack
+// (range check), optional voxel list upload
 static int prepare(const int32_t* image, const uint8_t* mask, const int* size, int nd, const int* distances, int ndist,
                    bool bidirectional, int Ng, int force2D, int force2Ddimension, const int* voxels, int nvox,
-                   int kernelRadius, Prepared& R, const void* levels_dev = nullptr) {
-  if (!size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "image/mask must be 2-D or 3-D");
-  if (Ng < 1 || Ng > 65535) return fail(RB_ERR_UNSUPPORTED, "Ng=%d outside 1..65535", Ng);
+                   int kernelRadius, int* angles_out, Prepared& R) {
+  if (!image || !mask || !size || (nd != 2 && nd != 3)) return fail(RB_ERR_ARG, "image/mask must be 2-D or 3-D");
   if (voxels && kernelRadius <= 0) return fail(RB_ERR_ARG, "Expecting kernelRadius > 0");
+  int rc = segment_geometry(size, nd, distances, ndist, bidirectional, force2D, force2Ddimension, Ng, NA_MAX, angles_out,
+                            R.G);
+  if (rc) return rc;
   R.nd = nd;
-  R.Z = nd == 3 ? size[0] : 1; R.Y = size[nd - 2]; R.X = size[nd - 1];
-  R.n = (long long)R.Z * R.Y * R.X;
-  if (R.n <= 0 || R.n >= (1ll << 31)) return fail(RB_ERR_UNSUPPORTED, "volume must have 1..2^31-1 voxels");
-  const int f2_nd = force2D ? force2Ddimension : -1;
-  R.f2 = f2_nd < 0 ? -1 : f2_nd + (3 - nd);
-  R.na = generate_angles(size, nd, distances, ndist, bidirectional, f2_nd, R.ang_nd);
-  if (R.na <= 0) return fail(RB_ERR_ARG, "Error getting angle count.");
-  if (R.na > NA_MAX) return fail(RB_ERR_UNSUPPORTED, "more than %d angles", NA_MAX);
-  R.A.na = R.na;
-  for (int a = 0; a < R.na; a++)
-    for (int d = 0; d < 3; d++) R.A.a[a][d] = d < 3 - nd ? 0 : (int8_t)R.ang_nd[a * nd + d - (3 - nd)];
+  R.f2 = force2D ? force2Ddimension + (3 - nd) : -1;
   R.lb = Ng <= 255 ? 1 : 2;
-  DevBuf dimg, dmsk;
-  RB_CUDA(R.status.alloc(16));
-  RB_CUDA(cudaMemsetAsync(R.status.p, 0, 16, 0));
-  if (levels_dev) {                                  // device-resident packed levels (rb_pack_levels_dev)
-    R.lev = levels_dev;
-  } else {
-    if (!image || !mask) return fail(RB_ERR_ARG, "image/mask must be 2-D or 3-D");
-    RB_CUDA(dimg.alloc(R.n * 4));
-    RB_CUDA(dmsk.alloc(R.n));
-    RB_CUDA(R.own_lev.alloc(R.n * R.lb));
-    R.lev = R.own_lev.p;
-    RB_CUDA(cudaMemcpyAsync(dimg.p, image, R.n * 4, cudaMemcpyHostToDevice, 0));
-    RB_CUDA(cudaMemcpyAsync(dmsk.p, mask, R.n, cudaMemcpyHostToDevice, 0));
-    int rc = pack_levels(dimg.as<int32_t>(), dmsk.as<uint8_t>(), R.n, Ng, R.own_lev.p, nullptr, R.status.as<int>(), 0);
-    if (rc) return rc;
-  }
+  RB_CUDA(R.status.alloc(4));
+  RB_CUDA(cudaMemsetAsync(R.status.p, 0, 4, 0));
+  rc = upload_levels(image, mask, R.G.n, Ng, R.lev, R.status.as<int>());
+  if (rc) return rc;
   if (voxels) {
     if (nvox < 1) return fail(RB_ERR_ARG, "empty voxel list");
     std::vector<int> v3((size_t)3 * nvox, 0);
@@ -284,21 +212,19 @@ static int prepare(const int32_t* image, const uint8_t* mask, const int* size, i
     RB_CUDA(cudaMemcpyAsync(R.vox.p, v3.data(), sizeof(int) * 3 * (size_t)nvox, cudaMemcpyHostToDevice, 0));
     RB_CUDA(cudaStreamSynchronize(0));   // v3 is a temporary
   }
-  RB_CUDA(cudaStreamSynchronize(0));     // dimg/dmsk go out of scope
   return RB_OK;
 }
 
-static int check_status(Prepared& R, const char* what) {
-  int st[4] = {0, 0, 0, 0};
-  RB_CUDA(cudaMemcpy(st, R.status.p, sizeof st, cudaMemcpyDeviceToHost));
-  if (st[0] & 1) return fail(RB_ERR_LEVEL_RANGE, "Calculation of %s Failed: gray level outside 1..Ng inside the mask", what);
-  if (st[1] & 1) return fail(RB_ERR_LEVEL_RANGE, "Calculation of %s Failed: index out of range", what);
+static int check_status(const Prepared& R, const char* what) {
+  int st = 0;
+  RB_CUDA(cudaMemcpy(&st, R.status.p, sizeof st, cudaMemcpyDeviceToHost));
+  if (st & 1) return fail(RB_ERR_LEVEL_RANGE, "Calculation of %s Failed: gray level outside 1..Ng inside the mask", what);
   return RB_OK;
 }
 
 static BatchGeom batch_geom(const Prepared& R, int kernelRadius, int nvox) {
   BatchGeom G;
-  G.Z = R.Z; G.Y = R.Y; G.X = R.X; G.nvox = nvox;
+  G.Z = R.G.Z; G.Y = R.G.Y; G.X = R.G.X; G.nvox = nvox;
   G.rz = (R.f2 == 0 || R.nd == 2) ? 0 : kernelRadius;
   G.ry = R.f2 == 1 ? 0 : kernelRadius;
   G.rx = R.f2 == 2 ? 0 : kernelRadius;
@@ -309,21 +235,15 @@ template <typename T, int MODE>
 static int launch_batch(const Prepared& R, const BatchGeom& G, int Ng, int Nr, int alpha, double* out) {
   const int cap = (2 * G.rz + 1) * (2 * G.ry + 1) * (2 * G.rx + 1);
   const int grid = (G.nvox + 127) / 128;
-  const T* lev = (const T*)R.lev;
-  const int* vox = (const int*)R.vox.p;
-  if (cap <= 27) batch_matrix_kernel<T, 27, MODE><<<grid, 128>>>(lev, G, vox, R.A, Ng, Nr, alpha, out);
-  else if (cap <= 125) batch_matrix_kernel<T, 125, MODE><<<grid, 128>>>(lev, G, vox, R.A, Ng, Nr, alpha, out);
-  else if (cap <= 343) batch_matrix_kernel<T, 343, MODE><<<grid, 128>>>(lev, G, vox, R.A, Ng, Nr, alpha, out);
+  const T* lev = R.lev.as<const T>();
+  const int* vox = R.vox.as<const int>();
+  if (cap <= 27) batch_matrix_kernel<T, 27, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out);
+  else if (cap <= 125) batch_matrix_kernel<T, 125, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out);
+  else if (cap <= 343) batch_matrix_kernel<T, 343, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out);
   else return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
-
-int segment_matrices(const void* lev, int level_bytes, int nd, int Z, int Y, int X, const int* distances, int ndist, int Ng,
-                     int alpha, int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
-                     int* angles_out, cudaStream_t st);
-int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X, int Ng, int Nr, int force2D, int force2Ddimension,
-                  double* glrlm_host, int* angles_out, cudaStream_t st);
 
 // one driver for GLCM (mode 0) / GLDM (1) / NGTDM (2) / GLRLM (3) from host image + mask
 int calculate_matrix_host(int mode, const int32_t* image, const uint8_t* mask, const int* size, int nd,
@@ -334,18 +254,18 @@ int calculate_matrix_host(int mode, const int32_t* image, const uint8_t* mask, c
   const int one[1] = {1};
   const bool bidir = mode == 1 || mode == 2;
   int rc = prepare(image, mask, size, nd, mode == 3 ? one : distances, mode == 3 ? 1 : ndist, bidir, Ng, force2D,
-                   force2Ddimension, voxels, nvox, kernelRadius, R);
+                   force2Ddimension, voxels, nvox, kernelRadius, angles_out, R);
   if (rc) return rc;
   if (!voxels) {
-    rc = mode == 3 ? segment_glrlm(R.lev, R.lb, nd, R.Z, R.Y, R.X, Ng, Nr, force2D, force2Ddimension, out_host, angles_out, 0)
-                   : segment_matrices(R.lev, R.lb, nd, R.Z, R.Y, R.X, distances, ndist, Ng, alpha, force2D, force2Ddimension,
+    rc = mode == 3 ? segment_glrlm(R.lev.p, R.lb, size, nd, Ng, Nr, force2D, force2Ddimension, out_host, angles_out, 0)
+                   : segment_matrices(R.lev.p, R.lb, size, nd, distances, ndist, Ng, alpha, force2D, force2Ddimension,
                                       mode == 0 ? out_host : nullptr, mode == 1 ? out_host : nullptr,
                                       mode == 2 ? out_host : nullptr, angles_out, 0);
     return rc ? rc : check_status(R, names[mode]);
   }
-  if (angles_out) memcpy(angles_out, R.ang_nd.data(), sizeof(int) * R.ang_nd.size());
-  size_t per = mode == 0 ? (size_t)Ng * Ng * R.na : mode == 1 ? (size_t)Ng * (2 * R.na + 1) : mode == 2 ? (size_t)Ng * 3
-                                                                                                  : (size_t)Ng * Nr * R.na;
+  const int na = R.G.A.na;
+  size_t per = mode == 0 ? (size_t)Ng * Ng * na : mode == 1 ? (size_t)Ng * (2 * na + 1) : mode == 2 ? (size_t)Ng * 3
+                                                                                            : (size_t)Ng * Nr * na;
   if (mode == 3 && Nr < 1) return fail(RB_ERR_ARG, "Nr must be >= 1");
   DevBuf dout;
   RB_CUDA(dout.alloc(sizeof(double) * per * nvox));
@@ -363,108 +283,71 @@ int calculate_matrix_host(int mode, const int32_t* image, const uint8_t* mask, c
 }
 
 // ---- GLSZM two-phase --------------------------------------------------------------------
-struct GlszmHandle {
-  bool batch;
-  int nvox, wcap, Ng;
-  unsigned nzones;
-  DevBuf zones;   // segment: int[2*nzones]; batch: int[nvox][2*wcap]
-  DevBuf nz;      // batch: int[nvox]
-};
-
+// phase one from host image + mask: the whole ROI (segment mode) or one zone list per listed voxel
 int glszm_zones_host(const int32_t* image, const uint8_t* mask, const int* size, int nd, int Ng, int force2D,
                      int force2Ddimension, int kernelRadius, const int* voxels, int nvox, int* max_region_out,
-                     void** handle_out, const void* levels_dev) {
+                     void** handle_out) {
   Prepared R;
   const int one[1] = {1};
-  int rc = prepare(image, mask, size, nd, one, 1, true, Ng, force2D, force2Ddimension, voxels, nvox, kernelRadius, R, levels_dev);
+  int rc = prepare(image, mask, size, nd, one, 1, true, Ng, force2D, force2Ddimension, voxels, nvox, kernelRadius, nullptr, R);
   if (rc) return rc;
   rc = check_status(R, "GLSZM");
   if (rc) return rc;
+  if (!voxels) return segment_glszm(R.lev.p, R.lb, size, nd, Ng, force2D, force2Ddimension, max_region_out, handle_out, 0);
+  BatchGeom G = batch_geom(R, kernelRadius, nvox);
+  const int cap = (2 * G.rz + 1) * (2 * G.ry + 1) * (2 * G.rx + 1);
+  const int wcap = cap <= 27 ? 27 : cap <= 125 ? 125 : 343;
+  if (cap > 343) return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
   std::unique_ptr<GlszmHandle> H(new GlszmHandle);   // handed to the caller only on success
-  H->Ng = Ng;
-  DevBuf scal;   // [0] nzones, [1] max_region
-  RB_CUDA(scal.alloc(8));
-  cudaMemsetAsync(scal.p, 0, 8, 0);
-  unsigned* sc = scal.as<unsigned>();
-  if (voxels) {
-    BatchGeom G = batch_geom(R, kernelRadius, nvox);
-    const int cap = (2 * G.rz + 1) * (2 * G.ry + 1) * (2 * G.rx + 1);
-    const int wcap = cap <= 27 ? 27 : cap <= 125 ? 125 : 343;
-    if (cap > 343) return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
-    H->batch = true; H->nvox = nvox; H->wcap = wcap;
-    RB_CUDA(H->zones.alloc(sizeof(int) * 2 * (size_t)wcap * nvox));
-    RB_CUDA(H->nz.alloc(sizeof(int) * (size_t)nvox));
-    const int grid = (nvox + 127) / 128;
-    const int* vox = (const int*)R.vox.p;
-#define RB_Z(T, W) batch_glszm_zones_kernel<T, W><<<grid, 128>>>((const T*)R.lev, G, vox, R.A, H->zones.as<int>(), H->nz.as<int>(), sc + 1)
-    if (R.lb == 1) { if (wcap == 27) RB_Z(uint8_t, 27); else if (wcap == 125) RB_Z(uint8_t, 125); else RB_Z(uint8_t, 343); }
-    else { if (wcap == 27) RB_Z(uint16_t, 27); else if (wcap == 125) RB_Z(uint16_t, 125); else RB_Z(uint16_t, 343); }
+  H->batch = true; H->nvox = nvox; H->wcap = wcap;
+  RB_CUDA(H->zones.alloc(sizeof(int) * 2 * (size_t)wcap * nvox));
+  RB_CUDA(H->nz.alloc(sizeof(int) * (size_t)nvox));
+  DevBuf mx;
+  RB_CUDA(mx.alloc(4));
+  RB_CUDA(cudaMemsetAsync(mx.p, 0, 4, 0));
+  const int grid = (nvox + 127) / 128;
+  const int* vox = R.vox.as<const int>();
+#define RB_Z(T, W) batch_glszm_zones_kernel<T, W><<<grid, 128>>>(R.lev.as<const T>(), G, vox, R.G.A, H->zones.as<int>(), H->nz.as<int>(), mx.as<unsigned>())
+  if (R.lb == 1) { if (wcap == 27) RB_Z(uint8_t, 27); else if (wcap == 125) RB_Z(uint8_t, 125); else RB_Z(uint8_t, 343); }
+  else { if (wcap == 27) RB_Z(uint16_t, 27); else if (wcap == 125) RB_Z(uint16_t, 125); else RB_Z(uint16_t, 343); }
 #undef RB_Z
-  } else {
-    H->batch = false; H->nvox = 1; H->wcap = 0;
-    Vol V{R.Z, R.Y, R.X};
-    const int grid = grid_for(R.n, 256, 8);
-    DevBuf L, sz;
-    RB_CUDA(L.alloc(R.n * 4));
-    RB_CUDA(sz.alloc(R.n * 4));
-    cudaMemsetAsync(sz.p, 0, R.n * 4, 0);
-    // the unidirectional half of the distance-1 neighbourhood = first half of the bidirectional set
-    AngleSet half = R.A;
-    half.na = R.A.na / 2;
-    if (R.lb == 1) {
-      ccl_init_kernel<uint8_t><<<grid, 256>>>((const uint8_t*)R.lev, R.n, L.as<int>());
-      ccl_merge_kernel<uint8_t><<<grid, 256>>>((const uint8_t*)R.lev, V, half, L.as<int>());
-    } else {
-      ccl_init_kernel<uint16_t><<<grid, 256>>>((const uint16_t*)R.lev, R.n, L.as<int>());
-      ccl_merge_kernel<uint16_t><<<grid, 256>>>((const uint16_t*)R.lev, V, half, L.as<int>());
-    }
-    ccl_count_kernel<<<grid, 256>>>(L.as<int>(), R.n, sz.as<unsigned>());
-    RB_CUDA(H->zones.alloc(sizeof(int) * 2 * (size_t)R.n));
-    if (R.lb == 1) ccl_zones_kernel<uint8_t><<<grid, 256>>>((const uint8_t*)R.lev, L.as<int>(), sz.as<unsigned>(), R.n, H->zones.as<int>(), sc, sc + 1);
-    else ccl_zones_kernel<uint16_t><<<grid, 256>>>((const uint16_t*)R.lev, L.as<int>(), sz.as<unsigned>(), R.n, H->zones.as<int>(), sc, sc + 1);
-    cudaError_t e = cudaStreamSynchronize(0);
-    if (e != cudaSuccess) return fail(RB_ERR_CUDA, "GLSZM labelling: %s", cudaGetErrorString(e));
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(RB_ERR_CUDA, "GLSZM kernels: %s", cudaGetErrorString(e));
-  unsigned host_sc[2] = {0, 0};
-  e = cudaMemcpy(host_sc, sc, 8, cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return fail(RB_ERR_CUDA, "GLSZM: %s", cudaGetErrorString(e));
-  H->nzones = host_sc[0];
-  *max_region_out = (int)host_sc[1];
+  RB_LAUNCH_CHECK();
+  unsigned max_region = 0;
+  RB_CUDA(cudaMemcpy(&max_region, mx.p, 4, cudaMemcpyDeviceToHost));
+  *max_region_out = (int)max_region;
   *handle_out = H.release();
   return RB_OK;
 }
 
-// consumes the handle on every path
-int glszm_fill_host(void* handle, int Ng, int max_region, double* out_host) {
+// phase two on the handle's stream; consumes the handle on every path
+int glszm_fill(void* handle, int Ng, int max_region, double* out_host) {
   std::unique_ptr<GlszmHandle> H((GlszmHandle*)handle);
   if (!H) return fail(RB_ERR_ARG, "null GLSZM handle");
   if (max_region < 1) max_region = 1;
+  const cudaStream_t st = H->st;
   const size_t per = (size_t)Ng * max_region, tot = per * H->nvox;
-  DevBuf dout, status;
+  DevBuf dout, status, hist;
   RB_CUDA(dout.alloc(tot * 8));
   RB_CUDA(status.alloc(4));
-  cudaMemsetAsync(dout.p, 0, tot * 8, 0);
-  cudaMemsetAsync(status.p, 0, 4, 0);
+  RB_CUDA(cudaMemsetAsync(dout.p, 0, tot * 8, st));
+  RB_CUDA(cudaMemsetAsync(status.p, 0, 4, st));
   if (H->batch) {
-    batch_glszm_fill_kernel<<<(H->nvox + 127) / 128, 128>>>(H->zones.as<const int>(), H->nz.as<const int>(), H->nvox, H->wcap, Ng, max_region, dout.as<double>(), status.as<int>());
+    batch_glszm_fill_kernel<<<(H->nvox + 127) / 128, 128, 0, st>>>(H->zones.as<const int>(), H->nz.as<const int>(), H->nvox,
+                                                                  H->wcap, Ng, max_region, dout.as<double>(), status.as<int>());
   } else {
-    DevBuf hist;
     RB_CUDA(hist.alloc(per * 4));
-    cudaMemsetAsync(hist.p, 0, per * 4, 0);
-    if (H->nzones) zones_fill_kernel<<<grid_for(H->nzones, 256, 8), 256>>>(H->zones.as<const int>(), H->nzones, Ng, max_region, hist.as<unsigned>(), status.as<int>());
-    u32_to_f64_kernel<<<grid_for((long long)per, 256, 8), 256>>>(hist.as<unsigned>(), (long long)per, dout.as<double>());
-    cudaStreamSynchronize(0);
+    RB_CUDA(cudaMemsetAsync(hist.p, 0, per * 4, st));
+    if (H->nzones) zones_fill_kernel<<<grid_for(H->nzones, 256, 8), 256, 0, st>>>(H->zones.as<const int>(), H->nzones, Ng, max_region, hist.as<unsigned>(), status.as<int>());
+    u32_to_f64_kernel<<<grid_for((long long)per, 256, 8), 256, 0, st>>>(hist.as<unsigned>(), (long long)per, dout.as<double>());
   }
-  int st = 0;
-  cudaError_t e = cudaMemcpy(&st, status.p, 4, cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return fail(RB_ERR_CUDA, "GLSZM fill: %s", cudaGetErrorString(e));
-  if (st) return fail(RB_ERR_LEVEL_RANGE, "Error filling GLSZM.");
-  if (cudaMemcpy(out_host, dout.p, tot * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return fail(RB_ERR_CUDA, "GLSZM copy back failed");
+  RB_LAUNCH_CHECK();
+  int stv = 0;
+  RB_CUDA(cudaMemcpyAsync(&stv, status.p, 4, cudaMemcpyDeviceToHost, st));
+  RB_CUDA(cudaStreamSynchronize(st));
+  if (stv) return fail(RB_ERR_LEVEL_RANGE, "Error filling GLSZM.");
+  RB_CUDA(cudaMemcpyAsync(out_host, dout.p, tot * 8, cudaMemcpyDeviceToHost, st));
+  RB_CUDA(cudaStreamSynchronize(st));
   return RB_OK;
 }
-
-void glszm_release(void* handle) { delete (GlszmHandle*)handle; }
 
 }  // namespace rb

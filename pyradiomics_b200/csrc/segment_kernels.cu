@@ -17,8 +17,12 @@
 //                          reference's "angle without a line of two voxels loses its length-1 column" rule
 //                          (cmatrices.c:524-534) comes from a pigeonhole count: some line holds two masked voxels <=>
 //                          #masked voxels > #lines that hold any.
+//   segment_glszm          GLSZM's zones (cmatrices.c:94-279): union-find connected-component labelling (26 / 8
+//                          neighbours of equal level) -> zone sizes -> one (gray, size) pair per zone.
 // Integer counts are exact; NGTDM's s_i is accumulated as integers T[g][count] += |g*count - sum| and divided by count
 // once at the end, so both kernels give bit-identical matrices.
+//
+// Every builder starts from segment_geometry and runs all its launches and copies on the caller's stream.
 #include <cuda.h>
 
 #include <vector>
@@ -32,6 +36,7 @@ namespace rb {
 struct SegAngles {
   int na;                 // unidirectional offsets (GLCM); GLDM / NGTDM use +- each of them
   int8_t a[NW_MAX][3];
+  explicit SegAngles(const AngleSet& A) : na(A.na) { memcpy(a, A.a, sizeof(a[0]) * na); }
 };
 struct SegVol {
   int Z, Y, X;
@@ -282,6 +287,71 @@ seg_glrlm_ends_kernel(const T* __restrict__ lev, SegVol V, const __grid_constant
   if (threadIdx.x == 0 && s_masked) atomicAdd(&counts[0], (unsigned long long)s_masked);
 }
 
+// ---- GLSZM: union-find connected components over equal-level 26/8-neighbours -----------------------------------------
+struct Vol {
+  int Z, Y, X;
+  __host__ __device__ long long n() const { return (long long)Z * Y * X; }
+  __device__ bool in(int z, int y, int x) const { return z >= 0 && z < Z && y >= 0 && y < Y && x >= 0 && x < X; }
+  __device__ long long idx(int z, int y, int x) const { return ((long long)z * Y + y) * X + x; }
+};
+
+__device__ __forceinline__ int uf_find(int* L, int i) {
+  int p = L[i];
+  while (p != i) { i = p; p = L[i]; }
+  return i;
+}
+__device__ __forceinline__ void uf_union(int* L, int a, int b) {
+  while (true) {
+    a = uf_find(L, a); b = uf_find(L, b);
+    if (a == b) return;
+    if (a < b) { const int t = a; a = b; b = t; }
+    const int old = atomicMin(&L[a], b);
+    if (old == a) return;
+    a = old;
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) ccl_init_kernel(const T* __restrict__ lev, long long n, int* __restrict__ L) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    L[i] = lev[i] ? (int)i : -1;
+}
+template <typename T>
+__global__ void __launch_bounds__(256)
+ccl_merge_kernel(const T* __restrict__ lev, Vol V, const __grid_constant__ AngleSet A, int* __restrict__ L) {
+  const long long n = V.n(), plane = (long long)V.Y * V.X;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x) {
+    const int g = lev[t];
+    if (!g) continue;
+    const int z = (int)(t / plane), rem = (int)(t % plane), y = rem / V.X, x = rem % V.X;
+    for (int a = 0; a < A.na; a++) {       // unidirectional half of the neighbourhood is enough
+      const int z2 = z + A.a[a][0], y2 = y + A.a[a][1], x2 = x + A.a[a][2];
+      if (!V.in(z2, y2, x2)) continue;
+      const long long j = V.idx(z2, y2, x2);
+      if (lev[j] == g) uf_union(L, (int)t, (int)j);
+    }
+  }
+}
+__global__ void __launch_bounds__(256) ccl_count_kernel(int* __restrict__ L, long long n, unsigned* __restrict__ size) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (L[i] < 0) continue;
+    const int r = uf_find(L, (int)i);
+    atomicAdd(&size[r], 1u);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(256)
+ccl_zones_kernel(const T* __restrict__ lev, const int* __restrict__ L, const unsigned* __restrict__ size, long long n,
+                 int* __restrict__ zones, unsigned* __restrict__ nzones, unsigned* __restrict__ max_region) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (L[i] != (int)i) continue;            // roots only
+    const unsigned k = atomicAdd(nzones, 1u);
+    zones[2 * (size_t)k] = lev[i];
+    zones[2 * (size_t)k + 1] = (int)size[i];
+    atomicMax(max_region, size[i]);
+  }
+}
+
 // counts -> float64 with the multi-voxel-line rule (cmatrices.c:524-534) from the pigeonhole counts
 __global__ void glrlm_to_f64_kernel(const unsigned* __restrict__ hist, long long n, double* __restrict__ out,
                                     const unsigned long long* __restrict__ counts, int Nr, int na) {
@@ -303,6 +373,28 @@ __global__ void ngtdm_seg_finish_kernel(const unsigned long long* __restrict__ a
   out[g * 3 + 0] = (double)acc[g * ncol];
   out[g * 3 + 1] = s;
   out[g * 3 + 2] = (double)(g + 1);
+}
+
+int segment_geometry(const int* size, int nd, const int* distances, int ndist, bool bidirectional, int force2D,
+                     int force2Ddimension, int Ng, int na_max, int* angles_out, SegmentGeometry& G) {
+  G.Z = nd == 3 ? size[0] : 1; G.Y = size[nd - 2]; G.X = size[nd - 1];
+  G.n = (long long)G.Z * G.Y * G.X;
+  if (Ng < 1 || Ng > 65535) return fail(RB_ERR_UNSUPPORTED, "Ng=%d outside 1..65535", Ng);
+  if (G.n <= 0 || G.n >= (1ll << 31)) return fail(RB_ERR_UNSUPPORTED, "volume must have 1..2^31-1 voxels");
+  std::vector<int> ang;
+  const int na = generate_angles(size, nd, distances, ndist, bidirectional, force2D ? force2Ddimension : -1, ang);
+  if (na <= 0) return fail(RB_ERR_ARG, "Error getting angle count.");
+  if (na > na_max) return fail(RB_ERR_UNSUPPORTED, "more than %d angles", NA_MAX);
+  G.A.na = na;
+  G.H = 0;
+  for (int a = 0; a < na; a++)
+    for (int d = 0; d < 3; d++) {
+      const int v = d < 3 - nd ? 0 : ang[a * nd + d - (3 - nd)];
+      G.A.a[a][d] = (int8_t)v;
+      G.H = v > G.H ? v : (-v > G.H ? -v : G.H);
+    }
+  if (angles_out) memcpy(angles_out, ang.data(), sizeof(int) * ang.size());
+  return RB_OK;
 }
 
 // B200_SEG_TMA=0 forces the cooperative-load staging (A/B runs, tests); default: TMA whenever a tensor map can be built
@@ -327,9 +419,7 @@ static size_t tile_plan(int Z, int Y, int X, int H, int Ng, int na, int flags, S
 
 static int launch_tile(const uint8_t* lev, SegVol V, const AngleSet& A, const SegTileGeom& G, size_t smem, int Ng, int alpha,
                        int flags, unsigned* d_gl, unsigned* d_gd, unsigned long long* d_ng, cudaStream_t st) {
-  SegAngles S;
-  S.na = A.na;
-  memcpy(S.a, A.a, sizeof(S.a[0]) * A.na);
+  const SegAngles S(A);
   // tensor map: needs a 16-byte aligned base and row / plane pitches that are multiples of 16 bytes
   CUtensorMap tmap;
   memset(&tmap, 0, sizeof tmap);
@@ -377,7 +467,6 @@ template <typename T>
 static int launch_direct(const T* lev, SegVol V, const AngleSet& A, int Ng, int alpha, int flags, unsigned* d_gl,
                          unsigned* d_gd, unsigned long long* d_ng, cudaStream_t st) {
   const long long n = (long long)V.Z * V.Y * V.X;
-  if (n <= 0 || n >= (1ll << 31)) return fail(RB_ERR_UNSUPPORTED, "volume must have 1..2^31-1 voxels");
   const size_t sh = (size_t)Ng * Ng * A.na * 4;
   const int glcm_shared = (flags & 1) && sh <= 160 * 1024;
   if (glcm_shared) RB_CUDA(cudaFuncSetAttribute(seg_direct_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
@@ -389,30 +478,18 @@ static int launch_direct(const T* lev, SegVol V, const AngleSet& A, int Ng, int 
 
 // GLCM / GLDM / NGTDM of one packed level volume (uint8 or uint16) in one pass; outputs are HOST float64 buffers in the
 // reference layouts (NULL = not wanted), angles_out gets the unidirectional offsets.  3-D volumes or 2-D (Z = 1).
-int segment_matrices(const void* lev, int level_bytes, int nd, int Z, int Y, int X, const int* distances, int ndist, int Ng,
+int segment_matrices(const void* lev, int level_bytes, const int* size, int nd, const int* distances, int ndist, int Ng,
                      int alpha, int force2D, int force2Ddimension, double* glcm_host, double* gldm_host, double* ngtdm_host,
                      int* angles_out, cudaStream_t st) {
-  int size[3] = {Z, Y, X};
-  const int* sz = nd == 3 ? size : size + 1;
-  std::vector<int> ang;
-  const int na = generate_angles(sz, nd, distances, ndist, false, force2D ? force2Ddimension : -1, ang);
-  if (na <= 0) return fail(RB_ERR_ARG, "Error getting angle count.");
-  if (Ng < 1 || Ng > 65535) return fail(RB_ERR_UNSUPPORTED, "Ng=%d outside 1..65535", Ng);
+  SegmentGeometry sg;
   // GLCM counts the na offsets, GLDM / NGTDM each offset and its mirror
-  const int na_max = (gldm_host || ngtdm_host) ? NA_MAX / 2 : NA_MAX;
-  if (na > na_max) return fail(RB_ERR_UNSUPPORTED, "more than %d angles", NA_MAX);
-  if (angles_out) memcpy(angles_out, ang.data(), sizeof(int) * ang.size());
+  int rc = segment_geometry(size, nd, distances, ndist, false, force2D, force2Ddimension, Ng,
+                            (gldm_host || ngtdm_host) ? NA_MAX / 2 : NA_MAX, angles_out, sg);
+  if (rc) return rc;
   const int flags = (glcm_host ? 1 : 0) | (gldm_host ? 2 : 0) | (ngtdm_host ? 4 : 0);
   if (!flags) return RB_OK;
-  AngleSet A;
-  A.na = na;
-  int H = 0;
-  for (int a = 0; a < na; a++)
-    for (int d = 0; d < 3; d++) {
-      const int v = d < 3 - nd ? 0 : ang[a * nd + d - (3 - nd)];
-      A.a[a][d] = (int8_t)v;
-      H = v > H ? v : (-v > H ? -v : H);
-    }
+  const AngleSet& A = sg.A;
+  const int na = A.na;
   const size_t n_gl = (size_t)Ng * Ng * na, n_gd = (size_t)Ng * (2 * (2 * na) + 1), n_ng = (size_t)Ng * (2 * na + 2);
   DevBuf gl, gd, ng, out;
   if (flags & 1) { RB_CUDA(gl.alloc(n_gl * 4)); RB_CUDA(cudaMemsetAsync(gl.p, 0, n_gl * 4, st)); }
@@ -425,12 +502,12 @@ int segment_matrices(const void* lev, int level_bytes, int nd, int Z, int Y, int
   RB_CUDA(out.alloc(n_out * 8));
   unsigned *d_gl = gl.as<unsigned>(), *d_gd = gd.as<unsigned>();
   unsigned long long* d_ng = ng.as<unsigned long long>();
-  const SegVol V{Z, Y, X, (long long)X, (long long)Y * X};
+  const SegVol V{sg.Z, sg.Y, sg.X, (long long)sg.X, (long long)sg.Y * sg.X};
   SegTileGeom G;
-  const size_t smem = level_bytes == 1 && H <= 3 && na <= NW_MAX ? tile_plan(Z, Y, X, H, Ng, na, flags, G) : 0;
-  const int rc = smem ? launch_tile((const uint8_t*)lev, V, A, G, smem, Ng, alpha, flags, d_gl, d_gd, d_ng, st)
-                 : level_bytes == 1 ? launch_direct((const uint8_t*)lev, V, A, Ng, alpha, flags, d_gl, d_gd, d_ng, st)
-                                    : launch_direct((const uint16_t*)lev, V, A, Ng, alpha, flags, d_gl, d_gd, d_ng, st);
+  const size_t smem = level_bytes == 1 && sg.H <= 3 && na <= NW_MAX ? tile_plan(sg.Z, sg.Y, sg.X, sg.H, Ng, na, flags, G) : 0;
+  rc = smem ? launch_tile((const uint8_t*)lev, V, A, G, smem, Ng, alpha, flags, d_gl, d_gd, d_ng, st)
+       : level_bytes == 1 ? launch_direct((const uint8_t*)lev, V, A, Ng, alpha, flags, d_gl, d_gd, d_ng, st)
+                          : launch_direct((const uint16_t*)lev, V, A, Ng, alpha, flags, d_gl, d_gd, d_ng, st);
   if (rc) return rc;
   const int cg = sm_count() * 4;
   double* d_out = out.as<double>();
@@ -453,23 +530,15 @@ int segment_matrices(const void* lev, int level_bytes, int nd, int Z, int Y, int
 }
 
 // GLRLM of one packed level volume (uint8 or uint16) -> HOST float64 [Ng][Nr][Na]
-int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X, int Ng, int Nr, int force2D, int force2Ddimension,
+int segment_glrlm(const void* lev, int level_bytes, const int* size, int nd, int Ng, int Nr, int force2D, int force2Ddimension,
                   double* glrlm_host, int* angles_out, cudaStream_t st) {
-  if (Ng < 1 || Ng > 65535) return fail(RB_ERR_UNSUPPORTED, "Ng=%d outside 1..65535", Ng);
-  const long long n = (long long)Z * Y * X;
-  if (n <= 0 || n >= (1ll << 31)) return fail(RB_ERR_UNSUPPORTED, "volume must have 1..2^31-1 voxels");
-  int size[3] = {Z, Y, X};
-  const int* sz = nd == 3 ? size : size + 1;
-  std::vector<int> ang;
+  SegmentGeometry sg;
   const int one[1] = {1};
-  const int na = generate_angles(sz, nd, one, 1, false, force2D ? force2Ddimension : -1, ang);
-  if (na <= 0) return fail(RB_ERR_ARG, "Error getting angle count.");
+  const int rc = segment_geometry(size, nd, one, 1, false, force2D, force2Ddimension, Ng, NW_MAX, angles_out, sg);
+  if (rc) return rc;
   if (Nr < 1) return fail(RB_ERR_ARG, "Nr must be >= 1");
-  SegAngles A;
-  A.na = na;
-  for (int a = 0; a < na; a++)
-    for (int d = 0; d < 3; d++) A.a[a][d] = d < 3 - nd ? 0 : (int8_t)ang[a * nd + d - (3 - nd)];
-  if (angles_out) memcpy(angles_out, ang.data(), sizeof(int) * ang.size());
+  const SegAngles A(sg.A);
+  const int na = A.na;
   const size_t per = (size_t)Ng * Nr * na;
   DevBuf h, c, status, out;
   RB_CUDA(h.alloc(per * 4));
@@ -482,8 +551,8 @@ int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X,
   unsigned* d_h = h.as<unsigned>();
   unsigned long long* d_c = c.as<unsigned long long>();
   int* d_st = status.as<int>();
-  const SegVol V{Z, Y, X, (long long)X, (long long)Y * X};
-  const int grid = grid_for(n, 256, 8);
+  const SegVol V{sg.Z, sg.Y, sg.X, (long long)sg.X, (long long)sg.Y * sg.X};
+  const int grid = grid_for(sg.n, 256, 8);
   const size_t sh = (size_t)Ng * RL_SH * na * 4 <= 96 * 1024 ? (size_t)Ng * RL_SH * na * 4 : 0;
   if (level_bytes == 1) {
     RB_CUDA(cudaFuncSetAttribute(seg_glrlm_ends_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
@@ -500,6 +569,50 @@ int segment_glrlm(const void* lev, int level_bytes, int nd, int Z, int Y, int X,
   RB_CUDA(cudaMemcpyAsync(glrlm_host, out.p, per * 8, cudaMemcpyDeviceToHost, st));
   RB_CUDA(cudaStreamSynchronize(st));
   if (stv & 1) return fail(RB_ERR_LEVEL_RANGE, "Calculation of GLRLM Failed: run longer than Nr");
+  return RB_OK;
+}
+
+// GLSZM phase one of a packed level volume (uint8 or uint16) into a new handle on `st` (one (gray, size) pair per zone;
+// *max_region = the largest zone); rb_fill_glszm finishes it.
+int segment_glszm(const void* lev, int level_bytes, const int* size, int nd, int Ng, int force2D, int force2Ddimension,
+                  int* max_region, void** handle, cudaStream_t st) {
+  SegmentGeometry sg;
+  const int one[1] = {1};
+  // the unidirectional distance-1 offsets: union-find joins each neighbour pair once
+  const int rc = segment_geometry(size, nd, one, 1, false, force2D, force2Ddimension, Ng, NA_MAX, nullptr, sg);
+  if (rc) return rc;
+  std::unique_ptr<GlszmHandle> H(new GlszmHandle);   // handed to the caller only on success
+  H->st = st;
+  const long long n = sg.n;
+  const Vol V{sg.Z, sg.Y, sg.X};
+  const int grid = grid_for(n, 256, 8);
+  DevBuf L, sz, scal;   // scal: [0] zones, [1] largest zone
+  RB_CUDA(L.alloc(n * 4));
+  RB_CUDA(sz.alloc(n * 4));
+  RB_CUDA(scal.alloc(8));
+  RB_CUDA(H->zones.alloc(sizeof(int) * 2 * (size_t)n));
+  RB_CUDA(cudaMemsetAsync(sz.p, 0, n * 4, st));
+  RB_CUDA(cudaMemsetAsync(scal.p, 0, 8, st));
+  unsigned *d_sz = sz.as<unsigned>(), *sc = scal.as<unsigned>();
+  int* zones = H->zones.as<int>();
+  if (level_bytes == 1) {
+    ccl_init_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)lev, n, L.as<int>());
+    ccl_merge_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)lev, V, sg.A, L.as<int>());
+    ccl_count_kernel<<<grid, 256, 0, st>>>(L.as<int>(), n, d_sz);
+    ccl_zones_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)lev, L.as<int>(), d_sz, n, zones, sc, sc + 1);
+  } else {
+    ccl_init_kernel<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)lev, n, L.as<int>());
+    ccl_merge_kernel<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)lev, V, sg.A, L.as<int>());
+    ccl_count_kernel<<<grid, 256, 0, st>>>(L.as<int>(), n, d_sz);
+    ccl_zones_kernel<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)lev, L.as<int>(), d_sz, n, zones, sc, sc + 1);
+  }
+  RB_LAUNCH_CHECK();
+  unsigned host_sc[2] = {0, 0};
+  RB_CUDA(cudaMemcpyAsync(host_sc, sc, 8, cudaMemcpyDeviceToHost, st));
+  RB_CUDA(cudaStreamSynchronize(st));
+  H->nzones = host_sc[0];
+  *max_region = (int)host_sc[1];
+  *handle = H.release();
   return RB_OK;
 }
 

@@ -110,8 +110,8 @@ CASES = {
 
 
 # ---------------------------------------------------------------------------------------------------- launch geometry
-# The dispatch of segment_kernels.cu (segment_matrices, tile_plan, launch_tile, launch_direct, segment_glrlm) and of the
-# GLSZM labelling in matrix_kernels.cu (glszm_zones_host), restated: which kernel builds a matrix and with how many blocks.
+# The dispatch of segment_kernels.cu (segment_matrices, tile_plan, launch_tile, launch_direct, segment_glrlm, and the
+# GLSZM labelling in segment_glszm), restated: which kernel builds a matrix and with how many blocks.
 # (torch.profiler does record these kernels, but over the many sessions of one test process it lost kernel records of
 # some sessions on an H100, so the launches are computed from the same rules instead of read back.)
 def _sms():
