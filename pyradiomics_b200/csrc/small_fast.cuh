@@ -3,7 +3,7 @@
 // ngtdm_voxel (vox_features.cuh, the generic fallback and cross-check), built on the 27 x 27-bit
 // equality masks of the window like the GLCM / GLRLM fast paths:
 //   GLDM  dependence of a voxel = popcount(close-level mask & static neighbour mask); merged
-//         (level, dependence) counts = popcount(equal-level mask & equal-dependence mask)
+//         (level, dependence) counts = popcount(equal-(level, dependence) mask)
 //   NGTDM a full-window body in exact integers and a general one; Busyness from one sort, Contrast and
 //         Strength in closed forms of integer moments, only Complexity keeps a pairwise level loop
 //   GLSZM zones of one level = flood fill of its equality mask by separable bitmask dilation
@@ -18,6 +18,7 @@ struct SmallFastTables {
   double inv2[256];     // 1 / g^2
   double invsq[32];     // 1 / j^2, j = 1..28
   double rcp[64];       // 1 / c
+  double dclog2[32];    // (c + 1) log2(c + 1) - c log2(c): what one more zone adds to a (level, size) group of c
 };
 
 inline void small_fast_build_tables(SmallFastTables& T) {
@@ -25,6 +26,7 @@ inline void small_fast_build_tables(SmallFastTables& T) {
   for (int c = 1; c < 32; c++) { T.log2t[c] = log2((double)c); T.invsq[c] = 1.0 / ((double)c * c); }
   for (int g = 1; g < 256; g++) T.inv2[g] = 1.0 / ((double)g * g);
   for (int c = 1; c < 64; c++) T.rcp[c] = 1.0 / (double)c;
+  for (int c = 0; c < 32; c++) T.dclog2[c] = (c + 1) * log2((double)(c + 1)) - (c ? c * log2((double)c) : 0.0);
 }
 
 // 26-neighbourhood of window position v inside the 3x3x3 window (compile-time constant per v)
@@ -48,14 +50,23 @@ template <int V, int END> struct ForPos {
 template <int END> struct ForPos<END, END> { template <typename F> static RB_HD void go(F&) {} };
 
 // ---------------------------------------------------------------------------------------- GLDM
+// Two bodies, chosen by the window alone: FULL (all 27 levels non-zero) has no unmasked positions, so Nz = 27 and the
+// reciprocals are constants.  The dependence counts n_j come from a packed histogram (DependenceNonUniformity =
+// sum_j n_j^2), the merged (level, dependence) counts from the equality masks of the keys g << 5 | dependence; once
+// those keys are formed the levels and the level masks are dead, which keeps the kernel within 128 registers.
 struct GldmPass1 {
-  const int* wl; const uint32_t* cl; int* dep; uint32_t M;
-  template <int V> RB_HD void at() { dep[V] = wl[V] ? (int)RB_POPC(cl[V] & NB26<V>::value) : -1 - V; }
+  const uint32_t* cl; int* dep;
+  template <int V> RB_HD void at() { dep[V] = (int)RB_POPC(cl[V] & NB26<V>::value); }
 };
 
-RB_HD void gldm_fast_voxel(const int* wl, int alpha, const SmallFastTables& T, double* out) {
+template <bool FULL>
+RB_HD void gldm_fast_body(const int* wl, int alpha, const SmallFastTables& T, double* out) {
   uint32_t eq[27];
-  RB_EQMASKS_27(wl, eq);
+  if (FULL) RB_EQMASKS_27_KEY(wl, eq);
+  else RB_EQMASKS_27(wl, eq);
+  int gl = 0;
+#pragma unroll
+  for (int v = 0; v < 27; v++) gl += RB_POPC(eq[v]);
   uint32_t cl[27];
   if (alpha == 0) {
 #pragma unroll
@@ -69,29 +80,43 @@ RB_HD void gldm_fast_voxel(const int* wl, int alpha, const SmallFastTables& T, d
 #pragma unroll
       for (int q = p + 1; q < 27; q++) {
         const int d = wl[p] - wl[q];
-        if (wl[p] && wl[q] && d <= alpha && -d <= alpha) { cl[p] |= 1u << q; cl[q] |= 1u << p; }
+        if ((FULL || (wl[p] && wl[q])) && d <= alpha && -d <= alpha) { cl[p] |= 1u << q; cl[q] |= 1u << p; }
       }
   }
   int dep[27];
-  GldmPass1 p1{wl, cl, dep, 0};
+  GldmPass1 p1{cl, dep};
   ForPos<0, 27>::go(p1);
-  // equal-dependence masks (unmasked positions carry distinct negative sentinels)
-  uint32_t dq[27];
-  RB_EQMASKS_27_KEY(dep, dq);
-  int Nz = 0, Sj = 0, Sj2 = 0, B = 0, C = 0, X4 = 0, gl = 0, dn = 0;
+  int Nz = 0, Sj = 0, Sj2 = 0, B = 0, C = 0, X4 = 0;
   double Sinv = 0, A = 0, X1 = 0, X2 = 0, X3 = 0, lg = 0;
+  unsigned long long h0 = 0, h1 = 0, h2 = 0;   // dependence histogram, 5-bit fields: 0..11 | 12..23 | 24..26
+  int key[27];                         // g << 5 | dependence; unmasked positions: distinct negative sentinels
 #pragma unroll
   for (int v = 0; v < 27; v++) {
-    if (wl[v]) {
-      const int g = wl[v], g2 = g * g, j = dep[v] + 1, j2 = j * j;
+    const bool in = FULL || wl[v];
+    const int g = wl[v], g2 = g * g, j = dep[v] + 1, j2 = j * j;
+    key[v] = in ? g << 5 | dep[v] : -1 - v;
+    if (in) {
       const double ig = T.inv2[g], ij = T.invsq[j];
       Nz++; Sj += j; Sj2 += j2; B += g2; C += g; X4 += g2 * j2;
       Sinv += ij; A += ig; X1 += ig * ij; X2 += g2 * ij; X3 += j2 * ig;
-      gl += RB_POPC(eq[v]); dn += RB_POPC(dq[v]);
-      lg += T.log2t[RB_POPC(eq[v] & dq[v])];
+      if (dep[v] < 12) h0 += 1ull << (5 * dep[v]);
+      else if (dep[v] < 24) h1 += 1ull << (5 * (dep[v] - 12));
+      else h2 += 1ull << (5 * (dep[v] - 24));
     }
   }
-  const double inv = 1.0 / Nz, inv2 = inv * inv;
+  int dn = 0;                          // sum_j n_j^2
+#pragma unroll
+  for (int k = 0; k < 12; k++) { const int c = (int)(h0 >> (5 * k)) & 31; dn += c * c; }
+#pragma unroll
+  for (int k = 0; k < 12; k++) { const int c = (int)(h1 >> (5 * k)) & 31; dn += c * c; }
+#pragma unroll
+  for (int k = 0; k < 3; k++) { const int c = (int)(h2 >> (5 * k)) & 31; dn += c * c; }
+  uint32_t kq[27];
+  RB_EQMASKS_27_KEY(key, kq);
+#pragma unroll
+  for (int v = 0; v < 27; v++)
+    if (FULL || key[v] >= 0) lg += T.log2t[RB_POPC(kq[v])];
+  const double inv = FULL ? 1.0 / 27 : 1.0 / Nz, inv2 = inv * inv;
   out[0] = T.log2t[Nz] - lg * inv;                 // DependenceEntropy
   out[1] = dn * inv;                               // DependenceNonUniformity
   out[2] = dn * inv2;                              // DependenceNonUniformityNormalized
@@ -261,7 +286,7 @@ RB_HD void ngtdm_fast_body(const int* wl, const SmallFastTables& T, double* out,
 }
 
 // a window is full when all 27 levels are non-zero
-RB_HD bool ngtdm_window_full(const int* wl) {
+RB_HD bool window27_full(const int* wl) {
   bool full = true;
 #pragma unroll
   for (int v = 0; v < 27; v++) full &= wl[v] != 0;
@@ -272,7 +297,7 @@ RB_HD bool ngtdm_window_full(const int* wl) {
 RB_HD void ngtdm_fast_voxel(const int* wl, const SmallFastTables& T, double* out) {
   int pk[27] = {0};
   double ns[27] = {0};
-  if (ngtdm_window_full(wl)) ngtdm_fast_body<true>(wl, T, out, pk, ns, 1);
+  if (window27_full(wl)) ngtdm_fast_body<true>(wl, T, out, pk, ns, 1);
   else ngtdm_fast_body<false>(wl, T, out, pk, ns, 1);
 }
 
@@ -292,23 +317,26 @@ struct GlszmAcc {
   unsigned long long h0, h1, h2;      // zone-size histogram, 5-bit fields: sizes 1..12 | 13..24 | 25..27
 };
 
-RB_HD void glszm_fast_voxel(const int* wl, const SmallFastTables& T, double* out) {
-  // equality masks of the window (as the other fast paths).  A level that occurs ONCE is one zone of size 1: its share
-  // of every sum is added in the static loop below (27 i.i.d. levels out of 32: ~12 such levels); only the levels that
-  // occur at least twice (<= 13 of them, ~7) go through the flood fill.
+// Equality masks of the window as the other fast paths.  A level that occurs ONCE is one zone of size 1: its share of
+// every sum is added in the static loop below (27 i.i.d. levels out of 32: ~12 such levels); only the levels that
+// occur at least twice (<= 13 of them, ~7) go through the flood fill.  Their masks and levels live in per-thread
+// scratch scr (mask | g << 32, 13 entries, element stride st; device: shared memory laid out [entry][thread]).  The
+// merged (level, size) counts come from the histogram's growth inside the level: a zone that joins c earlier zones of
+// its level and size adds (c+1) log2(c+1) - c log2(c) to sum_groups c log2(c).  FULL: wl must be a full window.
+template <bool FULL>
+RB_HD void glszm_fast_body(const int* wl, const SmallFastTables& T, double* out, unsigned long long* scr, int st) {
   uint32_t eq[27];
-  RB_EQMASKS_27(wl, eq);
+  if (FULL) RB_EQMASKS_27_KEY(wl, eq);
+  else RB_EQMASKS_27(wl, eq);
   uint32_t M = 0;
-  uint32_t cls[13];
-  int clg[13];
   int nl = 0, S_n = 0, S_g = 0, S_g2 = 0;
   double S_ig = 0;
 #pragma unroll
   for (int v = 0; v < 27; v++) {
-    if (wl[v]) M |= 1u << v;
+    if (!FULL && wl[v]) M |= 1u << v;
     if (eq[v] && (eq[v] & ((1u << v) - 1)) == 0) {
       if (eq[v] == (1u << v)) { S_n++; S_g += wl[v]; S_g2 += wl[v] * wl[v]; S_ig += T.inv2[wl[v]]; }
-      else { cls[nl] = eq[v]; clg[nl] = wl[v]; nl++; }
+      else { scr[nl * st] = eq[v] | (unsigned long long)wl[v] << 32; nl++; }
     }
   }
   GlszmAcc a;
@@ -316,12 +344,13 @@ RB_HD void glszm_fast_voxel(const int* wl, const SmallFastTables& T, double* out
   a.A = S_ig; a.Sinv = (double)S_n; a.X1 = S_ig; a.X2 = (double)S_g2; a.X3 = S_ig; a.lg = 0;
   a.h0 = (unsigned long long)S_n; a.h1 = a.h2 = 0;
   for (int k = 0; k < nl; k++) {
-    const int g = clg[k], g2 = g * g;
-    uint32_t m = cls[k];
+    const unsigned long long e = scr[k * st];
+    uint32_t m = (uint32_t)e;
+    const int g = (int)(e >> 32), g2 = g * g;
     const double ig = T.inv2[g];
-    int zs[8];                                         // <= 8 mutually non-adjacent zones fit a 3x3x3 window
-    int zc = 0;
-    while (m && zc < 8) {
+    const unsigned long long l0 = a.h0, l1 = a.h1, l2 = a.h2;    // the histogram before this level
+    int zc = 0;                                        // <= 8 mutually non-adjacent zones fit a 3x3x3 window
+    while (m) {
       uint32_t comp = m & (0u - m);
       for (;;) {
         const uint32_t nx = dilate26(comp) & m;
@@ -330,21 +359,17 @@ RB_HD void glszm_fast_voxel(const int* wl, const SmallFastTables& T, double* out
       }
       m &= ~comp;
       const int sz = RB_POPC(comp), s2 = sz * sz;
-      zs[zc++] = sz;
+      zc++;
       const double is = T.invsq[sz];
       a.Nz++; a.Sg += g; a.Sg2 += g2; a.Ss2 += s2; a.X4 += g2 * s2;
       a.A += ig; a.Sinv += is; a.X1 += ig * is; a.X2 += g2 * is; a.X3 += s2 * ig;
-      if (sz <= 12) a.h0 += 1ull << (5 * (sz - 1));
-      else if (sz <= 24) a.h1 += 1ull << (5 * (sz - 13));
-      else a.h2 += 1ull << (5 * (sz - 25));
+      int c;                                           // earlier zones of this level and size
+      if (sz <= 12) { c = (int)((a.h0 - l0) >> (5 * (sz - 1))) & 31; a.h0 += 1ull << (5 * (sz - 1)); }
+      else if (sz <= 24) { c = (int)((a.h1 - l1) >> (5 * (sz - 13))) & 31; a.h1 += 1ull << (5 * (sz - 13)); }
+      else { c = (int)((a.h2 - l2) >> (5 * (sz - 25))) & 31; a.h2 += 1ull << (5 * (sz - 25)); }
+      a.lg += T.dclog2[c];
     }
     a.gln += zc * zc;
-    // merged (level, size) counts inside this level: zones of equal size
-    for (int k = 0; k < zc; k++) {
-      int c = 0;
-      for (int l = 0; l < zc; l++) c += zs[l] == zs[k];
-      a.lg += T.log2t[c];
-    }
   }
   int szn = 0;
 #pragma unroll
@@ -354,16 +379,27 @@ RB_HD void glszm_fast_voxel(const int* wl, const SmallFastTables& T, double* out
   }
 #pragma unroll
   for (int k = 0; k < 3; k++) { const int c2 = (int)(a.h2 >> (5 * k)) & 31; szn += c2 * c2; }
-  const int Np = RB_POPC(M), Nz = a.Nz;
-  const double inv = 1.0 / Nz, inv2 = inv * inv;
+  const int Np = FULL ? 27 : RB_POPC(M), Nz = a.Nz;
+  const double inv = FULL ? T.rcp[Nz] : 1.0 / Nz, inv2 = inv * inv;
   out[S_GLN] = a.gln * inv; out[S_GLNN] = a.gln * inv2;
   out[S_GLV] = (double)(Nz * a.Sg2 - a.Sg * a.Sg) * inv2;
   out[S_HGLE] = a.Sg2 * inv; out[S_LargeE] = a.Ss2 * inv; out[S_LargeHGLE] = a.X4 * inv; out[S_LargeLGLE] = a.X3 * inv;
   out[S_LGLE] = a.A * inv; out[S_SizeNU] = szn * inv; out[S_SizeNUN] = szn * inv2; out[S_SmallE] = a.Sinv * inv;
   out[S_SmallHGLE] = a.X2 * inv; out[S_SmallLGLE] = a.X1 * inv;
   out[S_Entropy] = T.log2t[Nz] - a.lg * inv;
-  out[S_Percentage] = (double)Nz / Np;
+  out[S_Percentage] = FULL ? Nz * (1.0 / 27) : (double)Nz / Np;
   out[S_SizeVar] = (double)(Nz * a.Ss2 - Np * Np) * inv2;
+}
+
+// convenience: private scratch, body chosen by the window (host emulation)
+RB_HD void glszm_fast_voxel(const int* wl, const SmallFastTables& T, double* out) {
+  unsigned long long scr[13];
+  if (window27_full(wl)) glszm_fast_body<true>(wl, T, out, scr, 1);
+  else glszm_fast_body<false>(wl, T, out, scr, 1);
+}
+RB_HD void gldm_fast_voxel(const int* wl, int alpha, const SmallFastTables& T, double* out) {
+  if (window27_full(wl)) gldm_fast_body<true>(wl, alpha, T, out);
+  else gldm_fast_body<false>(wl, alpha, T, out);
 }
 
 }  // namespace rb

@@ -142,42 +142,77 @@ int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& 
 }
 
 // ------------------------------------------------------------------ GLSZM / GLDM / NGTDM fast paths
-// SYNC: block-uniform tiles with a barrier per tile, so the block's warps stream the (large,
-// straight-line) GLDM body together and share instruction-cache lines (free-running warps stall
-// on instruction fetch).
-template <int CLS, int NT, bool SYNC>
-__global__ void __launch_bounds__(NT)
-small_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
-                  const __grid_constant__ VoxParams P, const SmallFastTables* __restrict__ Tg,
-                  double* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
+// GLSZM and GLDM over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh), like NGTDM: a centre whose 27
+// window levels are all non-zero runs the class's FULL body in its tile, the other centres are drained through the
+// general body.  GLSZM's level classes live in per-thread shared scratch laid out [entry][thread].
+template <int CLS> struct TileClass;
+template <> struct TileClass<C_GLSZM> { static constexpr int NF = GLSZM_NF, NMG = 13; };
+template <> struct TileClass<C_GLDM> { static constexpr int NF = GLDM_NF, NMG = 0; };
+
+template <int CLS, bool FULL>
+__device__ __forceinline__ void tile_body(const int* wl, const SmallFastTables& T, int alpha, unsigned long long* mg,
+                                          int st, double* f) {
+  if constexpr (CLS == C_GLSZM) glszm_fast_body<FULL>(wl, T, f, mg, st);
+  else gldm_fast_body<FULL>(wl, alpha, T, f);
+}
+
+template <int CLS, int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB)
+tiles_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers, const __grid_constant__ VoxParams P,
+                  const SmallFastTables* __restrict__ Tg, double* __restrict__ out, long long fstride,
+                  int z0, int z1, int out_z0) {
+  using K = TileClass<CLS>;
   __shared__ SmallFastTables T;
+  __shared__ unsigned long long scr_mg[K::NMG * NT + 1];
+  __shared__ long long defer[2 * NT];                              // chunk indices of the centres left to the general body
+  __shared__ unsigned ndefer;
   copy_tables_to_shared<NT>(T, Tg);
+  const int tid = threadIdx.x;
+  if (tid == 0) ndefer = 0;
   __syncthreads();
-  constexpr int NF = CLS == C_GLSZM ? GLSZM_NF : GLDM_NF;
   const long long plane = (long long)P.Y * P.X;
-  const long long total = (long long)(z1 - z0) * plane;
-  const long long ntiles = (total + NT - 1) / NT;
-  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    if (SYNC) __syncthreads();
-    const long long t = tile * NT + threadIdx.x;
-    const bool live = t < total;
-    if (!SYNC && !live) continue;
-    const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t, live);
-    const bool is_center = live && chunk_center(lev, centers, plane, v);
-    if (!SYNC && !is_center) {
+  full_window_tiles<NT>((long long)(z1 - z0) * plane, defer, ndefer,
+    [&](long long t, bool live, auto defer_it) {
+      if (!live) return;
+      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t);
+      const bool is_center = chunk_center(lev, centers, plane, v);
+      int wl[27];
+      const bool full = load_window27(lev, P, v.z, v.y, v.x, v.vi, is_center, wl, 1);
+      if (full) {
+        double f[K::NF];
+        tile_body<CLS, true>(wl, T, P.alpha, scr_mg + tid, NT, f);
 #pragma unroll
-      for (int k = 0; k < NF; k++) out[k * fstride + v.oi] = P.init_value;
-      continue;
-    }
-    int wl[27];
-    load_window27(lev, P, v.z, v.y, v.x, v.vi, is_center, wl, 1);
-    double f[16];
-    if (CLS == C_GLSZM) glszm_fast_voxel(wl, T, f);
-    else gldm_fast_voxel(wl, P.alpha, T, f);
-    if (!live) continue;
+        for (int k = 0; k < K::NF; k++) out[k * fstride + v.oi] = f[k];
+      } else if (is_center) {
+        defer_it();
+      } else {
 #pragma unroll
-    for (int k = 0; k < NF; k++) out[k * fstride + v.oi] = is_center ? f[k] : P.init_value;
-  }
+        for (int k = 0; k < K::NF; k++) out[k * fstride + v.oi] = P.init_value;
+      }
+    },
+    [&](auto entry, bool live) {
+      if (!live) return;
+      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, entry());
+      int wl[27];
+      load_window27(lev, P, v.z, v.y, v.x, v.vi, true, wl, 1);
+      double f[K::NF];
+      tile_body<CLS, false>(wl, T, P.alpha, scr_mg + tid, NT, f);
+#pragma unroll
+      for (int k = 0; k < K::NF; k++) out[k * fstride + v.oi] = f[k];
+    });
+}
+
+// block size and blocks per SM (registers <= 65536 / (NT * MINB): 16 warps per SM for both)
+constexpr int GLSZM_NT = 128, GLSZM_MINB = 4, GLDM_NT = 256, GLDM_MINB = 2;
+
+template <int CLS, int NT, int MINB>
+static int tiles_fast_launch(const SmallFastTables* T, const uint8_t* lev, const uint8_t* centers, const VoxParams& P,
+                             double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
+  int grid = 0;
+  RB_CUDA(resident_grid(tiles_fast_kernel<CLS, NT, MINB>, NT, 0, (long long)(z1 - z0) * P.Y * P.X, grid));
+  tiles_fast_kernel<CLS, NT, MINB><<<grid, NT, 0, st>>>(lev, centers, P, T, out, fstride, z0, z1, out_z0);
+  RB_LAUNCH_CHECK();
+  return RB_OK;
 }
 
 // NGTDM over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh).  Per-thread scratch for the level classes
@@ -205,7 +240,7 @@ ngtdm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
       const bool is_center = chunk_center(lev, centers, plane, v);
       int wl[27];
       load_window27(lev, P, v.z, v.y, v.x, v.vi, is_center, wl, 1);
-      if (is_center && ngtdm_window_full(wl)) {
+      if (is_center && window27_full(wl)) {
         double f[NGTDM_NF];
         ngtdm_fast_body<true>(wl, T, f, ng_pk + tid, ng_ns + tid, NT);
 #pragma unroll
@@ -246,13 +281,11 @@ int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const Vo
     int grid = 0;
     RB_CUDA(resident_grid(ngtdm_fast_kernel<NGTDM_NT>, NGTDM_NT, 0, total, grid));
     ngtdm_fast_kernel<NGTDM_NT><<<grid, NGTDM_NT, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
-  } else if (cls == C_GLSZM) {
-    small_fast_kernel<C_GLSZM, 128, false><<<grid_for(total, 128, 32), 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
-  } else {
-    small_fast_kernel<C_GLDM, 256, true><<<grid_for(total, 256, 16), 256, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
   }
-  RB_LAUNCH_CHECK();
-  return RB_OK;
+  if (cls == C_GLSZM) return tiles_fast_launch<C_GLSZM, GLSZM_NT, GLSZM_MINB>(T, l8, centers, P, out, fstride, z0, z1, out_z0, st);
+  return tiles_fast_launch<C_GLDM, GLDM_NT, GLDM_MINB>(T, l8, centers, P, out, fstride, z0, z1, out_z0, st);
 }
 
 }  // namespace rb
