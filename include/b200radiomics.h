@@ -96,7 +96,10 @@ int rb_pack_levels_dev(const int32_t *image_dev, const uint8_t *mask_dev, long l
  * `cls` over its (2r+1)^3 kernel window and store them; otherwise store settings->initValue.
  * Feature f of voxel (z,y,x) goes to
  *     out[f * out_feature_stride + ((z - out_z0) * Y + y) * X + x]
- * as float64 (out_is_f32 == 0, the reference's map dtype, base.py:205-209) or float32.
+ * as float64 (out_is_f32 == 0, the reference's map dtype, base.py:205-209) or float32 (out_is_f32 != 0; every path:
+ * fast, generic, every kernelRadius <= 3, weighted / asymmetric GLCM, force2D, 16-bit levels).  out_feature_stride and
+ * out_z0 count elements of that type.  Features are computed in float64 either way and a float32 map holds each value
+ * rounded to nearest once (NaN stays NaN), so it equals the float64 map converted to float32 bit for bit.
  * Angles that are empty for every voxel of the ROI are "deleted" like in the reference
  * (glcm.py:187-196); rb_glcm_alive_angles_dev computes that set (32-bit words, bit a = angle a,
  * RB_ALIVE_WORDS words, zero-initialised by the caller) and alive_dev may be NULL to keep all.
@@ -117,7 +120,8 @@ int rb_voxel_features_dev(int cls, const void *levels_dev, int level_bytes, cons
  * rb_memcpy2d_async: `height` rows of `width` bytes, row pitches in bytes; kind 1 = host->device, 2 = device->host,
  *   3 = device->device (cudaMemcpy2DAsync on `stream`; host memory should be page-locked for a true async copy).
  * rb_maps_to_f32_dev: rows of `width` float64 elements -> float32 (element pitches), the opt-in compact map type
- *   (half the PCIe bytes; the tolerance of the path is 1e-5 relative, float32 carries 6e-8). */
+ *   (half the PCIe bytes; the tolerance of the path is 1e-5 relative, float32 carries 6e-8) for maps computed in
+ *   float64, such as first order's; the texture classes write float32 maps directly (out_is_f32). */
 int rb_memcpy2d_async(void *dst, unsigned long long dpitch, const void *src, unsigned long long spitch,
                       unsigned long long width, unsigned long long height, int kind, void *stream);
 int rb_maps_to_f32_dev(const double *src_dev, long long src_pitch, float *dst_dev, long long dst_pitch,

@@ -24,24 +24,26 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+// the voxel kernels' launch functions: `out` holds float maps when out_f32, else double
 int voxel_features_generic(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P,
-                           double* out, long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st);
+                           void* out, bool out_f32, long long fstride, int z0, int z1, int out_z0, int* status,
+                           cudaStream_t st);
 int glcm_alive_angles(const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P, uint32_t* alive,
                       cudaStream_t st);
 int pack_levels(const int32_t* image, const uint8_t* mask, long long n, int Ng, void* lev, uint32_t* presence,
                 int* status, cudaStream_t st);
 bool glcm_fast_applicable(int cls, int level_bytes, const VoxParams& P);
 int glcm_release_queues();
-int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, double* out, long long fstride,
+int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
                      int z0, int z1, int out_z0, cudaStream_t st);
 
 bool glrlm_fast_applicable(int cls, int level_bytes, const VoxParams& P);
-int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, double* out, long long fstride,
+int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
                       int z0, int z1, int out_z0, cudaStream_t st);
 
 bool small_fast_applicable(int cls, int level_bytes, const VoxParams& P);
-int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, double* out, long long fstride,
-                      int z0, int z1, int out_z0, cudaStream_t st);
+int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
+                      long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
 
 // B200_RADIOMICS_FORCE_GENERIC=1 routes everything through the generic kernels (used by the
 // tests to cross-check the fast paths on the GPU)
@@ -194,21 +196,21 @@ int rb_voxel_features_dev(int cls, const void* levels_dev, int level_bytes, cons
                           void* out_dev, int out_is_f32, long long out_feature_stride, int out_z0, int* status_dev,
                           void* stream) {
   if (cls < 0 || cls > 4) return fail(RB_ERR_ARG, "unknown texture class %d", cls);
-  if (out_is_f32) return fail(RB_ERR_UNSUPPORTED, "float32 maps not implemented yet");
   if (z0 < 0 || z1 > Z || z0 > z1) return fail(RB_ERR_ARG, "bad z range");
   VoxParams P;
   if (fill_vox_params(cls, Z, Y, X, *settings, P)) return fail(RB_ERR_ARG, "bad voxel settings");
   if (alive_host && cls == C_GLCM) memcpy(P.alive, alive_host, sizeof P.alive);
+  const bool f32 = out_is_f32 != 0;
   if (!force_generic() && glcm_fast_applicable(cls, level_bytes, P))
-    return glcm_fast_launch(levels_dev, centers_dev, P, (double*)out_dev, out_feature_stride, z0, z1, out_z0,
+    return glcm_fast_launch(levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
                             (cudaStream_t)stream);
   if (!force_generic() && small_fast_applicable(cls, level_bytes, P))
-    return small_fast_launch(cls, levels_dev, centers_dev, P, (double*)out_dev, out_feature_stride, z0, z1, out_z0,
+    return small_fast_launch(cls, levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
                              (cudaStream_t)stream);
   if (!force_generic() && glrlm_fast_applicable(cls, level_bytes, P))
-    return glrlm_fast_launch(levels_dev, centers_dev, P, (double*)out_dev, out_feature_stride, z0, z1, out_z0,
+    return glrlm_fast_launch(levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
                              (cudaStream_t)stream);
-  return voxel_features_generic(cls, levels_dev, level_bytes, centers_dev, P, (double*)out_dev, out_feature_stride, z0,
+  return voxel_features_generic(cls, levels_dev, level_bytes, centers_dev, P, out_dev, f32, out_feature_stride, z0,
                                 z1, out_z0, status_dev, (cudaStream_t)stream);
 }
 

@@ -173,18 +173,23 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
 
 // ---- phase A (one thread per centre voxel) and phase C (finish) ---------------------------------
 // phase A of one centre voxel; store: write its 24 maps and queue its eigen-tasks (the general body holds barriers, so
-// every thread of the block runs it, idle ones with store = false)
-template <bool FULL, int NT>
+// every thread of the block runs it, idle ones with store = false).  Float maps: the partial MCC of a voxel with tasks
+// also goes to mcc_part[t] (t = chunk index) in double, so that phase C rounds the finished MCC once.
+template <bool FULL, int NT, typename OutT>
 __device__ __forceinline__ void glcm_phaseA_voxel(const uint8_t* w, uint32_t* eq, const GlcmFastTables& T, const VoxParams& P,
-                                                  const ChunkVoxel& v, bool store, double* __restrict__ out, long long fstride,
-                                                  GlcmTask* __restrict__ queue, unsigned* __restrict__ qcount) {
+                                                  const ChunkVoxel& v, bool store, OutT* __restrict__ out, long long fstride,
+                                                  GlcmTask* __restrict__ queue, unsigned* __restrict__ qcount,
+                                                  double* __restrict__ mcc_part, long long t) {
   double f[GLCM_NF];
   int n_ok = 0;
   unsigned long long tcls = 0;
   const uint32_t tasks = glcm_fast_voxel_phaseA<FULL>(w, NT, eq, NT, T, P, f, &n_ok, &tcls);
   if (!store) return;
 #pragma unroll
-  for (int k = 0; k < GLCM_NF; k++) out[k * fstride + v.oi] = f[k];
+  for (int k = 0; k < GLCM_NF; k++) store_map(out + k * fstride + v.oi, f[k]);
+  if constexpr (!std::is_same<OutT, double>::value) {
+    if (tasks) mcc_part[t] = f[G_MCC];
+  }
   if (tasks) {
     const int k = __popc(tasks);
     unsigned q = atomicAdd(qcount, (unsigned)k);
@@ -202,12 +207,13 @@ __device__ __forceinline__ void glcm_phaseA_voxel(const uint8_t* w, uint32_t* eq
 // Phase A over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh).  The window bytes live in shared
 // memory, [27][NT].  (List entries are chunk indices: a chunk of 2^32 voxels would need a 1.3 TB eigen-task queue,
 // which glcm_fast_launch fails to allocate first.)
-template <int MINB, int NT>
+// OutT: the map type (store_map).  mcc_part: the chunk's float64 partial-MCC plane, float maps only.
+template <int MINB, int NT, typename OutT>
 __global__ void __launch_bounds__(NT, MINB)
 glcm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
                  const __grid_constant__ VoxParams P, const GlcmFastTables* __restrict__ Tg,
-                 double* __restrict__ out, long long fstride, int z0, int z1, int out_z0,
-                 GlcmTask* __restrict__ queue, unsigned* __restrict__ qcount) {
+                 OutT* __restrict__ out, long long fstride, int z0, int z1, int out_z0,
+                 GlcmTask* __restrict__ queue, unsigned* __restrict__ qcount, double* __restrict__ mcc_part = nullptr) {
   __shared__ GlcmFastTables T;
   __shared__ unsigned defer[2 * NT];                                // chunk indices of the voxels left to the general body
   __shared__ unsigned ndefer;
@@ -224,27 +230,32 @@ glcm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ ce
       const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t, live);
       const bool center = live && chunk_center(lev, centers, plane, v);
       if (load_window27(lev, P, v.z, v.y, v.x, v.vi, center, w, NT)) {
-        glcm_phaseA_voxel<true, NT>(w, eq, T, P, v, true, out, fstride, queue, qcount);
+        glcm_phaseA_voxel<true, NT>(w, eq, T, P, v, true, out, fstride, queue, qcount, mcc_part, t);
       } else if (center) {
         defer_it();
       } else if (live) {
 #pragma unroll
-        for (int k = 0; k < GLCM_NF; k++) out[k * fstride + v.oi] = P.init_value;
+        for (int k = 0; k < GLCM_NF; k++) store_map(out + k * fstride + v.oi, P.init_value);
       }
     },
     [&](auto entry, bool live) {                                    // idle threads run on an all-zero window
       const long long plane = (long long)P.Y * P.X;
-      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, live ? entry() : 0, live);
+      const long long t = live ? entry() : 0;
+      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t, live);
       load_window27(lev, P, v.z, v.y, v.x, v.vi, live && chunk_center(lev, centers, plane, v), w, NT);
-      glcm_phaseA_voxel<false, NT>(w, eq, T, P, v, live, out, fstride, queue, qcount);
+      glcm_phaseA_voxel<false, NT>(w, eq, T, P, v, live, out, fstride, queue, qcount, mcc_part, t);
     });
 }
 
 
+// Float maps: the partial MCC comes from phase A's float64 plane mcc_part (chunk of planes from za), and the finished
+// double sum is rounded once as it is stored.
+template <typename OutT>
 __global__ void __launch_bounds__(256)
 glcm_fast_finish_kernel(const __grid_constant__ VoxParams P, const GlcmTask* __restrict__ queue,
                         const unsigned* __restrict__ qcount, const double* __restrict__ res,
-                        double* __restrict__ mcc_map /* out + G_MCC*fstride */, int out_z0) {
+                        OutT* __restrict__ mcc_map /* out + G_MCC*fstride */, int out_z0,
+                        const double* __restrict__ mcc_part = nullptr, int za = 0) {
   const unsigned n = *qcount;
   const long long plane = (long long)P.Y * P.X;
   for (unsigned k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
@@ -253,7 +264,11 @@ glcm_fast_finish_kernel(const __grid_constant__ VoxParams P, const GlcmTask* __r
     double add = 0;
     for (int j = 0; j < e.count; j++) add += res[k + j];
     const long long oi = e.vi - (long long)out_z0 * plane;   // contiguous volume: vi = z*plane + rem
-    mcc_map[oi] += add / e.n_ok;
+    if constexpr (std::is_same<OutT, double>::value) mcc_map[oi] += add / e.n_ok;
+    else {
+      const double mcc = mcc_part[e.vi - (long long)za * plane] + add / e.n_ok;
+      store_map(mcc_map + oi, mcc);
+    }
   }
 }
 

@@ -1,6 +1,7 @@
 // Fast fused voxel-based kernels for the headline configuration (kernelRadius 1, 3-D,
 // distances [1], 8-bit levels).  One thread per centre voxel, consecutive threads = consecutive
-// x so the 24 float64 map stores of a warp are 256-byte coalesced segments.
+// x so the 24 float64 map stores of a warp are 256-byte coalesced segments (128-byte for float32 maps).
+// Every kernel and launch function takes the map type (double or float, store_map in voxel_tiles.cuh).
 #include <map>
 #include <mutex>
 
@@ -19,8 +20,12 @@ bool glcm_fast_applicable(int cls, int level_bytes, const VoxParams& P) {
          !P.weighted && P.Ng <= 255;
 }
 
-// per (device, stream) task queue, grown on demand
-struct GlcmQueue { GlcmTask* q = nullptr; double* res = nullptr; unsigned* count = nullptr; size_t cap = 0; };
+// per (device, stream) task queue, grown on demand; float maps add the float64 partial-MCC plane of a chunk (mcc,
+// mcc_cap doubles)
+struct GlcmQueue {
+  GlcmTask* q = nullptr; double* res = nullptr; unsigned* count = nullptr; size_t cap = 0;
+  double* mcc = nullptr; size_t mcc_cap = 0;
+};
 static std::mutex g_queue_mu;
 static std::map<std::pair<int, cudaStream_t>, GlcmQueue> g_queue_cache;
 // rb_release_device_caches: give the eigen-task queues of the current device back (up to 1.15 GB per stream that ran GLCM)
@@ -31,13 +36,13 @@ int glcm_release_queues() {
   std::lock_guard<std::mutex> lk(g_queue_mu);
   for (auto it = g_queue_cache.begin(); it != g_queue_cache.end();) {
     if (it->first.first == dev) {
-      cudaFree(it->second.q); cudaFree(it->second.res); cudaFree(it->second.count);
+      cudaFree(it->second.q); cudaFree(it->second.res); cudaFree(it->second.count); cudaFree(it->second.mcc);
       it = g_queue_cache.erase(it);
     } else ++it;
   }
   return RB_OK;
 }
-static GlcmQueue* glcm_queue(cudaStream_t st, size_t need) {
+static GlcmQueue* glcm_queue(cudaStream_t st, size_t need, size_t mcc_need) {
   std::mutex& mu = g_queue_mu;
   auto& cache = g_queue_cache;
   int dev = 0;
@@ -51,11 +56,17 @@ static GlcmQueue* glcm_queue(cudaStream_t st, size_t need) {
     if (cudaMalloc(&Q.res, need * sizeof(double)) != cudaSuccess) { cudaFree(Q.q); Q.q = nullptr; return nullptr; }
     Q.cap = need;
   }
+  if (Q.mcc_cap < mcc_need) {
+    if (Q.mcc) { cudaStreamSynchronize(st); cudaFree(Q.mcc); Q.mcc = nullptr; Q.mcc_cap = 0; }
+    if (cudaMalloc(&Q.mcc, mcc_need * sizeof(double)) != cudaSuccess) return nullptr;
+    Q.mcc_cap = mcc_need;
+  }
   return &Q;
 }
 
-int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, double* out, long long fstride,
-                     int z0, int z1, int out_z0, cudaStream_t st) {
+template <typename OutT>
+static int glcm_fast_run(const void* lev, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
+                         int z0, int z1, int out_z0, cudaStream_t st) {
   const GlcmFastTables* T = device_table<GlcmFastTables>([&](GlcmFastTables& h) { glcm_fast_build_tables(h, P.Ng); }, P.Ng);
   if (!T) return fail(RB_ERR_CUDA, "could not build the GLCM table block on the device");
   const long long plane = (long long)P.Y * P.X;
@@ -68,14 +79,17 @@ int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P
   int zchunk = (int)(max_entries / (plane * GF_NA));
   if (zchunk < 1) zchunk = 1;
   if (zchunk > z1 - z0) zchunk = z1 - z0;
-  GlcmQueue* Q = glcm_queue(st, (size_t)zchunk * plane * GF_NA);
+  // float maps: phase A keeps the partial MCC of the voxels with eigen-tasks in float64 (zchunk planes), so the finished
+  // MCC is rounded to float once
+  constexpr bool f64 = std::is_same<OutT, double>::value;
+  GlcmQueue* Q = glcm_queue(st, (size_t)zchunk * plane * GF_NA, f64 ? 0 : (size_t)zchunk * plane);
   if (!Q) return fail(RB_ERR_NOMEM, "could not allocate the GLCM eigen-task queue");
   // phase A: one CTA per SM (register-bound).  512 threads at 128 registers (a hundred spilled words per thread, L1-
   // resident) put 16 warps on an SM instead of the 8 of a 256-thread / 236-register build, which hides more of the
   // latency of this issue-bound kernel.
   constexpr int NT = 512;
   const int smem = glcm_phaseA_smem_bytes(NT);
-  RB_CUDA(set_max_dynamic_smem(glcm_fast_kernel<1, NT>, smem));
+  RB_CUDA(set_max_dynamic_smem(glcm_fast_kernel<1, NT, OutT>, smem));
   // register Lanczos: 90 KB of per-thread shared vectors per CTA -> two CTAs per SM
   RB_CUDA(set_max_dynamic_smem(glcm_fast_solve_kernel<2>, GF_LZ_SMEM_BYTES));
   const uint8_t* l8 = (const uint8_t*)lev;
@@ -83,8 +97,9 @@ int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P
     const int zb = za + zchunk < z1 ? za + zchunk : z1;
     RB_CUDA(cudaMemsetAsync(Q->count, 0, sizeof(unsigned), st));
     int grid = 0;
-    RB_CUDA(resident_grid(glcm_fast_kernel<1, NT>, NT, smem, (long long)(zb - za) * plane, grid));
-    glcm_fast_kernel<1, NT><<<grid, NT, smem, st>>>(l8, centers, P, T, out, fstride, za, zb, out_z0, Q->q, Q->count);
+    RB_CUDA(resident_grid(glcm_fast_kernel<1, NT, OutT>, NT, smem, (long long)(zb - za) * plane, grid));
+    glcm_fast_kernel<1, NT, OutT><<<grid, NT, smem, st>>>(l8, centers, P, T, out, fstride, za, zb, out_z0, Q->q, Q->count,
+                                                         Q->mcc);
     RB_LAUNCH_CHECK();
     // One launch per size group keeps ONE solver body in the instruction cache (the three Lanczos templates together are
     // 18.5 k SASS instructions, 296 KB, and on a smooth volume the blocks of an SM otherwise sit in different groups); the
@@ -94,17 +109,25 @@ int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P
     for (int g = 18; g >= 14; g -= 2)
       glcm_fast_solve_kernel<2><<<sms * 2, 128, GF_LZ_SMEM_BYTES, st>>>(l8, P, T, Q->q, Q->count, Q->res, g);
     RB_LAUNCH_CHECK();
-    glcm_fast_finish_kernel<<<sms * 8, 256, 0, st>>>(P, Q->q, Q->count, Q->res, out + (long long)G_MCC * fstride, out_z0);
+    glcm_fast_finish_kernel<OutT><<<sms * 8, 256, 0, st>>>(P, Q->q, Q->count, Q->res, out + (long long)G_MCC * fstride,
+                                                           out_z0, Q->mcc, za);
     RB_LAUNCH_CHECK();
   }
   return RB_OK;
 }
 
+int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
+                     int z0, int z1, int out_z0, cudaStream_t st) {
+  if (out_f32) return glcm_fast_run(lev, centers, P, (float*)out, fstride, z0, z1, out_z0, st);
+  return glcm_fast_run(lev, centers, P, (double*)out, fstride, z0, z1, out_z0, st);
+}
+
 // ---------------------------------------------------------------------------------- GLRLM
+template <typename OutT>
 __global__ void __launch_bounds__(128)
 glrlm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
                   const __grid_constant__ VoxParams P, const GlrlmFastTables* __restrict__ Tg,
-                  double* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
+                  OutT* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
   __shared__ GlrlmFastTables T;
   copy_tables_to_shared(T, Tg);
   __syncthreads();
@@ -114,7 +137,7 @@ glrlm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
     const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t);
     if (!chunk_center(lev, centers, plane, v)) {
 #pragma unroll
-      for (int k = 0; k < GLRLM_NF; k++) out[k * fstride + v.oi] = P.init_value;
+      for (int k = 0; k < GLRLM_NF; k++) store_map(out + k * fstride + v.oi, P.init_value);
       continue;
     }
     int wl[27];
@@ -122,7 +145,7 @@ glrlm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
     double f[GLRLM_NF];
     glrlm_fast_voxel(wl, T, f);
 #pragma unroll
-    for (int k = 0; k < GLRLM_NF; k++) out[k * fstride + v.oi] = f[k];
+    for (int k = 0; k < GLRLM_NF; k++) store_map(out + k * fstride + v.oi, f[k]);
   }
 }
 
@@ -130,13 +153,15 @@ bool glrlm_fast_applicable(int cls, int level_bytes, const VoxParams& P) {
   return cls == C_GLRLM && level_bytes == 1 && P.rz == 1 && P.ry == 1 && P.rx == 1 && P.na == 13 && !P.weighted && P.Ng <= 255;
 }
 
-int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, double* out, long long fstride,
+int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
                       int z0, int z1, int out_z0, cudaStream_t st) {
   const GlrlmFastTables* T = device_table<GlrlmFastTables>(glrlm_fast_build_tables);
   if (!T) return fail(RB_ERR_CUDA, "could not build the GLRLM table block on the device");
   const long long total = (long long)(z1 - z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
-  glrlm_fast_kernel<<<grid_for(total, 128, 32), 128, 0, st>>>((const uint8_t*)lev, centers, P, T, out, fstride, z0, z1, out_z0);
+  const int grid = grid_for(total, 128, 32);
+  if (out_f32) glrlm_fast_kernel<<<grid, 128, 0, st>>>((const uint8_t*)lev, centers, P, T, (float*)out, fstride, z0, z1, out_z0);
+  else glrlm_fast_kernel<<<grid, 128, 0, st>>>((const uint8_t*)lev, centers, P, T, (double*)out, fstride, z0, z1, out_z0);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
@@ -156,10 +181,10 @@ __device__ __forceinline__ void tile_body(const int* wl, const SmallFastTables& 
   else gldm_fast_body<FULL>(wl, alpha, T, f);
 }
 
-template <int CLS, int NT, int MINB>
+template <int CLS, int NT, int MINB, typename OutT>
 __global__ void __launch_bounds__(NT, MINB)
 tiles_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers, const __grid_constant__ VoxParams P,
-                  const SmallFastTables* __restrict__ Tg, double* __restrict__ out, long long fstride,
+                  const SmallFastTables* __restrict__ Tg, OutT* __restrict__ out, long long fstride,
                   int z0, int z1, int out_z0) {
   using K = TileClass<CLS>;
   __shared__ SmallFastTables T;
@@ -182,12 +207,12 @@ tiles_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
         double f[K::NF];
         tile_body<CLS, true>(wl, T, P.alpha, scr_mg + tid, NT, f);
 #pragma unroll
-        for (int k = 0; k < K::NF; k++) out[k * fstride + v.oi] = f[k];
+        for (int k = 0; k < K::NF; k++) store_map(out + k * fstride + v.oi, f[k]);
       } else if (is_center) {
         defer_it();
       } else {
 #pragma unroll
-        for (int k = 0; k < K::NF; k++) out[k * fstride + v.oi] = P.init_value;
+        for (int k = 0; k < K::NF; k++) store_map(out + k * fstride + v.oi, P.init_value);
       }
     },
     [&](auto entry, bool live) {
@@ -198,19 +223,19 @@ tiles_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
       double f[K::NF];
       tile_body<CLS, false>(wl, T, P.alpha, scr_mg + tid, NT, f);
 #pragma unroll
-      for (int k = 0; k < K::NF; k++) out[k * fstride + v.oi] = f[k];
+      for (int k = 0; k < K::NF; k++) store_map(out + k * fstride + v.oi, f[k]);
     });
 }
 
 // block size and blocks per SM (registers <= 65536 / (NT * MINB): 16 warps per SM for both)
 constexpr int GLSZM_NT = 128, GLSZM_MINB = 4, GLDM_NT = 256, GLDM_MINB = 2;
 
-template <int CLS, int NT, int MINB>
+template <int CLS, int NT, int MINB, typename OutT>
 static int tiles_fast_launch(const SmallFastTables* T, const uint8_t* lev, const uint8_t* centers, const VoxParams& P,
-                             double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
+                             OutT* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
   int grid = 0;
-  RB_CUDA(resident_grid(tiles_fast_kernel<CLS, NT, MINB>, NT, 0, (long long)(z1 - z0) * P.Y * P.X, grid));
-  tiles_fast_kernel<CLS, NT, MINB><<<grid, NT, 0, st>>>(lev, centers, P, T, out, fstride, z0, z1, out_z0);
+  RB_CUDA(resident_grid(tiles_fast_kernel<CLS, NT, MINB, OutT>, NT, 0, (long long)(z1 - z0) * P.Y * P.X, grid));
+  tiles_fast_kernel<CLS, NT, MINB, OutT><<<grid, NT, 0, st>>>(lev, centers, P, T, out, fstride, z0, z1, out_z0);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
@@ -218,11 +243,11 @@ static int tiles_fast_launch(const SmallFastTables* T, const uint8_t* lev, const
 // NGTDM over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh).  Per-thread scratch for the level classes
 // lives in shared memory, [entry][thread].
 constexpr int NGTDM_NT = 128;
-template <int NT>
+template <int NT, typename OutT>
 __global__ void __launch_bounds__(NT, 4)
 ngtdm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
                   const __grid_constant__ VoxParams P, const SmallFastTables* __restrict__ Tg,
-                  double* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
+                  OutT* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
   __shared__ SmallFastTables T;
   __shared__ double ng_ns[27 * NT];
   __shared__ int ng_pk[27 * NT];
@@ -244,12 +269,12 @@ ngtdm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
         double f[NGTDM_NF];
         ngtdm_fast_body<true>(wl, T, f, ng_pk + tid, ng_ns + tid, NT);
 #pragma unroll
-        for (int k = 0; k < NGTDM_NF; k++) out[k * fstride + v.oi] = f[k];
+        for (int k = 0; k < NGTDM_NF; k++) store_map(out + k * fstride + v.oi, f[k]);
       } else if (is_center) {
         defer_it();
       } else {
 #pragma unroll
-        for (int k = 0; k < NGTDM_NF; k++) out[k * fstride + v.oi] = P.init_value;
+        for (int k = 0; k < NGTDM_NF; k++) store_map(out + k * fstride + v.oi, P.init_value);
       }
     },
     [&](auto entry, bool live) {
@@ -261,7 +286,7 @@ ngtdm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
       double f[NGTDM_NF];
       ngtdm_fast_body<false>(wl, T, f, ng_pk + tid, ng_ns + tid, NT);
 #pragma unroll
-      for (int k = 0; k < NGTDM_NF; k++) out[k * fstride + v.oi] = f[k];
+      for (int k = 0; k < NGTDM_NF; k++) store_map(out + k * fstride + v.oi, f[k]);
     });
 }
 
@@ -270,22 +295,29 @@ bool small_fast_applicable(int cls, int level_bytes, const VoxParams& P) {
          P.na == 26 && P.Ng <= 255;
 }
 
-int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, double* out, long long fstride,
-                      int z0, int z1, int out_z0, cudaStream_t st) {
-  const SmallFastTables* T = device_table<SmallFastTables>(small_fast_build_tables);
-  if (!T) return fail(RB_ERR_CUDA, "could not build the table block on the device");
-  const long long total = (long long)(z1 - z0) * P.Y * P.X;
-  if (total <= 0) return RB_OK;
-  const uint8_t* l8 = (const uint8_t*)lev;
+template <typename OutT>
+static int small_fast_run(int cls, const SmallFastTables* T, const uint8_t* l8, const uint8_t* centers, const VoxParams& P,
+                          OutT* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
   if (cls == C_NGTDM) {
     int grid = 0;
-    RB_CUDA(resident_grid(ngtdm_fast_kernel<NGTDM_NT>, NGTDM_NT, 0, total, grid));
-    ngtdm_fast_kernel<NGTDM_NT><<<grid, NGTDM_NT, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
+    RB_CUDA(resident_grid(ngtdm_fast_kernel<NGTDM_NT, OutT>, NGTDM_NT, 0, (long long)(z1 - z0) * P.Y * P.X, grid));
+    ngtdm_fast_kernel<NGTDM_NT, OutT><<<grid, NGTDM_NT, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
     RB_LAUNCH_CHECK();
     return RB_OK;
   }
   if (cls == C_GLSZM) return tiles_fast_launch<C_GLSZM, GLSZM_NT, GLSZM_MINB>(T, l8, centers, P, out, fstride, z0, z1, out_z0, st);
   return tiles_fast_launch<C_GLDM, GLDM_NT, GLDM_MINB>(T, l8, centers, P, out, fstride, z0, z1, out_z0, st);
+}
+
+int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
+                      long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
+  const SmallFastTables* T = device_table<SmallFastTables>(small_fast_build_tables);
+  if (!T) return fail(RB_ERR_CUDA, "could not build the table block on the device");
+  const long long total = (long long)(z1 - z0) * P.Y * P.X;
+  if (total <= 0) return RB_OK;
+  const uint8_t* l8 = (const uint8_t*)lev;
+  if (out_f32) return small_fast_run(cls, T, l8, centers, P, (float*)out, fstride, z0, z1, out_z0, st);
+  return small_fast_run(cls, T, l8, centers, P, (double*)out, fstride, z0, z1, out_z0, st);
 }
 
 }  // namespace rb

@@ -2,7 +2,7 @@
 // whole texture class over its kernel window with the per-voxel math of vox_features.cuh and
 // writes the feature maps with coalesced stores (consecutive threads = consecutive x).  Handles
 // any kernelRadius <= 3, distances subset {1,2,3}, force2D, asymmetric / weighted GLCM, uint8 or
-// uint16 levels.  The r=1 fast path lives in voxel_fast.cu.
+// uint16 levels, float64 or float32 maps (store_map).  The r=1 fast path lives in voxel_fast.cu.
 #include "common.cuh"
 #include "host_common.hpp"
 #include "vox_features.cuh"
@@ -10,10 +10,10 @@
 
 namespace rb {
 
-template <typename T, int WCAP, int CLS, bool WEIGHTED>
+template <typename T, int WCAP, int CLS, bool WEIGHTED, typename OutT>
 __global__ void __launch_bounds__(128)
 voxel_features_kernel(const T* __restrict__ lev, const uint8_t* __restrict__ centers,
-                      const __grid_constant__ VoxParams P, double* __restrict__ out, long long fstride,
+                      const __grid_constant__ VoxParams P, OutT* __restrict__ out, long long fstride,
                       int z0, int z1, int out_z0, int* __restrict__ status) {
   const long long plane = (long long)P.Y * P.X;
   const long long total = (long long)(z1 - z0) * plane;
@@ -25,7 +25,7 @@ voxel_features_kernel(const T* __restrict__ lev, const uint8_t* __restrict__ cen
                        : CLS == C_GLDM ? GLDM_NF : NGTDM_NF;
     if (!is_center) {
 #pragma unroll
-      for (int k = 0; k < NF; k++) out[k * fstride + v.oi] = P.init_value;
+      for (int k = 0; k < NF; k++) store_map(out + k * fstride + v.oi, P.init_value);
       continue;
     }
     uint16_t w[WCAP];
@@ -38,7 +38,7 @@ voxel_features_kernel(const T* __restrict__ lev, const uint8_t* __restrict__ cen
     else if (CLS == C_GLDM) gldm_voxel<WCAP>(w, P, f);
     else ngtdm_voxel<WCAP>(w, P, f);
 #pragma unroll
-    for (int k = 0; k < NF; k++) out[k * fstride + v.oi] = f[k];
+    for (int k = 0; k < NF; k++) store_map(out + k * fstride + v.oi, f[k]);
     if (st && status) atomicOr(status, st);
   }
 }
@@ -94,13 +94,13 @@ pack_levels_kernel(const int32_t* __restrict__ image, const uint8_t* __restrict_
   if (bad && status) atomicOr(status, 1);
 }
 
-template <typename T, int WCAP>
-static int launch_cls(int cls, bool weighted, const T* lev, const uint8_t* centers, const VoxParams& P, double* out,
+template <typename T, int WCAP, typename OutT>
+static int launch_cls(int cls, bool weighted, const T* lev, const uint8_t* centers, const VoxParams& P, OutT* out,
                       long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
   const long long total = (long long)(z1 - z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
   const int grid = grid_for(total, 128, 64);
-#define RB_GO(CLS, WGT) voxel_features_kernel<T, WCAP, CLS, WGT><<<grid, 128, 0, st>>>(lev, centers, P, out, fstride, z0, z1, out_z0, status)
+#define RB_GO(CLS, WGT) voxel_features_kernel<T, WCAP, CLS, WGT, OutT><<<grid, 128, 0, st>>>(lev, centers, P, out, fstride, z0, z1, out_z0, status)
   switch (cls) {
     case C_GLCM: if (weighted) RB_GO(C_GLCM, true); else RB_GO(C_GLCM, false); break;
     case C_GLRLM: if (weighted) RB_GO(C_GLRLM, true); else RB_GO(C_GLRLM, false); break;
@@ -114,22 +114,30 @@ static int launch_cls(int cls, bool weighted, const T* lev, const uint8_t* cente
   return RB_OK;
 }
 
-template <typename T>
-static int launch_generic(int cls, const T* lev, const uint8_t* centers, const VoxParams& P, double* out,
+template <typename T, typename OutT>
+static int launch_generic(int cls, const T* lev, const uint8_t* centers, const VoxParams& P, OutT* out,
                           long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
   const int cap = window_capacity(P);
   const bool wgt = P.weighted != 0;
-  if (cap <= 27) return launch_cls<T, 27>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  if (cap <= 125) return launch_cls<T, 125>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  if (cap <= 343) return launch_cls<T, 343>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
+  if (cap <= 27) return launch_cls<T, 27, OutT>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
+  if (cap <= 125) return launch_cls<T, 125, OutT>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
+  if (cap <= 343) return launch_cls<T, 343, OutT>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
   return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
 }
 
-int voxel_features_generic(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P,
-                           double* out, long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
-  if (level_bytes == 1) return launch_generic<uint8_t>(cls, (const uint8_t*)lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  if (level_bytes == 2) return launch_generic<uint16_t>(cls, (const uint16_t*)lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
+template <typename OutT>
+static int generic_run(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P,
+                       OutT* out, long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
+  if (level_bytes == 1) return launch_generic(cls, (const uint8_t*)lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
+  if (level_bytes == 2) return launch_generic(cls, (const uint16_t*)lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
   return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
+}
+
+int voxel_features_generic(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P,
+                           void* out, bool out_f32, long long fstride, int z0, int z1, int out_z0, int* status,
+                           cudaStream_t st) {
+  if (out_f32) return generic_run(cls, lev, level_bytes, centers, P, (float*)out, fstride, z0, z1, out_z0, status, st);
+  return generic_run(cls, lev, level_bytes, centers, P, (double*)out, fstride, z0, z1, out_z0, status, st);
 }
 
 int glcm_alive_angles(const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P, uint32_t* alive,

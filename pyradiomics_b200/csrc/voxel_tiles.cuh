@@ -3,6 +3,8 @@
 // tests/host_emul/solve_kernel_emul.cpp compiles this header for the CPU (through glcm_kernels.cuh) with __device__,
 // __shared__ and __syncthreads defined as macros.
 #pragma once
+#include <type_traits>
+
 #include "vox_features.cuh"
 
 namespace rb {
@@ -25,6 +27,12 @@ RB_HD ChunkVoxel chunk_voxel(const VoxParams& P, long long plane, int z0, int ou
   v.oi = (long long)(v.z - out_z0) * plane + v.rem;
   return v;
 }
+
+// The one place the map type of the texture voxel kernels is decided: every map element is stored through here.  OutT
+// is double (the reference's map type) or float.  Every value is computed in double and rounded once, here: the float
+// conversion is round-to-nearest-even, as __double2float_rn, and keeps NaN.
+template <typename OutT>
+RB_HD void store_map(OutT* p, double v) { *p = (OutT)v; }
 
 // whether the voxel is a centre: centers[] if given, else a non-zero level (a read, so callers gate it with
 // `live && ...` where the thread may have no voxel)

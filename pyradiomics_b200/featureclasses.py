@@ -348,7 +348,8 @@ class RadiomicsFeaturesBase:
         z0, z1 = self.settings.get("b200_zrange") or (0, int(lev.shape[0]))
         with self.progressReporter(total=int(z1 - z0), desc="planes") as pbar:
             host = voxel.maps_to_host(launch, len(names), lev.shape, lev.device, idx, z0=int(z0), z1=int(z1),
-                                      zchunk=self._zchunk(int(z1 - z0)), out_dtype=self._map_dtype(), progress=pbar.update)
+                                      zchunk=self._zchunk(int(z1 - z0)), out_dtype=self._map_dtype(), progress=pbar.update,
+                                      map_dtypes=voxel.MAP_DTYPES if self.CLASS in _lib.CLASSES else (torch.float64,))
         st = 0 if status is None else int(status.item())
         if st & 2:
             raise _lib.B200Error("weighted GLCM entry list overflow")

@@ -63,7 +63,7 @@ def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1"
 
 def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CLASSES, spacing_zyx=(1.0, 1.0, 1.0),
                              wavelet="coif1", sigmas=(1.0, 2.0, 3.0), consume=None, lbp3d=None, image_types=(),
-                             gradient_use_spacing=True, normalize=None, resegment=None, **kw):
+                             gradient_use_spacing=True, normalize=None, resegment=None, map_dtype=torch.float64, **kw):
     """image: CUDA tensor (Z,Y,X) of raw intensities, mask: CUDA uint8/bool.  For every derived
     image (`image_types`, `gradient_use_spacing`, `lbp3d`: see derived_images): bin (binWidth/binCount in kw) -> pack ->
     fused kernels.
@@ -71,8 +71,11 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
     derived image comes from the normalised one; `resegment` (a dict with resegmentRange, resegmentMode) then resegments
     the mask against that image, and binning, the texture kernels and the LBP 3-D ROI use the resegmented mask -- the
     reference's order (featureextractor.py:316-392).  None (default) skips either step.
-    `consume(name, cls, maps)` is called with each float64 [F,Z,Y,X] result (maps are reused buffers unless consume keeps
-    them); returns the list of (image name, Ng, number of levels)."""
+    `consume(name, cls, maps)` is called with each [F,Z,Y,X] result of type `map_dtype` (float64, the reference's, or
+    float32: half the device memory, so a 512^3 suite fits on one 80 GB GPU; maps are reused buffers unless consume
+    keeps them); returns the list of (image name, Ng, number of levels)."""
+    if map_dtype not in voxel.MAP_DTYPES:
+        raise TypeError(f"voxel feature maps are float64 or float32, not {map_dtype}")
     if normalize is not None:
         image = IO.normalize_image_device(image, normalize.get("normalizeScale", 1), normalize.get("removeOutliers"))
     msk = (mask != 0).to(torch.uint8).contiguous()
@@ -89,7 +92,7 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
         for c in classes:
             nf = _lib.lib().rb_num_features(_lib.CLASS_ID[c])
             if c not in outs:
-                outs[c] = torch.empty((nf,) + tuple(lev.shape), dtype=torch.float64, device=lev.device)
+                outs[c] = torch.empty((nf,) + tuple(lev.shape), dtype=map_dtype, device=lev.device)
             maps = voxel.voxel_features(c, lev, s, out=outs[c], out_z0=0)
             if consume is not None:
                 consume(name, c, maps)

@@ -66,6 +66,17 @@ def level_bytes(lev: torch.Tensor) -> int:
     return 1 if lev.dtype == torch.uint8 else 2
 
 
+# the map types the texture kernels write: float64 (the reference's) or float32, each value rounded once from float64
+MAP_DTYPES = (torch.float64, torch.float32)
+
+
+def out_is_f32(out: torch.Tensor) -> int:
+    """rb_voxel_features_dev's out_is_f32 for a map buffer; any other dtype raises TypeError"""
+    if out.dtype not in MAP_DTYPES:
+        raise TypeError(f"voxel feature maps are float64 or float32, not {out.dtype}")
+    return int(out.dtype == torch.float32)
+
+
 def glcm_alive_angles(lev, settings, centers=None):
     Z, Y, X = lev.shape
     alive = torch.zeros(_lib.ALIVE_WORDS, dtype=torch.int32, device=lev.device)
@@ -75,17 +86,20 @@ def glcm_alive_angles(lev, settings, centers=None):
 
 
 def voxel_features(cls: str, lev: torch.Tensor, settings, *, centers=None, z0=0, z1=None, out=None, out_z0=None,
-                   alive=None, status=None):
+                   alive=None, status=None, dtype=torch.float64):
     """Launch the fused kernel of one class on planes [z0,z1) of `lev` (Z,Y,X).  Returns `out`:
-    float64 tensor [F, z1-z0, Y, X] (allocated when None).  Asynchronous on the current stream."""
+    [F, z1-z0, Y, X] maps of type `dtype` (float64 or float32), allocated when None.  A given `out` is float64 or float32
+    (its dtype decides; `dtype` is then ignored), with contiguous (Y, X) planes and any feature stride; plane z of the
+    volume goes to out[:, z - out_z0].  Asynchronous on the current stream."""
     cid = CLASS_ID[cls]
     Z, Y, X = lev.shape
     z1 = Z if z1 is None else z1
     nf = lib().rb_num_features(cid)
     if out is None:
-        out = torch.empty((nf, z1 - z0, Y, X), dtype=torch.float64, device=lev.device)
+        out = torch.empty((nf, z1 - z0, Y, X), dtype=dtype, device=lev.device)
         out_z0 = z0
-    assert out.dtype == torch.float64 and out.is_contiguous() and out.shape[0] == nf
+    f32 = out_is_f32(out)
+    assert out.shape[0] == nf and out.shape[2:] == (Y, X) and out.stride()[1:] == (Y * X, X, 1)
     if out_z0 is None:
         out_z0 = z0
     if cls == "glcm" and alive is None:
@@ -93,7 +107,7 @@ def voxel_features(cls: str, lev: torch.Tensor, settings, *, centers=None, z0=0,
     if status is None:
         status = torch.zeros(1, dtype=torch.int32, device=lev.device)
     check(lib().rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(z0), int(z1),
-                                      C.byref(settings), ptr(alive), ptr(out), 0, out.stride(0), int(out_z0), ptr(status),
+                                      C.byref(settings), ptr(alive), ptr(out), f32, out.stride(0), int(out_z0), ptr(status),
                                       stream()), cls)
     return out
 
@@ -134,7 +148,7 @@ def _runs(idx):
 
 def texture_launch(cls: str, lev: torch.Tensor, settings, *, centers=None, alive=None, status=None):
     """the `launch(za, zb, buf)` of maps_to_host for the fused kernel of one texture class: planes [za,zb) of `lev` into
-    `buf` [F, >= zb-za, Y, X] (plane za at buf[:, 0]) on the current stream"""
+    `buf` [F, >= zb-za, Y, X] (plane za at buf[:, 0], float64 or float32 maps as buf's dtype) on the current stream"""
     cid = CLASS_ID[cls]
     Z, Y, X = lev.shape
     if cls == "glcm" and alive is None:
@@ -144,8 +158,8 @@ def texture_launch(cls: str, lev: torch.Tensor, settings, *, centers=None, alive
 
     def launch(za, zb, buf):
         check(lib().rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(za), int(zb),
-                                          C.byref(settings), ptr(alive), ptr(buf), 0, buf.stride(0), int(za), ptr(status),
-                                          torch.cuda.current_stream(lev.device).cuda_stream), cls)
+                                          C.byref(settings), ptr(alive), ptr(buf), out_is_f32(buf), buf.stride(0), int(za),
+                                          ptr(status), torch.cuda.current_stream(lev.device).cuda_stream), cls)
     return launch
 
 
@@ -156,16 +170,20 @@ def class_maps_to_host(cls: str, lev: torch.Tensor, settings, feature_idx=None, 
     (texture_launch)."""
     launch = texture_launch(cls, lev, settings, centers=centers, alive=alive, status=status)
     return maps_to_host(launch, lib().rb_num_features(CLASS_ID[cls]), lev.shape, lev.device, feature_idx, z0=z0, z1=z1,
-                        zchunk=zchunk, out_dtype=out_dtype, host=host, copy_stream=copy_stream, progress=progress, sync=sync)
+                        zchunk=zchunk, out_dtype=out_dtype, host=host, copy_stream=copy_stream, progress=progress, sync=sync,
+                        map_dtypes=MAP_DTYPES)
 
 
 def maps_to_host(launch, nf, shape, dev, feature_idx=None, *, z0=0, z1=None, zchunk=64, out_dtype=torch.float64,
-                 host=None, copy_stream=None, progress=None, sync=True):
+                 host=None, copy_stream=None, progress=None, sync=True, map_dtypes=(torch.float64,)):
     """The voxel-map driver of every voxel class: `launch(za, zb, buf)` enqueues the `nf` maps of planes [za,zb) of a
     (Z,Y,X) = `shape` volume into `buf` [nf, >= zb-za, Y, X] on the current stream of device `dev`.  Planes [z0,z1) run
     in z-chunks into a two-slot device ring; every finished chunk leaves for the host on `copy_stream` -- ONE strided DMA
     per run of consecutive selected features (rb_memcpy2d_async) -- while the next chunk computes.  Only the maps in
-    `feature_idx` (default: all) are copied.  `out_dtype` float32 converts on the device first (half the PCIe bytes).
+    `feature_idx` (default: all) are copied.  `map_dtypes` are the map types `launch` writes (the texture kernels:
+    MAP_DTYPES): an `out_dtype` among them is the ring's type, so float32 maps go from the kernel to the host with no
+    float64 copy on the device; otherwise the ring is float64 and float32 converts on the device before the copy (half
+    the PCIe bytes either way).
     Returns the page-locked host tensor [len(feature_idx), z1-z0, Y, X] (allocated from torch's caching pinned
     allocator when `host` is None: the caller owns it, dropping it recycles the block).  sync=False returns without
     waiting for the last copies (the caller synchronises `copy_stream` before touching `host`), so a following class
@@ -183,9 +201,12 @@ def maps_to_host(launch, nf, shape, dev, feature_idx=None, *, z0=0, z1=None, zch
     copy_stream = copy_stream or torch.cuda.Stream(device=dev)
     zc = max(1, min(int(zchunk), nz))
     plane = Y * X
-    ring = [torch.empty((nf, zc, Y, X), dtype=torch.float64, device=dev) for _ in range(2 if nz > zc else 1)]
-    f32 = out_dtype == torch.float32
+    native = out_dtype in map_dtypes
+    ring = [torch.empty((nf, zc, Y, X), dtype=out_dtype if native else torch.float64, device=dev)
+            for _ in range(2 if nz > zc else 1)]
+    f32 = out_dtype == torch.float32 and not native         # convert float64 maps on the device
     ring32 = [torch.empty((len(idx), zc, Y, X), dtype=torch.float32, device=dev) for _ in ring] if f32 else None
+    esz = host.element_size()
     for t in ring + (ring32 or []):
         t.record_stream(copy_stream)                     # the caching allocator must not recycle them under the DMA
     copied = [None, None]
@@ -213,9 +234,9 @@ def maps_to_host(launch, nf, shape, dev, feature_idx=None, *, z0=0, z1=None, zch
                                       len(idx), 2, copy_stream.cuda_stream), "memcpy2d")
         else:
             for first, count, pos in _runs(idx):
-                check(L.rb_memcpy2d_async(host.data_ptr() + (pos * host.stride(0) + off) * 8, host.stride(0) * 8,
-                                          buf.data_ptr() + first * buf.stride(0) * 8, buf.stride(0) * 8, width * 8, count, 2,
-                                          copy_stream.cuda_stream), "memcpy2d")
+                check(L.rb_memcpy2d_async(host.data_ptr() + (pos * host.stride(0) + off) * esz, host.stride(0) * esz,
+                                          buf.data_ptr() + first * buf.stride(0) * esz, buf.stride(0) * esz, width * esz,
+                                          count, 2, copy_stream.cuda_stream), "memcpy2d")
         ev = torch.cuda.Event()
         ev.record(copy_stream)
         copied[slot] = ev
@@ -228,7 +249,7 @@ def maps_to_host(launch, nf, shape, dev, feature_idx=None, *, z0=0, z1=None, zch
 
 class HostExtractor:
     """End-to-end voxel-based extraction with HOST buffers (what a pyradiomics user holds):
-    int32 gray levels + mask in, float64 feature maps out, all transfers inside.  Pinned staging is
+    int32 gray levels + mask in, float64 (or `out_dtype` float32) feature maps out, all transfers inside.  Pinned staging is
     allocated once and reused.  The 80 GB of result maps is what bounds this path (PCIe), so the
     device->host stream is kept busy from the first milliseconds: classes run in order of
     (bytes out / compute time), every class is cut into z-chunks (class_maps_to_host), and a chunk's
