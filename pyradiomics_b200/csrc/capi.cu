@@ -102,6 +102,10 @@ int lbp2d_launch(const void* img, int dt, int Z, int Y, int X, int axis, int P, 
 int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
                       int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
                       double init_value, double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
+bool firstorder_fast_applicable(int level_bytes, int rz, int ry, int rx);
+int firstorder_fast_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
+                           int Z, int Y, int X, double shift, double voxel_volume, double init_value, double* out,
+                           long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
 static const char* kFirstOrderNames[] = {"10Percentile", "90Percentile", "Energy", "Entropy", "InterquartileRange", "Kurtosis",
   "Maximum", "MeanAbsoluteDeviation", "Mean", "Median", "Minimum", "Range", "RobustMeanAbsoluteDeviation", "RootMeanSquared",
   "Skewness", "TotalEnergy", "Uniformity", "Variance"};
@@ -476,6 +480,9 @@ int rb_firstorder_voxel_dev(const void* image_dev, int dtype, const uint8_t* mas
   if (int rc = check_dtypes({dtype})) return rc;
   if (level_bytes != 1 && level_bytes != 2) return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
   if (rz < 0 || ry < 0 || rx < 0 || z0 < 0 || z1 > Z || z0 > z1) return fail(RB_ERR_ARG, "bad window / z range");
+  if (!force_generic() && firstorder_fast_applicable(level_bytes, rz, ry, rx))
+    return firstorder_fast_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, Z, Y, X, voxelArrayShift,
+                                  voxel_volume, initValue, out_dev, out_feature_stride, z0, z1, out_z0, (cudaStream_t)stream);
   return firstorder_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, level_bytes, Z, Y, X, rz, ry, rx,
                            voxelArrayShift, voxel_volume, initValue, out_dev, out_feature_stride, z0, z1, out_z0,
                            (cudaStream_t)stream);

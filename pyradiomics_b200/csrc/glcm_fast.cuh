@@ -19,14 +19,6 @@ using std::max;
 using std::min;
 #endif
 
-#ifdef __CUDA_ARCH__
-#define RB_CTZ(x) (__ffs((int)(x)) - 1)
-#define RB_POPC(x) __popc((unsigned)(x))
-#else
-#define RB_CTZ(x) __builtin_ctz((unsigned)(x))
-#define RB_POPC(x) __builtin_popcount((unsigned)(x))
-#endif
-
 #if (defined(__CUDA_ARCH__) || defined(RB_EMULATE_BLOCK)) && defined(RB_GLCM_BLOCK_SYNC)
 #define RB_ANGLE_SYNC() __syncthreads()
 #else

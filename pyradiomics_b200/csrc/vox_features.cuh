@@ -26,6 +26,15 @@
 #define RB_HDN inline
 #endif
 
+// bit tricks of the 27-bit window masks (RB_EQMASKS_27, straightline.inc)
+#ifdef __CUDA_ARCH__
+#define RB_CTZ(x) (__ffs((int)(x)) - 1)
+#define RB_POPC(x) __popc((unsigned)(x))
+#else
+#define RB_CTZ(x) __builtin_ctz((unsigned)(x))
+#define RB_POPC(x) __builtin_popcount((unsigned)(x))
+#endif
+
 namespace rb {
 
 constexpr int NA_MAX = 344;      // bidirectional offsets for distances subset of {1,2,3}

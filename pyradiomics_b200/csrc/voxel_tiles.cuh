@@ -16,8 +16,10 @@ struct ChunkVoxel {
   long long oi;        // index in the output maps, whose plane 0 is out_z0
 };
 
-// !live: a stand-in for a thread without a voxel, decoded as t = 0
-RB_HD ChunkVoxel chunk_voxel(const VoxParams& P, long long plane, int z0, int out_z0, long long t, bool live = true) {
+// !live: a stand-in for a thread without a voxel, decoded as t = 0.  Par: VoxParams, or any parameter block with the
+// volume's Z, Y, X and element strides sz, sy (first order's FoParams)
+template <typename Par>
+RB_HD ChunkVoxel chunk_voxel(const Par& P, long long plane, int z0, int out_z0, long long t, bool live = true) {
   ChunkVoxel v;
   v.z = z0 + (int)((live ? t : 0) / plane);
   v.rem = (int)((live ? t : 0) % plane);
@@ -42,9 +44,9 @@ RB_HD bool chunk_center(const L* lev, const uint8_t* centers, long long plane, c
 }
 
 // the 27 window levels of voxel (z, y, x) with volume index vi to w[p * ws], p in z, y, x order: zeros outside the
-// volume, all zeros unless `gate`.  Returns whether the window is full (gate and no zero level).
-template <typename W, typename L>
-RB_HD bool load_window27(const L* lev, const VoxParams& P, int z, int y, int x, long long vi, bool gate, W* w,
+// volume, all zeros unless `gate`.  Returns whether the window is full (gate and no zero level).  Par as chunk_voxel.
+template <typename W, typename L, typename Par>
+RB_HD bool load_window27(const L* lev, const Par& P, int z, int y, int x, long long vi, bool gate, W* w,
                          int ws) {
   bool full = gate;
   int p = 0;

@@ -574,41 +574,23 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
         return self._device.binned_host()
 
     def _window_radii(self):
-        r = int(self.settings.get("kernelRadius", 1))
         nd = self._rawImageArray.ndim
-        if self.masked:
-            m = self._centerMask
-            size = []
-            for d in range(m.ndim):
-                on = np.flatnonzero(m.any(axis=tuple(k for k in range(m.ndim) if k != d)))
-                size.append(int(on[-1] - on[0] + 1))
-            size = np.array(size)
-        else:
-            size = np.array(self._rawImageArray.shape)
-        rad = [int(min(r, s - 1)) for s in size]
-        if self.settings.get("force2D", False):
-            rad[self.settings.get("force2Ddimension", 0)] = 0
+        rad = voxel.firstorder_radii(self.settings.get("kernelRadius", 1), self._rawImageArray.shape,
+                                     self._centerMask if self.masked else None, self.settings.get("force2D", False),
+                                     self.settings.get("force2Ddimension", 0))
         return [0] * (3 - nd) + rad
 
     def _voxel_launch(self, lev):
-        """rb_firstorder_voxel_dev on the raw intensities (uploaded once), a chunk of planes per launch: every window reads
+        """voxel.firstorder_launch on the raw intensities (uploaded once), a chunk of planes per launch: every window reads
         the whole volume, so a chunk's maps are those of one whole-volume launch"""
         img = imageoperations._to_device(self._rawImageArray)
         msk = imageoperations._to_device(self.maskArray)
         if img.ndim == 2:
             img, msk = img[None], msk[None]
-        centers = self._centers_dev()
-        Z, Y, X = img.shape
-        rz, ry, rx = self._window_radii()
         vv = float(np.multiply.reduce(self.pixelSpacing))
-        ptr = _lib.ptr
-
-        def launch(za, zb, buf):
-            _lib.check(_lib.lib().rb_firstorder_voxel_dev(
-                ptr(img), _lib.TORCH_DTYPE_CODE[img.dtype], ptr(msk), ptr(centers), ptr(lev), voxel.level_bytes(lev), Z, Y, X,
-                rz, ry, rx, float(self.voxelArrayShift), vv, float(self.settings.get("initValue", 0)), ptr(buf), buf.stride(0),
-                za, zb, za, _lib.stream()), "firstorder")
-        return launch, None
+        return voxel.firstorder_launch(img.contiguous(), lev, msk, self._window_radii(), centers=self._centers_dev(),
+                                       voxelArrayShift=self.voxelArrayShift, voxel_volume=vv,
+                                       initValue=self.settings.get("initValue", 0)), None
 
     def _initCalculation(self, voxelCoordinates=None):
         pass

@@ -2,8 +2,8 @@
 
 * ``voxel_suite_with_filters`` -- Original + wavelet (8 sub-bands) + LoG (one per sigma) derived
   images (+ the square / squareroot / logarithm / exponential / gradient and 3-D LBP images on
-  request) -> per-image gray-level discretisation -> the five fused voxel-based texture kernels,
-  everything on one GPU without host round trips (what ``RadiomicsFeatureExtractor.execute(...,
+  request) -> per-image gray-level discretisation -> the five fused voxel-based texture kernels and,
+  on request, the first-order kernel on the image's own intensities, everything on one GPU without host round trips (what ``RadiomicsFeatureExtractor.execute(...,
   voxelBased=True)`` does image type by image type, reference radiomics/featureextractor.py:371-392).
 * ``segment_batch`` -- segment-based matrices + features for a list of independent cases, sharded
   round-robin over the ranks of the process group with no collective (the reference's own
@@ -71,11 +71,18 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
     derived image comes from the normalised one; `resegment` (a dict with resegmentRange, resegmentMode) then resegments
     the mask against that image, and binning, the texture kernels and the LBP 3-D ROI use the resegmented mask -- the
     reference's order (featureextractor.py:316-392).  None (default) skips either step.
+    `classes` are names out of CLASSES and "firstorder": the first-order maps of each derived image's own intensities,
+    with its packed levels and the (resegmented) ROI as the kernel mask (voxel.firstorder_features; kernelRadius,
+    force2D, force2Ddimension, voxelArrayShift and initValue from kw, the voxel volume from `spacing_zyx`).
     `consume(name, cls, maps)` is called with each [F,Z,Y,X] result of type `map_dtype` (float64, the reference's, or
     float32: half the device memory, so a 512^3 suite fits on one 80 GB GPU; maps are reused buffers unless consume
     keeps them); returns the list of (image name, Ng, number of levels)."""
     if map_dtype not in voxel.MAP_DTYPES:
         raise TypeError(f"voxel feature maps are float64 or float32, not {map_dtype}")
+    unknown = [c for c in classes if c not in CLASSES and c != "firstorder"]
+    if unknown:
+        raise ValueError(f"unknown voxel classes {unknown} (known: {CLASSES + ('firstorder',)})")
+    fo_kw = {k: kw[k] for k in ("kernelRadius", "force2D", "force2Ddimension", "voxelArrayShift", "initValue") if k in kw}
     if normalize is not None:
         image = IO.normalize_image_device(image, normalize.get("normalizeScale", 1), normalize.get("removeOutliers"))
     msk = (mask != 0).to(torch.uint8).contiguous()
@@ -86,14 +93,18 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
     info = []
     for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=msk, image_types=image_types,
                                     gradient_use_spacing=gradient_use_spacing):
-        _, _, lev, levels, Ng = voxel.discretize(img.contiguous(), msk, **kw)
+        img = img.contiguous()
+        _, _, lev, levels, Ng = voxel.discretize(img, msk, **kw)
         nlev = len(levels)
         s = _lib.make_settings(Ng, nlev, spacing_zyx=spacing_zyx, **kw)
         for c in classes:
-            nf = _lib.lib().rb_num_features(_lib.CLASS_ID[c])
+            nf = voxel.FIRSTORDER_NF if c == "firstorder" else _lib.lib().rb_num_features(_lib.CLASS_ID[c])
             if c not in outs:
                 outs[c] = torch.empty((nf,) + tuple(lev.shape), dtype=map_dtype, device=lev.device)
-            maps = voxel.voxel_features(c, lev, s, out=outs[c], out_z0=0)
+            if c == "firstorder":
+                maps = voxel.firstorder_features(img, lev, msk, spacing_zyx=spacing_zyx, out=outs[c], out_z0=0, **fo_kw)
+            else:
+                maps = voxel.voxel_features(c, lev, s, out=outs[c], out_z0=0)
             if consume is not None:
                 consume(name, c, maps)
         info.append((name, Ng, nlev))

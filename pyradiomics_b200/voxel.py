@@ -134,6 +134,109 @@ def extract_maps(image, mask, classes=CLASSES, **kw):
     return res
 
 
+FIRSTORDER_NF = 18
+
+
+def roi_extent(roi):
+    """per-axis size of the bounding box of the non-zero voxels of `roi` (an ndarray or a CUDA tensor, 2-D or 3-D)"""
+    if isinstance(roi, torch.Tensor):
+        on = roi != 0
+        first, last = [], []
+        for d in range(on.ndim):
+            proj = on.any(dim=tuple(k for k in range(on.ndim) if k != d))
+            idx = torch.nonzero(proj).flatten()
+            first.append(idx[0])
+            last.append(idx[-1])
+        return [int(v) for v in (torch.stack(last) - torch.stack(first) + 1).tolist()]
+    m = np.asarray(roi) != 0
+    size = []
+    for d in range(m.ndim):
+        on = np.flatnonzero(m.any(axis=tuple(k for k in range(m.ndim) if k != d)))
+        size.append(int(on[-1] - on[0] + 1))
+    return size
+
+
+def firstorder_radii(kernelRadius, shape, roi=None, force2D=False, force2Ddimension=0):
+    """The window radii of voxel-based first order, one per axis of `shape`, as the reference forms them: kernelRadius
+    clipped to the ROI's bounding-box size - 1 (`roi`: non-zero = in the ROI; None, an unmasked kernel: to the image
+    size - 1), 0 on the force2D axis."""
+    size = list(shape) if roi is None else roi_extent(roi)
+    rad = [int(min(int(kernelRadius), s - 1)) for s in size]
+    if force2D:
+        rad[int(force2Ddimension)] = 0
+    return rad
+
+
+def voxel_volume(spacing_zyx):
+    """the product of the voxel spacing, multiplied in x, y, z order as the reference's np.multiply.reduce(pixelSpacing)"""
+    return float(np.multiply.reduce(np.asarray(spacing_zyx, dtype=np.float64)[::-1]))
+
+
+def firstorder_launch(image, lev, kmask, radii, *, centers=None, voxelArrayShift=0, voxel_volume=1.0, initValue=0):
+    """the `launch(za, zb, buf, out_z0=za)` of rb_firstorder_voxel_dev: the first-order maps of planes [za,zb) of the
+    (Z,Y,X) volume into the float64 `buf` [18, ..., Y, X] (plane z at buf[:, z - out_z0]) on the current stream.
+    `image`: raw or derived intensities (any device pixel type), `lev`: packed levels (0 = not in the kernel), `kmask`:
+    the voxels that enter windows (None: every voxel), `centers`: the voxels that get maps (None: kmask), `radii`:
+    (rz, ry, rx)."""
+    Z, Y, X = lev.shape
+    assert image.shape == lev.shape and image.is_contiguous() and lev.is_contiguous()
+    assert kmask is None or (kmask.shape == lev.shape and kmask.dtype == torch.uint8 and kmask.is_contiguous())
+    assert centers is None or (centers.shape == lev.shape and centers.dtype == torch.uint8 and centers.is_contiguous())
+    rz, ry, rx = (int(r) for r in radii)
+
+    def launch(za, zb, buf, out_z0=None):
+        if buf.dtype != torch.float64:
+            raise TypeError(f"first-order maps leave the kernel as float64, not {buf.dtype}")
+        assert buf.shape[0] == FIRSTORDER_NF and buf.stride()[1:] == (Y * X, X, 1)
+        check(lib().rb_firstorder_voxel_dev(ptr(image), _lib.TORCH_DTYPE_CODE[image.dtype], ptr(kmask), ptr(centers), ptr(lev),
+                                            level_bytes(lev), Z, Y, X, rz, ry, rx, float(voxelArrayShift),
+                                            float(voxel_volume), float(initValue), ptr(buf), buf.stride(0), int(za), int(zb),
+                                            int(za if out_z0 is None else out_z0),
+                                            torch.cuda.current_stream(lev.device).cuda_stream), "firstorder")
+    return launch
+
+
+def firstorder_features(image: torch.Tensor, lev: torch.Tensor, roi, *, kernelRadius=1, force2D=False, force2Ddimension=0,
+                        voxelArrayShift=0, initValue=0, spacing_zyx=(1.0, 1.0, 1.0), centers=None, z0=0, z1=None, out=None,
+                        out_z0=None, dtype=torch.float64, zchunk=16):
+    """The device-resident first-order maps, the counterpart of voxel_features: planes [z0,z1) of the (Z,Y,X) CUDA
+    volumes `image` (raw or derived intensities, any device pixel type), `lev` (packed levels, 0 outside the ROI) and
+    `roi` (the kernel mask: the voxels that enter windows; None = every voxel, an unmasked kernel).  `centers` (CUDA,
+    non-zero = gets maps) defaults to `roi`; other voxels get `initValue`.  The radii follow firstorder_radii.
+    Returns `out`: [18, z1-z0, Y, X] in feature_names("firstorder") order, of type `dtype` (float64 or float32),
+    allocated when None; a given `out` decides the type by its dtype and has contiguous (Y, X) planes, plane z at
+    out[:, z - out_z0].  Float32 maps are the float64 maps rounded once: the kernel writes z-chunks of `zchunk` planes
+    into a float64 scratch that converts on the device.  Asynchronous on the current stream."""
+    Z, Y, X = lev.shape
+    z1 = Z if z1 is None else int(z1)
+    z0 = int(z0)
+    if out is None:
+        out = torch.empty((FIRSTORDER_NF, z1 - z0, Y, X), dtype=dtype, device=lev.device)
+        out_z0 = z0
+    f32 = out_is_f32(out)
+    assert out.shape[0] == FIRSTORDER_NF and out.shape[2:] == (Y, X) and out.stride()[1:] == (Y * X, X, 1)
+    out_z0 = z0 if out_z0 is None else int(out_z0)
+    image = image.contiguous()
+    kmask = None if roi is None else (roi != 0).to(torch.uint8).contiguous()
+    cen = None if centers is None else (centers != 0).to(torch.uint8).contiguous()
+    radii = firstorder_radii(kernelRadius, lev.shape, kmask, force2D, force2Ddimension)
+    launch = firstorder_launch(image, lev, kmask, radii, centers=cen, voxelArrayShift=voxelArrayShift,
+                               voxel_volume=voxel_volume(spacing_zyx), initValue=initValue)
+    if not f32:
+        launch(z0, z1, out, out_z0)
+        return out
+    plane = Y * X
+    zc = max(1, min(int(zchunk), z1 - z0))
+    scratch = torch.empty((FIRSTORDER_NF, zc, Y, X), dtype=torch.float64, device=lev.device)
+    st = torch.cuda.current_stream(lev.device).cuda_stream
+    for za in range(z0, z1, zc):
+        zb = min(za + zc, z1)
+        launch(za, zb, scratch, za)
+        check(lib().rb_maps_to_f32_dev(ptr(scratch), scratch.stride(0), out.data_ptr() + (za - out_z0) * plane * 4,
+                                       out.stride(0), (zb - za) * plane, FIRSTORDER_NF, st), "maps_to_f32")
+    return out
+
+
 def _runs(idx):
     """[(first feature index, count, position in idx)] for every run of consecutive indices"""
     out, k = [], 0
@@ -302,29 +405,45 @@ class HostExtractor:
 
 def extract_to_nrrd(lev: torch.Tensor, settings, out_dir, classes=CLASSES, prefix="original", spacing_xyz=(1.0, 1.0, 1.0),
                     origin_xyz=(0.0, 0.0, 0.0), compress=True, level=1, workers=8, out_dtype=torch.float64, centers=None,
-                    zchunk=64, features=None):
+                    zchunk=64, features=None, image=None, voxelArrayShift=0):
     """Voxel driver + output assembly in one pipeline (the reference: extractor.execute(..., voxelBased=True) then one
     sitk.WriteImage(map, target, True) per map, radiomics/scripts/voxel.py:62-72): the fused kernels of one class stream
     their maps chunk by chunk into page-locked host memory (class_maps_to_host) while a pool of writer threads gzips the
     PREVIOUS class's maps into <prefix>_<class>_<Feature>.nrrd files (zlib releases the GIL), so compression and disk
     overlap the GPU and the PCIe stream.  `features` = {class: [names]} restricts what is copied and written.
+    "firstorder" in `classes` also writes the first-order maps of `image` (the CUDA intensities `lev` was binned from;
+    `voxelArrayShift` as the reference's setting): its kernel mask is `lev != 0`, or every voxel when `centers` is given
+    (an unmasked kernel), its radii, force2D and initValue come from `settings`, the voxel volume from `spacing_xyz`.
     Returns {feature key: path}."""
     import concurrent.futures as cf
     import os
 
     from . import nrrd
+    fo_launch = None
+    if "firstorder" in classes:
+        if image is None:
+            raise ValueError("first-order maps need the intensity image (image=...)")
+        kmask = (lev != 0).to(torch.uint8) if centers is None else None
+        radii = firstorder_radii(settings.kernelRadius, lev.shape, kmask, settings.force2D, settings.force2Ddimension)
+        cen = None if centers is None else (centers != 0).to(torch.uint8).contiguous()
+        fo_launch = firstorder_launch(image.contiguous(), lev, kmask, radii, centers=cen, voxelArrayShift=voxelArrayShift,
+                                      voxel_volume=voxel_volume(tuple(spacing_xyz)[::-1]), initValue=settings.initValue)
     os.makedirs(out_dir, exist_ok=True)
     jobs, keep = {}, []
     copy_stream = torch.cuda.Stream(device=lev.device)
     with cf.ThreadPoolExecutor(max_workers=max(1, int(workers))) as ex:
-        for c in [c for c in HostExtractor.ORDER if c in classes]:
+        for c in [c for c in HostExtractor.ORDER if c in classes] + (["firstorder"] if fo_launch else []):
             names = _lib.feature_names(c)
             want = names if not features or c not in features else [n for n in names if n in set(features[c])]
             idx = [names.index(n) for n in want]
             if not idx:
                 continue
-            host = class_maps_to_host(c, lev, settings, idx, centers=centers, zchunk=zchunk, out_dtype=out_dtype,
-                                      copy_stream=copy_stream, sync=True)
+            if c == "firstorder":
+                host = maps_to_host(fo_launch, FIRSTORDER_NF, lev.shape, lev.device, idx, zchunk=zchunk, out_dtype=out_dtype,
+                                    copy_stream=copy_stream, sync=True)
+            else:
+                host = class_maps_to_host(c, lev, settings, idx, centers=centers, zchunk=zchunk, out_dtype=out_dtype,
+                                          copy_stream=copy_stream, sync=True)
             keep.append(host)
             arr = host.numpy()
             for pos, n in enumerate(want):
