@@ -360,6 +360,25 @@ int rb_firstorder_voxel_dev(const void *image_dev, int dtype, const uint8_t *mas
                             double voxelArrayShift, double voxel_volume, double initValue, double *out_dev,
                             long long out_feature_stride, int z0, int z1, int out_z0, void *stream);
 
+/* ---- segment-based first order: replaces the targetVoxelArray path of RadiomicsFirstOrder (reference
+ *      radiomics/firstorder.py:40-60 and the get*FeatureValue methods :62-474), which sorts, takes percentiles and
+ *      moments of the ROI vector and histograms its discretised levels on the host.
+ *   image_dev: raw or derived intensities (image_type an rb_dtype code; read as float64, like NumPy's astype(np.float64));
+ *   roi_dev: uint8 ROI mask (non-zero = in the ROI); levels_dev: the packed levels of rb_pack_levels_dev (level_bytes 1
+ *   or 2) for Entropy / Uniformity; all contiguous [Z][Y][X] (a 2-D image is Z = 1).  out18 (HOST) = the 18 features in
+ *   rb_firstorder_feature_name order.  Every launch runs on `stream`; the host is synchronised once, at the end.
+ *   The order statistics (Minimum, Maximum, Range, 10/90Percentile, InterquartileRange, Median) are exact: a radix select
+ *   on the float64 keys, interpolated like NumPy 2.x np.percentile (method "linear") and np.median, with -0.0 taken as
+ *   +0.0.  The sums are deterministic (block partials in a fixed order, no floating-point atomics), so repeated calls
+ *   give the same bits; they differ from NumPy's pairwise sums by summation order only.
+ *   Z, Y or X < 1 returns RB_ERR_ARG before any launch.  Whether the ROI holds a voxel is only known on the device: a
+ *   ROI without voxels runs the launches (each returns at once) and returns RB_ERR_ARG after the synchronisation;
+ *   voxel.firstorder_segment checks the ROI first and raises ValueError before any launch.
+ *   Intensities must be finite: voxel.discretize rejects a ROI with NaN or +-inf before this is called. */
+int rb_firstorder_segment_dev(const void *image_dev, int image_type, const uint8_t *roi_dev, const void *levels_dev,
+                              int level_bytes, int Z, int Y, int X, double voxelArrayShift, double voxel_volume,
+                              double *out18, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

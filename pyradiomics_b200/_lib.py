@@ -107,6 +107,7 @@ PROTOTYPES = {
     "rb_firstorder_num_features": (_i, []),
     "rb_firstorder_feature_name": (_s, [_i]),
     "rb_firstorder_voxel_dev": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _d, _d, _d, _p, _ll, _i, _i, _i, _p]),
+    "rb_firstorder_segment_dev": (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _d, _d, _p, _p]),
 }
 
 _lib = None

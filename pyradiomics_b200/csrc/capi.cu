@@ -106,6 +106,8 @@ bool firstorder_fast_applicable(int level_bytes, int rz, int ry, int rx);
 int firstorder_fast_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
                            int Z, int Y, int X, double shift, double voxel_volume, double init_value, double* out,
                            long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
+int firstorder_segment(const void* img, int dtype, const uint8_t* roi, const void* lev, int level_bytes, long long n,
+                       double shift, double voxel_volume, double* out18_host, cudaStream_t st);
 static const char* kFirstOrderNames[] = {"10Percentile", "90Percentile", "Energy", "Entropy", "InterquartileRange", "Kurtosis",
   "Maximum", "MeanAbsoluteDeviation", "Mean", "Median", "Minimum", "Range", "RobustMeanAbsoluteDeviation", "RootMeanSquared",
   "Skewness", "TotalEnergy", "Uniformity", "Variance"};
@@ -486,6 +488,17 @@ int rb_firstorder_voxel_dev(const void* image_dev, int dtype, const uint8_t* mas
   return firstorder_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, level_bytes, Z, Y, X, rz, ry, rx,
                            voxelArrayShift, voxel_volume, initValue, out_dev, out_feature_stride, z0, z1, out_z0,
                            (cudaStream_t)stream);
+}
+
+int rb_firstorder_segment_dev(const void* image_dev, int image_type, const uint8_t* roi_dev, const void* levels_dev,
+                              int level_bytes, int Z, int Y, int X, double voxelArrayShift, double voxel_volume,
+                              double* out18, void* stream) {
+  if (int rc = check_dtypes({image_type})) return rc;
+  if (level_bytes != 1 && level_bytes != 2) return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
+  if (!image_dev || !roi_dev || !levels_dev || !out18) return fail(RB_ERR_ARG, "first order: null argument");
+  if (Z < 1 || Y < 1 || X < 1) return fail(RB_ERR_ARG, "first order: the ROI is empty");
+  return firstorder_segment(image_dev, image_type, roi_dev, levels_dev, level_bytes, (long long)Z * Y * X, voxelArrayShift,
+                            voxel_volume, out18, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -127,6 +127,7 @@ class DeviceImage:
         self._binned_host = None
         self._alive = {}
         self._segment = {}
+        self._extent = None
 
     def binned_host(self):
         """the reference's ``self.imageArray`` after binning: int64 levels, 0 outside the ROI (lazy: voxel mode never needs it)"""
@@ -134,6 +135,12 @@ class DeviceImage:
             self._binned_host = self._lev32.cpu().numpy().astype(np.int64)
             self._lev32 = None
         return self._binned_host
+
+    def roi_extent(self):
+        """size of the ROI's bounding box per axis (voxel.roi_extent of the device mask; computed once)"""
+        if self._extent is None:
+            self._extent = tuple(voxel.roi_extent(self.mask_dev))
+        return self._extent
 
     def levels3d(self):
         return self.levels if self.levels.ndim == 3 else self.levels[None]
@@ -195,14 +202,7 @@ class RadiomicsFeaturesBase:
         self.logger.debug("Initializing feature class")
         if inputImage is None or inputMask is None:
             raise ValueError("Missing input image or mask")
-        self.progressReporter = getProgressReporter
-        self.settings = kwargs
-        self.label = kwargs.get("label", 1)
-        self.voxelBased = kwargs.get("voxelBased", False)
-        self.coefficients = {}
-        self.enabledFeatures = {}
-        self.featureValues = {}
-        self.featureNames = self.getFeatureNames()
+        self._configure(kwargs)
         self.inputImage = inputImage
         self.inputMask = inputMask
         self._rawImageArray = I.as_array(inputImage)
@@ -213,8 +213,46 @@ class RadiomicsFeaturesBase:
         self._maskArray = None
         self.masked = kwargs.get("maskedKernel", True) if self.voxelBased else True
         self._labelledVoxelCoordinates = None          # lazy: 3 x Nvox int64 (3.2 GB and seconds of np.where at 512^3)
-        setattr(self, self.MATRIX_ATTR, None)
         self._initBinning()
+
+    def _configure(self, kwargs):
+        """the state that comes from the settings alone (a class with settings of its own extends this)"""
+        self.progressReporter = getProgressReporter
+        self.settings = kwargs
+        self.label = kwargs.get("label", 1)
+        self.voxelBased = kwargs.get("voxelBased", False)
+        self.coefficients = {}
+        self.enabledFeatures = {}
+        self.featureValues = {}
+        self.featureNames = self.getFeatureNames()
+        self._spacing = None
+        setattr(self, self.MATRIX_ATTR, None)
+
+    # why from_device cannot build this class (None: it can)
+    FROM_DEVICE_REFUSED = None
+
+    @classmethod
+    def from_device(cls, device, spacing_zyx, **kwargs):
+        """a segment-mode instance over `device`, a DeviceImage already on the GPU (built from CUDA tensors, e.g.
+        ``DeviceImage(img_t, roi_t, 1, True, settings)``): no host image or mask exists, `spacing_zyx` stands for the
+        image's spacing.  ``execute()`` then runs the same matrix post-processing, formulas and per-feature isolation
+        as an instance built from host images of the image cropped to the ROI's bounding box (the reference's flow): the
+        matrices see only ROI voxels, and GLRLM's run-length capacity is the box's largest extent.  The texture classes
+        support it; the others raise NotImplementedError."""
+        if cls.FROM_DEVICE_REFUSED:
+            raise NotImplementedError(f"{cls.__name__}.from_device: {cls.FROM_DEVICE_REFUSED}")
+        self = cls.__new__(cls)
+        self.logger = logging.getLogger("radiomics." + (cls.CLASS or "base"))
+        self._configure(dict(kwargs, voxelBased=False))
+        self.masked = True
+        self.inputImage = self.inputMask = self._rawImageArray = self._maskRaw = None
+        self._imageArray = self._labelMask = self._maskArray = self._labelledVoxelCoordinates = None
+        self._spacing = tuple(float(s) for s in spacing_zyx)
+        self._device = device
+        if device is not None:
+            self.coefficients["grayLevels"] = device.grayLevels
+            self.coefficients["Ng"] = device.Ng
+        return self
 
     # ---- discretisation on the GPU, shared by the classes that see the same image (reference base.py:119-125)
     def _initBinning(self):
@@ -292,7 +330,12 @@ class RadiomicsFeaturesBase:
         return self.featureValues
 
     def _spacing_zyx(self):
-        return tuple(I.spacing_xyz(self.inputImage))[::-1]
+        return self._spacing if self._spacing is not None else tuple(I.spacing_xyz(self.inputImage))[::-1]
+
+    def _image_shape(self):
+        """the shape of the image the matrices are built from: a from_device instance stands for the image cropped to
+        the ROI's bounding box"""
+        return tuple(self._rawImageArray.shape) if self._rawImageArray is not None else self._device.roi_extent()
 
     def _voxel_settings(self):
         kw = dict(self.settings)
@@ -363,18 +406,8 @@ class RadiomicsFeaturesBase:
 
     def _calculateSegment(self):
         self._initCalculation()
-        vals = self._segment_features()
-        for feature, enabled in self.enabledFeatures.items():
-            if not enabled:
-                continue
-            if self.featureNames.get(feature) and feature not in vals:
-                self.logger.debug("Feature %s is deprecated", feature)     # texture: the reference raises DeprecationWarning
-                continue
-            try:
-                self.featureValues[feature] = np.squeeze(np.float64(vals[feature]))
-            except Exception:                                  # per-feature isolation (base.py:271-273)
-                self.logger.error("FAILED: %s", feature, exc_info=True)
-                self.featureValues[feature] = np.nan
+        segment_feature_values(self._segment_features(), self.enabledFeatures, self.featureNames, self.logger,
+                               self.featureValues)
 
     def _initCalculation(self, voxelCoordinates=None):
         setattr(self, self.MATRIX_ATTR, self._calculateMatrix(voxelCoordinates))
@@ -397,6 +430,25 @@ class RadiomicsFeaturesBase:
         if getattr(self, self.MATRIX_ATTR) is None:
             self._initCalculation()
         return np.float64(self._segment_features()[name])
+
+
+def segment_feature_values(vals, enabledFeatures, featureNames, logger, out=None):
+    """the enabled features of a segment-mode class out of `vals` (its formulas' {name: value}) into `out` (a new dict
+    when None), in enabling order: deprecated ones without a value are skipped, a value that does not convert to a
+    float64 becomes NaN with a logged error (per-feature isolation, reference base.py:258-273)"""
+    out = {} if out is None else out
+    for feature, enabled in enabledFeatures.items():
+        if not enabled:
+            continue
+        if featureNames.get(feature) and feature not in vals:
+            logger.debug("Feature %s is deprecated", feature)     # texture: the reference raises DeprecationWarning
+            continue
+        try:
+            out[feature] = np.squeeze(np.float64(vals[feature]))
+        except Exception:                                  # per-feature isolation (base.py:271-273)
+            logger.error("FAILED: %s", feature, exc_info=True)
+            out[feature] = np.nan
+    return out
 
 
 def _add_feature_getters(cls, names, deprecated=(), computable_deprecated=()):
@@ -423,10 +475,10 @@ class RadiomicsGLCM(RadiomicsFeaturesBase):
     """Gray Level Co-occurrence Matrix features (reference radiomics/glcm.py)."""
     CLASS, MATRIX_ATTR = "glcm", "P_glcm"
 
-    def __init__(self, inputImage, inputMask, **kwargs):
+    def _configure(self, kwargs):
         self.symmetricalGLCM = kwargs.get("symmetricalGLCM", True)
         self.weightingNorm = kwargs.get("weightingNorm")
-        super().__init__(inputImage, inputMask, **kwargs)
+        super()._configure(kwargs)
 
     def _calculateMatrix(self, voxelCoordinates=None):
         f2, f2d = self._matrix_args()
@@ -453,15 +505,15 @@ class RadiomicsGLRLM(RadiomicsFeaturesBase):
     """Gray Level Run Length Matrix features (reference radiomics/glrlm.py)."""
     CLASS, MATRIX_ATTR = "glrlm", "P_glrlm"
 
-    def __init__(self, inputImage, inputMask, **kwargs):
+    def _configure(self, kwargs):
         self.weightingNorm = kwargs.get("weightingNorm")
-        super().__init__(inputImage, inputMask, **kwargs)
+        super()._configure(kwargs)
 
     def _calculateMatrix(self, voxelCoordinates=None):
         f2, f2d = self._matrix_args()
         if voxelCoordinates is None:
             P, angles = cmatrices.calculate_glrlm_device(self._device.levels, self.coefficients["Ng"],
-                                                         int(np.max(self._rawImageArray.shape)), f2, f2d)
+                                                         int(np.max(self._image_shape())), f2, f2d)
         else:
             P, angles = cmatrices.calculate_glrlm(self.imageArray, self.maskArray, self.coefficients["Ng"],
                                                   int(np.max(self.imageArray.shape)), f2, f2d, *self._batch_args(voxelCoordinates))
@@ -508,9 +560,9 @@ class RadiomicsGLDM(_SizeMatrixClass):
     """Gray Level Dependence Matrix features (reference radiomics/gldm.py)."""
     CLASS, MATRIX_ATTR, NAMES = "gldm", "P_gldm", MF.GLDM_NAMES
 
-    def __init__(self, inputImage, inputMask, **kwargs):
+    def _configure(self, kwargs):
         self.gldm_a = kwargs.get("gldm_a", 0)
-        super().__init__(inputImage, inputMask, **kwargs)
+        super()._configure(kwargs)
 
     def _calculateMatrix(self, voxelCoordinates=None):
         f2, f2d = self._matrix_args()
@@ -559,6 +611,7 @@ class RadiomicsFirstOrder(RadiomicsFeaturesBase):
     the other features; the reference indexes its unpadded discretised array with padded coordinates
     (firstorder.py:109), i.e. a window shifted by +kernelRadius, or raises IndexError."""
     CLASS, MATRIX_ATTR = "firstorder", "_unused_matrix"
+    FROM_DEVICE_REFUSED = "segment-mode first order of device tensors is voxel.firstorder_segment"
     NAMES = ["10Percentile", "90Percentile", "Energy", "Entropy", "InterquartileRange", "Kurtosis", "Maximum",
              "MeanAbsoluteDeviation", "Mean", "Median", "Minimum", "Range", "RobustMeanAbsoluteDeviation",
              "RootMeanSquared", "Skewness", "TotalEnergy", "Uniformity", "Variance"]
@@ -632,6 +685,7 @@ class _ShapeClass(RadiomicsFeaturesBase):
     shape.py:50-52 via base.py:66), no binning (shape ignores intensities), coefficients computed on first use"""
     MATRIX_ATTR = "_unused_matrix"
     VOXEL_BASED_ERROR = None
+    FROM_DEVICE_REFUSED = "shape2D is computed from a host mask only"
 
     def __init__(self, inputImage, inputMask, **kwargs):
         if kwargs.get("voxelBased", False):
@@ -665,13 +719,28 @@ class RadiomicsShape(_ShapeClass):
             raise AssertionError("Shape features are only available in 3D. If 2D, use shape2D instead")
         super().__init__(inputImage, inputMask, **kwargs)
 
+    FROM_DEVICE_REFUSED = None
+
+    @classmethod
+    def from_device(cls, roi, spacing_zyx, **kwargs):
+        """a segment-mode instance over the ROI `roi` (a 3-D CUDA tensor, non-zero = in the ROI; no host mask exists),
+        cropped to its bounding box as the reference's flow crops the mask before shape (cropToTumorMask)"""
+        self = super().from_device(None, spacing_zyx, **kwargs)
+        self._roi_dev = roi[voxel.roi_box(roi)]
+        return self
+
+    def _padded_mask_dev(self):
+        """the ROI padded with one plane of zeros on every side (shape.py:58-72), so every ROI voxel gets its 8 cubes,
+        as a uint8 CUDA tensor (a copy: the ROI mask stays as it is however often this is called)"""
+        roi = getattr(self, "_roi_dev", None)
+        if roi is not None:
+            return torch.nn.functional.pad((roi != 0).to(torch.uint8), (1, 1, 1, 1, 1, 1)).contiguous()
+        return imageoperations._to_device(np.pad(np.asarray(self.maskArray, dtype=np.uint8), 1))
+
     def _initCalculation(self, voxelCoordinates=None):
         from . import cshape
         self.pixelSpacing = np.array(self._spacing_zyx(), dtype=np.float64)
-        # pad with one plane of zeros on every side (shape.py:58-72): every ROI voxel gets its 8 cubes
-        # (a local copy: self.maskArray stays the ROI mask however often this is called)
-        padded = np.pad(np.asarray(self.maskArray, dtype=np.uint8), 1)
-        m_t = imageoperations._to_device(padded)
+        m_t = self._padded_mask_dev()
         self.SurfaceArea, self.Volume, self.diameters, self._n_vertices = cshape.coefficients_device(m_t, self.pixelSpacing)
         mom = cshape.moments_device(m_t)
         self._Np = mom[0]

@@ -5,11 +5,17 @@
   request) -> per-image gray-level discretisation -> the five fused voxel-based texture kernels and,
   on request, the first-order kernel on the image's own intensities, everything on one GPU without host round trips (what ``RadiomicsFeatureExtractor.execute(...,
   voxelBased=True)`` does image type by image type, reference radiomics/featureextractor.py:371-392).
+* ``segment_suite_with_filters`` -- the segment-based counterpart: shape of the ROI, then first order and the five
+  texture classes of every derived image, keyed like ``RadiomicsFeatureExtractor.execute()`` (voxelBased=False,
+  reference radiomics/featureextractor.py:302-396,485-604); only matrices and scalars leave the GPU.
 * ``segment_batch`` -- segment-based matrices + features for a list of independent cases, sharded
   round-robin over the ranks of the process group with no collective (the reference's own
   parallel model: one case per worker, radiomics/scripts/__init__.py:393-404).
 """
 from __future__ import annotations
+
+import collections
+import logging
 
 import torch
 
@@ -109,6 +115,58 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
                 consume(name, c, maps)
         info.append((name, Ng, nlev))
     return info
+
+
+def segment_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=("firstorder",) + CLASSES, shape=True,
+                               spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1", sigmas=(1.0, 2.0, 3.0), image_types=(),
+                               lbp3d=None, gradient_use_spacing=True, normalize=None, resegment=None,
+                               resegment_shape=False, label=1, **settings):
+    """Segment-based extraction over every image type on one GPU.  image: CUDA tensor (Z,Y,X) of raw intensities,
+    mask: CUDA label map; the ROI is ``mask == label``.  `normalize` / `resegment` as in voxel_suite_with_filters (first
+    normalisation, then resegmentation of the ROI against the normalised image, then the filters of derived_images, with
+    `wavelet`, `sigmas`, `image_types`, `gradient_use_spacing` and `lbp3d` as there).  `classes`: "firstorder" and names
+    out of CLASSES, in the order their features are wanted; binning, distances, symmetricalGLCM, weightingNorm, gldm_a,
+    force2D, force2Ddimension and voxelArrayShift come from `settings`.
+    Returns an ordered dict keyed like RadiomicsFeatureExtractor.execute() without the diagnostics: first
+    ``original_shape_<F>`` (when `shape`; of the label ROI, or of the resegmented one with `resegment_shape`), then
+    ``<image type>_<class>_<F>`` for every derived image and class, each class's features in the order its plugin
+    class's execute() gives them.  The texture features come from the plugin classes themselves (from_device) over the
+    image's device-resident levels, first order from voxel.firstorder_segment.  Nothing is cropped: every matrix and the
+    first-order reduction see the ROI voxels only, and GLRLM's run-length capacity and the shape mesh are those of the
+    ROI's bounding box, so the values are those of the reference's crop to that box.  ValueError for an unknown class or an empty ROI."""
+    unknown = [c for c in classes if c not in CLASSES and c != "firstorder"]
+    if unknown:
+        raise ValueError(f"unknown segment classes {unknown} (known: {('firstorder',) + CLASSES})")
+    if normalize is not None:
+        image = IO.normalize_image_device(image, normalize.get("normalizeScale", 1), normalize.get("removeOutliers"))
+    roi = (mask == label).to(torch.uint8).contiguous()
+    shape_roi = roi
+    if resegment is not None:
+        roi, _, _ = IO.resegment_mask_device(image, roi, resegment["resegmentRange"], resegment.get("resegmentMode", "absolute"))
+        if resegment_shape:
+            shape_roi = roi
+    if not bool(roi.any()) or not bool(shape_roi.any()):
+        raise ValueError("the ROI is empty")
+    out = collections.OrderedDict()
+    if shape:
+        for f, v in FC.RadiomicsShape.from_device(shape_roi, spacing_zyx, **settings).execute().items():
+            out[f"original_shape_{f}"] = v
+    fo_names = FC.RadiomicsFirstOrder.getFeatureNames()
+    fo_enabled = {n: True for n, deprecated in fo_names.items() if not deprecated}      # what enableAllFeatures enables
+    for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=roi, image_types=image_types,
+                                    gradient_use_spacing=gradient_use_spacing):
+        img = img.contiguous()
+        dev = FC.DeviceImage(img, roi, 1, True, settings)
+        for c in classes:
+            if c == "firstorder":
+                vals = voxel.firstorder_segment(img, dev.levels, roi, voxelArrayShift=settings.get("voxelArrayShift", 0),
+                                                spacing_zyx=spacing_zyx)
+                feats = FC.segment_feature_values(vals, fo_enabled, fo_names, logging.getLogger("radiomics.firstorder"))
+            else:
+                feats = FC.FEATURE_CLASSES[c].from_device(dev, spacing_zyx, **settings).execute()
+            for f, v in feats.items():
+                out[f"{name}_{c}_{f}"] = v
+    return out
 
 
 def segment_batch(cases, classes=tuple(FC.FEATURE_CLASSES), rank=0, world=1, **kw):

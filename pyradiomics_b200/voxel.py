@@ -137,17 +137,22 @@ def extract_maps(image, mask, classes=CLASSES, **kw):
 FIRSTORDER_NF = 18
 
 
+def roi_box(roi: torch.Tensor):
+    """the bounding box of the non-zero voxels of the CUDA tensor `roi` as a tuple of slices (one host copy)"""
+    on = roi != 0
+    first, last = [], []
+    for d in range(on.ndim):
+        idx = torch.nonzero(on.any(dim=tuple(k for k in range(on.ndim) if k != d))).flatten()
+        first.append(idx[0])
+        last.append(idx[-1])
+    lo, hi = torch.stack([torch.stack(first), torch.stack(last)]).tolist()
+    return tuple(slice(int(a), int(b) + 1) for a, b in zip(lo, hi))
+
+
 def roi_extent(roi):
     """per-axis size of the bounding box of the non-zero voxels of `roi` (an ndarray or a CUDA tensor, 2-D or 3-D)"""
     if isinstance(roi, torch.Tensor):
-        on = roi != 0
-        first, last = [], []
-        for d in range(on.ndim):
-            proj = on.any(dim=tuple(k for k in range(on.ndim) if k != d))
-            idx = torch.nonzero(proj).flatten()
-            first.append(idx[0])
-            last.append(idx[-1])
-        return [int(v) for v in (torch.stack(last) - torch.stack(first) + 1).tolist()]
+        return [s.stop - s.start for s in roi_box(roi)]
     m = np.asarray(roi) != 0
     size = []
     for d in range(m.ndim):
@@ -235,6 +240,27 @@ def firstorder_features(image: torch.Tensor, lev: torch.Tensor, roi, *, kernelRa
         check(lib().rb_maps_to_f32_dev(ptr(scratch), scratch.stride(0), out.data_ptr() + (za - out_z0) * plane * 4,
                                        out.stride(0), (zb - za) * plane, FIRSTORDER_NF, st), "maps_to_f32")
     return out
+
+
+def firstorder_segment(image: torch.Tensor, lev: torch.Tensor, roi: torch.Tensor, *, voxelArrayShift=0,
+                       spacing_zyx=(1.0, 1.0, 1.0)):
+    """Segment-based first order on the device, the counterpart of firstorder_features: the 18 features of the ROI
+    (`roi` non-zero) of the CUDA intensities `image` (raw or derived, any device pixel type), with Entropy / Uniformity
+    from the packed levels `lev` (rb_pack_levels_dev, e.g. discretize's), all of one 2-D or 3-D shape.  Runs on the
+    current stream with no host copy of the volumes (rb_firstorder_segment_dev) and returns {feature: np.float64} in
+    feature_names("firstorder") order.  ValueError for an empty ROI."""
+    assert image.is_cuda and lev.is_cuda and roi.is_cuda and image.shape == lev.shape == roi.shape and image.ndim in (2, 3)
+    Z, Y, X = ((1,) + tuple(image.shape)) if image.ndim == 2 else tuple(image.shape)
+    image = image.contiguous()
+    lev = lev.contiguous()
+    roi = (roi != 0).to(torch.uint8).contiguous()
+    if not bool(roi.any()):                  # before any launch of the reduction (it would only report it at its end)
+        raise ValueError("first order: the ROI is empty")
+    out = (C.c_double * FIRSTORDER_NF)()
+    check(lib().rb_firstorder_segment_dev(ptr(image), _lib.TORCH_DTYPE_CODE[image.dtype], ptr(roi), ptr(lev),
+                                          level_bytes(lev), Z, Y, X, float(voxelArrayShift), voxel_volume(spacing_zyx), out,
+                                          torch.cuda.current_stream(lev.device).cuda_stream), "firstorder")
+    return {n: np.float64(out[k]) for k, n in enumerate(_lib.feature_names("firstorder"))}
 
 
 def _runs(idx):

@@ -111,6 +111,15 @@ if "firstorder" in fams:
     raw = (vols["smooth"].astype(np.float64) - 1) * 25 + rng.random(mask_full.shape) * 20
     r = FC.RadiomicsFirstOrder(raw, mask_rag.astype(np.int32), voxelBased=True, binWidth=25).execute()
     print("firstorder ok", len(r), flush=True)
+    # segment mode (rb_firstorder_segment_dev): 8-bit levels on the ragged ROI, 16-bit levels, a sparse ROI of 3 voxels
+    sparse = np.zeros(mask_full.shape, bool)
+    sparse.reshape(-1)[[0, mask_full.size // 2, mask_full.size - 1]] = True
+    img_t = torch.from_numpy(raw).cuda()
+    for m, bw in ((mask_rag, 25), (mask_rag, 0.05), (sparse, 25)):
+        m_t = torch.from_numpy(m.astype(np.uint8)).cuda()
+        _, _, lev, _, _ = voxel.discretize(img_t, m_t, binWidth=bw)
+        f = voxel.firstorder_segment(img_t, lev, m_t, voxelArrayShift=10)
+        print("firstorder segment ok", lev.dtype, f["Median"], flush=True)
 if "lbp3d" in fams:
     raw = ((vols["smooth"] - 1) * 25 + 3).astype(np.int16)
     for kw in ({}, {"lbp3DLevels": 4, "lbp3DIcosphereRadius": 1.5, "lbp3DIcosphereSubdivision": 2}):
