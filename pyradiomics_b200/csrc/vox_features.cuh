@@ -305,16 +305,60 @@ static RB_HDN void tridiag_extreme_pair(const TD* d, const TD* e, int n, double*
   *lo_out = dl ? xl : tridiag_kth_eigenvalue(dc, ec, n, 0, lo - 1e-9, hi + 1e-9, 40);
 }
 
-// Second-largest eigenvalue of a symmetric positive semi-definite matrix with spectrum in [0, 1+]
-// (the generic MCC path: A = M M^T).  n >= 2.
-static RB_HDN double sym_psd_second_largest(double* A, int n, int ld, double* d, double* e) {
-  if (n == 2) {                        // closed form: the two roots of the characteristic quadratic
-    const double tr = A[0] + A[ld + 1], det = A[0] * A[ld + 1] - A[ld] * A[ld];
-    const double disc = sqrt(fmax(tr * tr - 4.0 * det, 0.0));
-    return 0.5 * (tr - disc);
+// Second-largest singular value of the m x n matrix A (row-major, leading dimension ld, m >= n >= 2,
+// singular values in [0, 1+]; destroyed) -- the generic MCC path of an asymmetric GLCM.  Householder
+// reflections from the left and the right reduce A to upper bidiagonal form (diagonal d[0..n-1],
+// super-diagonal e[0..n-2]) with the same singular values; the Golub-Kahan tridiagonal of size 2n (zero
+// diagonal, off-diagonals d0, e0, d1, e1, ..., d_{n-1}) has eigenvalues +-sigma_i, so sigma_2 is its
+// (2n-2)-th smallest eigenvalue.  No M M^T is formed: a small sigma_2 keeps an absolute error of ~eps
+// instead of ~sqrt(eps).  The tridiagonal is built in A's first 4n entries once the reduction is done.
+static RB_HDN double second_singular_value(double* A, int m, int n, int ld, double* d, double* e) {
+  for (int k = 0; k < n; k++) {
+    // left reflection: zero A[k+1..m-1][k]
+    double s = 0;
+    for (int i = k; i < m; i++) s += A[i * ld + k] * A[i * ld + k];
+    if (s == 0) {
+      d[k] = 0;
+    } else {
+      const double a = A[k * ld + k], alpha = a >= 0 ? -sqrt(s) : sqrt(s);
+      const double vtv = 2.0 * (s - a * alpha);             // |x - alpha e_1|^2
+      A[k * ld + k] = a - alpha;
+      for (int j = k + 1; j < n; j++) {
+        double t = 0;
+        for (int i = k; i < m; i++) t += A[i * ld + k] * A[i * ld + j];
+        t *= 2.0 / vtv;
+        for (int i = k; i < m; i++) A[i * ld + j] -= t * A[i * ld + k];
+      }
+      d[k] = alpha;
+    }
+    if (k + 1 >= n) break;
+    // right reflection: zero A[k][k+2..n-1]
+    s = 0;
+    for (int j = k + 1; j < n; j++) s += A[k * ld + j] * A[k * ld + j];
+    if (s == 0) {
+      e[k] = 0;
+    } else {
+      const double a = A[k * ld + k + 1], beta = a >= 0 ? -sqrt(s) : sqrt(s);
+      const double vtv = 2.0 * (s - a * beta);
+      A[k * ld + k + 1] = a - beta;
+      for (int i = k + 1; i < m; i++) {
+        double t = 0;
+        for (int j = k + 1; j < n; j++) t += A[k * ld + j] * A[i * ld + j];
+        t *= 2.0 / vtv;
+        for (int j = k + 1; j < n; j++) A[i * ld + j] -= t * A[k * ld + j];
+      }
+      e[k] = beta;
+    }
   }
-  sym_tridiagonalize(A, n, ld, d, e);
-  return tridiag_kth_eigenvalue(d, e, n, n - 2, -1e-6, 1.0 + 1e-6, 46);
+  double* td = A;
+  double* te = A + 2 * n;
+  for (int i = 0; i < 2 * n; i++) td[i] = 0;
+  te[0] = 0;
+  for (int i = 0; i < n; i++) {
+    te[2 * i + 1] = d[i];
+    if (i + 1 < n) te[2 * i + 2] = e[i];
+  }
+  return tridiag_kth_eigenvalue(td, te, 2 * n, 2 * n - 2, -1e-6, 1.0 + 1e-6, 46);
 }
 
 // Second-largest |eigenvalue| of a symmetric matrix with spectrum in [-1, 1] (the fast MCC path,
@@ -416,7 +460,9 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
   uint16_t ridx[NCAP], cidx[NCAP];
   int nr = 0, nc = 0;
   for (int k = 0; k < n; k++) { ridx[k] = px[k] > 0 ? (uint16_t)nr++ : NOLEV; cidx[k] = py[k] > 0 ? (uint16_t)nc++ : NOLEV; }
-  if (nr < 2) { f[G_MCC] = 0.0; return true; }  // eigenvalues {1,0,...}: second largest is 0
+  // one row or one column level (an asymmetric GLCM may have one and not the other): M has rank 1, Q's eigenvalues are
+  // {1, 0, ...}, the second largest is 0 -- before the capacity rule, which only a solve needs
+  if (nr < 2 || nc < 2) { f[G_MCC] = 0.0; return true; }
   {
     uint16_t parent[2 * NCAP];
     for (int k = 0; k < nr + nc; k++) parent[k] = (uint16_t)k;
@@ -430,11 +476,12 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
     for (int k = 0; k < nr + nc; k++) if (parent[k] == k) comps++;
     if (comps >= 2) { f[G_MCC] = 1.0; return true; }
   }
-  if (nr > NJCAP) { f[G_MCC] = NAN; if (status) *status |= 1; return true; }
+  // capacity: M is nr x nc (nr == nc for a symmetric GLCM) and must fit the NJCAP x NJCAP local array
+  if (nr > NJCAP || nc > NJCAP) { f[G_MCC] = NAN; if (status) *status |= 1; return true; }
   double A[NJCAP * NJCAP];
   double dd[NJCAP], ee[NJCAP];
-  for (int k = 0; k < nr * nr; k++) A[k] = 0;
   if (P.symmetric) {
+    for (int k = 0; k < nr * nr; k++) A[k] = 0;
     // symmetric P (px = py): M = P / sqrt(px_i px_j + eps) is itself symmetric, its singular values are the |eigenvalues|
     // of M, so MCC is M's second largest |eigenvalue|, solved for directly.  (sqrt of the second eigenvalue of M M^T
     // squares it first: an absolute rounding of eps in a small eigenvalue of M M^T becomes ~sqrt(eps) in MCC.)
@@ -445,18 +492,17 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
     f[G_MCC] = sym_second_largest_abs(A, nr, nr, dd, ee);
     return true;
   }
-  for (int e1 = 0; e1 < E.n; e1++) {
-    int l1 = E.key[e1] >> 16, c1 = E.key[e1] & 0xFFFF;
-    double m1 = ((double)E.w[e1] / S) / sqrt(px[l1] * py[c1] + EPS);
-    for (int e2 = 0; e2 < E.n; e2++) {
-      if ((int)(E.key[e2] & 0xFFFF) != c1) continue;
-      int l2 = E.key[e2] >> 16;
-      double m2 = ((double)E.w[e2] / S) / sqrt(px[l2] * py[c1] + EPS);
-      A[ridx[l1] * nr + ridx[l2]] += m1 * m2;
-    }
+  // asymmetric: MCC = sqrt(lambda_2(Q)) = sigma_2(M), M = P / sqrt(px py + eps) of nr rows and nc columns, solved on
+  // the taller orientation (m = max(nr, nc) rows; both are >= 2 here).
+  const bool tall = nr >= nc;
+  const int m = tall ? nr : nc, nn = tall ? nc : nr;
+  for (int k = 0; k < m * nn; k++) A[k] = 0;
+  for (int e = 0; e < E.n; e++) {
+    const int li = E.key[e] >> 16, lj = E.key[e] & 0xFFFF;
+    const double v = ((double)E.w[e] / S) / sqrt(px[li] * py[lj] + EPS);
+    if (tall) A[ridx[li] * nn + cidx[lj]] = v; else A[cidx[lj] * nn + ridx[li]] = v;
   }
-  const double l2 = sym_psd_second_largest(A, nr, nr, dd, ee);
-  f[G_MCC] = sqrt(l2 > 0 ? l2 : 0.0);
+  f[G_MCC] = second_singular_value(A, m, nn, nn, dd, ee);
   return true;
 }
 

@@ -45,7 +45,7 @@ if "generic" in fams:
     n = min(N, 12)
     lev = vols["smooth"][:n, :n, :n]
     for kw in ({}, {"kernelRadius": 2, "distances": [1, 2]}, {"weightingNorm": "euclidean"}, {"symmetricalGLCM": False},
-               {"force2D": True, "force2Ddimension": 0}):
+               {"kernelRadius": 3, "symmetricalGLCM": False}, {"force2D": True, "force2Ddimension": 0}):
         res = voxel.extract_maps(lev, mask_rag[:n, :n, :n], **kw)
         torch.cuda.synchronize()
         print("generic", kw, "ok", flush=True)

@@ -196,3 +196,27 @@ extern "C" int emul_glcm_graph_scan(const uint8_t* w27, int dsh, uint32_t lo_mas
   glcm_graph_scan(e, 1, EA, dsh, EA | (EA << dsh), selfpair != 0, &connected, &bipartite);
   return (connected ? 2 : 0) | (bipartite ? 1 : 0);
 }
+
+// MCC of ONE GLCM given as a dense n x n matrix of counts or weights (rows / columns = levels 1..n) through
+// glcm_angle_features, the generic kernel's per-angle math (entry list of 2048, 343 levels, the 32-row dense solve);
+// *status receives its status bits (bit 0: over the dense solve's capacity)
+extern "C" double emul_glcm_matrix_mcc(const double* M, int n, int symmetric, int* status) {
+  if (n < 1 || n > 343) return NAN;
+  Entries<2048, double>* E = new Entries<2048, double>;
+  E->clear();
+  for (int i = 0; i < n; i++)
+    for (int j = 0; j < n; j++)
+      if (M[i * n + j] != 0) E->add(((uint32_t)i << 16) | (uint32_t)j, M[i * n + j]);
+  VoxParams* P = new VoxParams;
+  memset(P, 0, sizeof(*P));
+  P->Ng = n; P->n_roi_levels = n < 2 ? 2 : n; P->symmetric = symmetric;
+  int val[343];
+  for (int k = 0; k < n; k++) val[k] = k + 1;
+  double f[GLCM_NF];
+  int st = 0;
+  const bool ok = glcm_angle_features<2048, 343, 32, double>(*E, n, val, *P, f, &st);
+  if (status) *status = st;
+  delete E;
+  delete P;
+  return ok ? f[G_MCC] : NAN;
+}
