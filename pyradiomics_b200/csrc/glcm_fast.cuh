@@ -414,7 +414,7 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
   // the diagonal).
   double rl = 0, lgE = 0;
   int E2 = 0, cmax = 0;
-  uint32_t reps = 0, all = 0, comp = 0;
+  uint32_t reps = 0, all = 0, comp = 0, ereps = 0;
   uint32_t em[NP];
 #pragma unroll
   for (int t = 0; t < NP; t++) {
@@ -426,7 +426,9 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
       em[t] = ea | eb;
       all |= em[t];
       if (!comp) comp = em[t];
-      const int c = RB_POPC(((ea & (eb >> dsh)) | (eb & (ea >> dsh))) & EA);
+      const uint32_t same = ((ea & (eb >> dsh)) | (eb & (ea >> dsh))) & EA;   // lower ends of the pairs equal to pair t
+      ereps |= same & (0u - same);                          // lowest one: one bit per distinct level pair (graph edge)
+      const int c = RB_POPC(same);
       const int cc = ea == eb ? 2 * c : c;                  // count of the matrix entry (a pair (i, i) adds 2)
       lgE += T.log2t[cc];
       E2 += 2 * cc;
@@ -437,15 +439,20 @@ RB_HD void glcm_fast_angle(const uint8_t* w, int ws, const uint32_t* eq, int es,
   // ---- MCC classification (glcm.py:679-707, see file header): several components -> 1; a connected bipartite
   // level graph (no level paired with itself, no odd cycle: 29 % of the connected graphs of i.i.d. uniform levels,
   // all trees among them) has the eigenvalue -1 next to +1 -> 1 without a solve; else an eigen-task for phase B.
+  // Counting settles most graphs first: a connected graph on nlev nodes has at least nlev - 1 distinct edges besides
+  // its self-loops, so a graph with at most nlev - 1 distinct level pairs (self-loops included) is either disconnected
+  // or a tree -- bipartite.  Both give 1 (nearly every face- and body-diagonal graph of i.i.d. levels, and the forests
+  // among the axis graphs); only the others take the sweep and the 2-colouring.
   double mcc;
   if (P.n_roi_levels < 2) mcc = 1.0;
   else if (nlev < 2) mcc = 0.0;
+  else if (RB_POPC(ereps) < nlev) mcc = 1.0;
   else {
     for (int sweep = 0; sweep < NP; sweep++) {
       const uint32_t before = comp;
 #pragma unroll
       for (int t = 0; t < NP; t++) if (em[t] & comp) comp |= em[t];
-      if (comp == before) break;
+      if (comp == before || comp == all) break;          // a fixed point, or every class reached: connected
     }
     bool bipartite = false;
     if (comp == all && !selfpair) {
