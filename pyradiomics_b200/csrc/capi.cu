@@ -32,17 +32,8 @@ int glcm_alive_angles(const void* lev, int level_bytes, const uint8_t* centers, 
                       cudaStream_t st);
 int pack_levels(const int32_t* image, const uint8_t* mask, long long n, int Ng, void* lev, uint32_t* presence,
                 int* status, cudaStream_t st);
-bool glcm_fast_applicable(int cls, int level_bytes, const VoxParams& P);
 int glcm_release_queues();
-int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
-                     int z0, int z1, int out_z0, cudaStream_t st);
-
-bool glrlm_fast_applicable(int cls, int level_bytes, const VoxParams& P);
-int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
-                      int z0, int z1, int out_z0, cudaStream_t st);
-
-bool small_fast_applicable(int cls, int level_bytes, const VoxParams& P);
-int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
+int voxel_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
                       long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
 
 // B200_RADIOMICS_FORCE_GENERIC=1 routes everything through the generic kernels (used by the
@@ -102,7 +93,6 @@ int lbp2d_launch(const void* img, int dt, int Z, int Y, int X, int axis, int P, 
 int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
                       int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
                       double init_value, double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
-bool firstorder_fast_applicable(int level_bytes, int rz, int ry, int rx);
 int firstorder_fast_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
                            int Z, int Y, int X, double shift, double voxel_volume, double init_value, double* out,
                            long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
@@ -207,14 +197,8 @@ int rb_voxel_features_dev(int cls, const void* levels_dev, int level_bytes, cons
   if (fill_vox_params(cls, Z, Y, X, *settings, P)) return fail(RB_ERR_ARG, "bad voxel settings");
   if (alive_host && cls == C_GLCM) memcpy(P.alive, alive_host, sizeof P.alive);
   const bool f32 = out_is_f32 != 0;
-  if (!force_generic() && glcm_fast_applicable(cls, level_bytes, P))
-    return glcm_fast_launch(levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
-                            (cudaStream_t)stream);
-  if (!force_generic() && small_fast_applicable(cls, level_bytes, P))
-    return small_fast_launch(cls, levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
-                             (cudaStream_t)stream);
-  if (!force_generic() && glrlm_fast_applicable(cls, level_bytes, P))
-    return glrlm_fast_launch(levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
+  if (!force_generic() && voxel_fast_path(cls, level_bytes, P))
+    return voxel_fast_launch(cls, levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
                              (cudaStream_t)stream);
   return voxel_features_generic(cls, levels_dev, level_bytes, centers_dev, P, out_dev, f32, out_feature_stride, z0,
                                 z1, out_z0, status_dev, (cudaStream_t)stream);
@@ -482,7 +466,7 @@ int rb_firstorder_voxel_dev(const void* image_dev, int dtype, const uint8_t* mas
   if (int rc = check_dtypes({dtype})) return rc;
   if (level_bytes != 1 && level_bytes != 2) return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
   if (rz < 0 || ry < 0 || rx < 0 || z0 < 0 || z1 > Z || z0 > z1) return fail(RB_ERR_ARG, "bad window / z range");
-  if (!force_generic() && firstorder_fast_applicable(level_bytes, rz, ry, rx))
+  if (!force_generic() && firstorder_fast_path(level_bytes, rz, ry, rx))
     return firstorder_fast_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, Z, Y, X, voxelArrayShift,
                                   voxel_volume, initValue, out_dev, out_feature_stride, z0, z1, out_z0, (cudaStream_t)stream);
   return firstorder_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, level_bytes, Z, Y, X, rz, ry, rx,

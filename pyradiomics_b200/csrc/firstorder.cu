@@ -153,10 +153,6 @@ static FoParams fo_params(int dtype, int level_bytes, int Z, int Y, int X, int r
                   init_value};
 }
 
-bool firstorder_fast_applicable(int level_bytes, int rz, int ry, int rx) {
-  return level_bytes == 1 && rz == 1 && ry == 1 && rx == 1;
-}
-
 int firstorder_fast_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
                            int Z, int Y, int X, double shift, double voxel_volume, double init_value, double* out,
                            long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {

@@ -206,7 +206,7 @@ __device__ __forceinline__ void glcm_phaseA_voxel(const uint8_t* w, uint32_t* eq
 
 // Phase A over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh).  The window bytes live in shared
 // memory, [27][NT].  (List entries are chunk indices: a chunk of 2^32 voxels would need a 1.3 TB eigen-task queue,
-// which glcm_fast_launch fails to allocate first.)
+// which glcm_fast_run fails to allocate first.)
 // OutT: the map type (store_map).  mcc_part: the chunk's float64 partial-MCC plane, float maps only.
 template <int MINB, int NT, typename OutT>
 __global__ void __launch_bounds__(NT, MINB)

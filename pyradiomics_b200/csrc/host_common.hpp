@@ -1,5 +1,5 @@
 // Host-side helpers shared by the C-ABI (capi.cu) and the test-only host emulation:
-// neighbour-offset ("angle") enumeration and the per-launch parameter block.
+// neighbour-offset ("angle") enumeration, the per-launch parameter block and the rule that picks the fast voxel kernels.
 #pragma once
 #include <math.h>
 #include <string.h>
@@ -117,5 +117,23 @@ inline int fill_vox_params(int cls, int Z, int Y, int X, const VoxSettings& s, V
 }
 
 inline int window_capacity(const VoxParams& P) { return (2 * P.rz + 1) * (2 * P.ry + 1) * (2 * P.rx + 1); }
+
+// Whether texture class cls runs its kernelRadius-1 fast kernel (voxel_fast_launch) rather than the generic one: 8-bit
+// levels and a 3x3x3 window, plus the angle set and weighting the class's fast body is written for.  The host
+// emulation takes the same decision.
+inline bool voxel_fast_path(int cls, int level_bytes, const VoxParams& P) {
+  if (level_bytes != 1 || P.rz != 1 || P.ry != 1 || P.rx != 1 || P.Ng > 255) return false;
+  switch (cls) {
+    case C_GLCM: return P.na == 13 && P.symmetric && !P.weighted;
+    case C_GLRLM: return P.na == 13 && !P.weighted;
+    case C_GLSZM: case C_GLDM: case C_NGTDM: return P.na == 26;
+    default: return false;
+  }
+}
+
+// the same for the first-order maps (firstorder_fast_launch): 8-bit levels and a 3x3x3 window
+inline bool firstorder_fast_path(int level_bytes, int rz, int ry, int rx) {
+  return level_bytes == 1 && rz == 1 && ry == 1 && rx == 1;
+}
 
 }  // namespace rb

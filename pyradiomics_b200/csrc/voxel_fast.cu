@@ -15,11 +15,6 @@
 
 namespace rb {
 
-bool glcm_fast_applicable(int cls, int level_bytes, const VoxParams& P) {
-  return cls == C_GLCM && level_bytes == 1 && P.rz == 1 && P.ry == 1 && P.rx == 1 && P.na == 13 && P.symmetric &&
-         !P.weighted && P.Ng <= 255;
-}
-
 // per (device, stream) task queue, grown on demand; float maps add the float64 partial-MCC plane of a chunk (mcc,
 // mcc_cap doubles)
 struct GlcmQueue {
@@ -65,7 +60,7 @@ static GlcmQueue* glcm_queue(cudaStream_t st, size_t need, size_t mcc_need) {
 }
 
 template <typename OutT>
-static int glcm_fast_run(const void* lev, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
+static int glcm_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
                          int z0, int z1, int out_z0, cudaStream_t st) {
   const GlcmFastTables* T = device_table<GlcmFastTables>([&](GlcmFastTables& h) { glcm_fast_build_tables(h, P.Ng); }, P.Ng);
   if (!T) return fail(RB_ERR_CUDA, "could not build the GLCM table block on the device");
@@ -92,7 +87,6 @@ static int glcm_fast_run(const void* lev, const uint8_t* centers, const VoxParam
   RB_CUDA(set_max_dynamic_smem(glcm_fast_kernel<1, NT, OutT>, smem));
   // register Lanczos: 90 KB of per-thread shared vectors per CTA -> two CTAs per SM
   RB_CUDA(set_max_dynamic_smem(glcm_fast_solve_kernel<2>, GF_LZ_SMEM_BYTES));
-  const uint8_t* l8 = (const uint8_t*)lev;
   for (int za = z0; za < z1; za += zchunk) {
     const int zb = za + zchunk < z1 ? za + zchunk : z1;
     RB_CUDA(cudaMemsetAsync(Q->count, 0, sizeof(unsigned), st));
@@ -114,12 +108,6 @@ static int glcm_fast_run(const void* lev, const uint8_t* centers, const VoxParam
     RB_LAUNCH_CHECK();
   }
   return RB_OK;
-}
-
-int glcm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
-                     int z0, int z1, int out_z0, cudaStream_t st) {
-  if (out_f32) return glcm_fast_run(lev, centers, P, (float*)out, fstride, z0, z1, out_z0, st);
-  return glcm_fast_run(lev, centers, P, (double*)out, fstride, z0, z1, out_z0, st);
 }
 
 // ---------------------------------------------------------------------------------- GLRLM
@@ -149,37 +137,48 @@ glrlm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
   }
 }
 
-bool glrlm_fast_applicable(int cls, int level_bytes, const VoxParams& P) {
-  return cls == C_GLRLM && level_bytes == 1 && P.rz == 1 && P.ry == 1 && P.rx == 1 && P.na == 13 && !P.weighted && P.Ng <= 255;
-}
-
-int glrlm_fast_launch(const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32, long long fstride,
-                      int z0, int z1, int out_z0, cudaStream_t st) {
+template <typename OutT>
+static int glrlm_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
+                          int z0, int z1, int out_z0, cudaStream_t st) {
   const GlrlmFastTables* T = device_table<GlrlmFastTables>(glrlm_fast_build_tables);
   if (!T) return fail(RB_ERR_CUDA, "could not build the GLRLM table block on the device");
   const long long total = (long long)(z1 - z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
-  const int grid = grid_for(total, 128, 32);
-  if (out_f32) glrlm_fast_kernel<<<grid, 128, 0, st>>>((const uint8_t*)lev, centers, P, T, (float*)out, fstride, z0, z1, out_z0);
-  else glrlm_fast_kernel<<<grid, 128, 0, st>>>((const uint8_t*)lev, centers, P, T, (double*)out, fstride, z0, z1, out_z0);
+  glrlm_fast_kernel<<<grid_for(total, 128, 32), 128, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
 
 // ------------------------------------------------------------------ GLSZM / GLDM / NGTDM fast paths
-// GLSZM and GLDM over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh), like NGTDM: a centre whose 27
-// window levels are all non-zero runs the class's FULL body in its tile, the other centres are drained through the
-// general body.  GLSZM's level classes live in per-thread shared scratch laid out [entry][thread].
+// One tile kernel over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh): a centre whose 27 window levels
+// are all non-zero runs the class's full-window body in its tile, the other centres are drained through its general
+// body.  Per class: the feature count, the block size NT and blocks per SM MINB (registers <= 65536 / (NT * MINB): 16
+// warps per SM), the per-thread shared scratch of the level classes, laid out [entry][thread], and the two bodies.
 template <int CLS> struct TileClass;
-template <> struct TileClass<C_GLSZM> { static constexpr int NF = GLSZM_NF, NMG = 13; };
-template <> struct TileClass<C_GLDM> { static constexpr int NF = GLDM_NF, NMG = 0; };
-
-template <int CLS, bool FULL>
-__device__ __forceinline__ void tile_body(const int* wl, const SmallFastTables& T, int alpha, unsigned long long* mg,
-                                          int st, double* f) {
-  if constexpr (CLS == C_GLSZM) glszm_fast_body<FULL>(wl, T, f, mg, st);
-  else gldm_fast_body<FULL>(wl, alpha, T, f);
-}
+template <> struct TileClass<C_GLSZM> {
+  static constexpr int NF = GLSZM_NF, NT = 128, MINB = 4;
+  struct Scratch { unsigned long long mg[13 * NT]; };                 // mask | level << 32 of each repeated level
+  template <bool FULL>
+  static __device__ __forceinline__ void body(const int* wl, const SmallFastTables& T, int, Scratch& s, int tid, double* f) {
+    glszm_fast_body<FULL>(wl, T, f, s.mg + tid, NT);
+  }
+};
+template <> struct TileClass<C_GLDM> {
+  static constexpr int NF = GLDM_NF, NT = 256, MINB = 2;
+  struct Scratch {};
+  template <bool FULL>
+  static __device__ __forceinline__ void body(const int* wl, const SmallFastTables& T, int alpha, Scratch&, int, double* f) {
+    gldm_fast_body<FULL>(wl, alpha, T, f);
+  }
+};
+template <> struct TileClass<C_NGTDM> {
+  static constexpr int NF = NGTDM_NF, NT = 128, MINB = 4;
+  struct Scratch { double ns[27 * NT]; int pk[27 * NT]; };            // per-class diff sums, then the compacted classes
+  template <bool FULL>
+  static __device__ __forceinline__ void body(const int* wl, const SmallFastTables& T, int, Scratch& s, int tid, double* f) {
+    ngtdm_fast_body<FULL>(wl, T, f, s.pk + tid, s.ns + tid, NT);
+  }
+};
 
 template <int CLS, int NT, int MINB, typename OutT>
 __global__ void __launch_bounds__(NT, MINB)
@@ -187,8 +186,9 @@ tiles_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
                   const SmallFastTables* __restrict__ Tg, OutT* __restrict__ out, long long fstride,
                   int z0, int z1, int out_z0) {
   using K = TileClass<CLS>;
+  static_assert(NT == K::NT && MINB == K::MINB, "the scratch is laid out for the class's block size");
   __shared__ SmallFastTables T;
-  __shared__ unsigned long long scr_mg[K::NMG * NT + 1];
+  __shared__ typename K::Scratch scr;
   __shared__ long long defer[2 * NT];                              // chunk indices of the centres left to the general body
   __shared__ unsigned ndefer;
   copy_tables_to_shared<NT>(T, Tg);
@@ -205,7 +205,7 @@ tiles_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
       const bool full = load_window27(lev, P, v.z, v.y, v.x, v.vi, is_center, wl, 1);
       if (full) {
         double f[K::NF];
-        tile_body<CLS, true>(wl, T, P.alpha, scr_mg + tid, NT, f);
+        K::template body<true>(wl, T, P.alpha, scr, tid, f);
 #pragma unroll
         for (int k = 0; k < K::NF; k++) store_map(out + k * fstride + v.oi, f[k]);
       } else if (is_center) {
@@ -221,103 +221,47 @@ tiles_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ c
       int wl[27];
       load_window27(lev, P, v.z, v.y, v.x, v.vi, true, wl, 1);
       double f[K::NF];
-      tile_body<CLS, false>(wl, T, P.alpha, scr_mg + tid, NT, f);
+      K::template body<false>(wl, T, P.alpha, scr, tid, f);
 #pragma unroll
       for (int k = 0; k < K::NF; k++) store_map(out + k * fstride + v.oi, f[k]);
     });
 }
 
-// block size and blocks per SM (registers <= 65536 / (NT * MINB): 16 warps per SM for both)
-constexpr int GLSZM_NT = 128, GLSZM_MINB = 4, GLDM_NT = 256, GLDM_MINB = 2;
-
-template <int CLS, int NT, int MINB, typename OutT>
-static int tiles_fast_launch(const SmallFastTables* T, const uint8_t* lev, const uint8_t* centers, const VoxParams& P,
-                             OutT* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
-  int grid = 0;
-  RB_CUDA(resident_grid(tiles_fast_kernel<CLS, NT, MINB, OutT>, NT, 0, (long long)(z1 - z0) * P.Y * P.X, grid));
-  tiles_fast_kernel<CLS, NT, MINB, OutT><<<grid, NT, 0, st>>>(lev, centers, P, T, out, fstride, z0, z1, out_z0);
-  RB_LAUNCH_CHECK();
-  return RB_OK;
-}
-
-// NGTDM over the full/deferred tiles of full_window_tiles (voxel_tiles.cuh).  Per-thread scratch for the level classes
-// lives in shared memory, [entry][thread].
-constexpr int NGTDM_NT = 128;
-template <int NT, typename OutT>
-__global__ void __launch_bounds__(NT, 4)
-ngtdm_fast_kernel(const uint8_t* __restrict__ lev, const uint8_t* __restrict__ centers,
-                  const __grid_constant__ VoxParams P, const SmallFastTables* __restrict__ Tg,
-                  OutT* __restrict__ out, long long fstride, int z0, int z1, int out_z0) {
-  __shared__ SmallFastTables T;
-  __shared__ double ng_ns[27 * NT];
-  __shared__ int ng_pk[27 * NT];
-  __shared__ long long defer[2 * NT];                              // chunk indices of the centres left to the general body
-  __shared__ unsigned ndefer;
-  copy_tables_to_shared<NT>(T, Tg);
-  const int tid = threadIdx.x;
-  if (tid == 0) ndefer = 0;
-  __syncthreads();
-  const long long plane = (long long)P.Y * P.X;
-  full_window_tiles<NT>((long long)(z1 - z0) * plane, defer, ndefer,
-    [&](long long t, bool live, auto defer_it) {
-      if (!live) return;
-      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, t);
-      const bool is_center = chunk_center(lev, centers, plane, v);
-      int wl[27];
-      load_window27(lev, P, v.z, v.y, v.x, v.vi, is_center, wl, 1);
-      if (is_center && window27_full(wl)) {
-        double f[NGTDM_NF];
-        ngtdm_fast_body<true>(wl, T, f, ng_pk + tid, ng_ns + tid, NT);
-#pragma unroll
-        for (int k = 0; k < NGTDM_NF; k++) store_map(out + k * fstride + v.oi, f[k]);
-      } else if (is_center) {
-        defer_it();
-      } else {
-#pragma unroll
-        for (int k = 0; k < NGTDM_NF; k++) store_map(out + k * fstride + v.oi, P.init_value);
-      }
-    },
-    [&](auto entry, bool live) {
-      if (!live) return;
-      const ChunkVoxel v = chunk_voxel(P, plane, z0, out_z0, entry());
-      const bool is_center = chunk_center(lev, centers, plane, v);
-      int wl[27];
-      load_window27(lev, P, v.z, v.y, v.x, v.vi, is_center, wl, 1);
-      double f[NGTDM_NF];
-      ngtdm_fast_body<false>(wl, T, f, ng_pk + tid, ng_ns + tid, NT);
-#pragma unroll
-      for (int k = 0; k < NGTDM_NF; k++) store_map(out + k * fstride + v.oi, f[k]);
-    });
-}
-
-bool small_fast_applicable(int cls, int level_bytes, const VoxParams& P) {
-  return (cls == C_GLSZM || cls == C_GLDM || cls == C_NGTDM) && level_bytes == 1 && P.rz == 1 && P.ry == 1 && P.rx == 1 &&
-         P.na == 26 && P.Ng <= 255;
-}
-
-template <typename OutT>
-static int small_fast_run(int cls, const SmallFastTables* T, const uint8_t* l8, const uint8_t* centers, const VoxParams& P,
-                          OutT* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
-  if (cls == C_NGTDM) {
-    int grid = 0;
-    RB_CUDA(resident_grid(ngtdm_fast_kernel<NGTDM_NT, OutT>, NGTDM_NT, 0, (long long)(z1 - z0) * P.Y * P.X, grid));
-    ngtdm_fast_kernel<NGTDM_NT, OutT><<<grid, NGTDM_NT, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-  }
-  if (cls == C_GLSZM) return tiles_fast_launch<C_GLSZM, GLSZM_NT, GLSZM_MINB>(T, l8, centers, P, out, fstride, z0, z1, out_z0, st);
-  return tiles_fast_launch<C_GLDM, GLDM_NT, GLDM_MINB>(T, l8, centers, P, out, fstride, z0, z1, out_z0, st);
-}
-
-int small_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
-                      long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
+template <int CLS, typename OutT>
+static int tiles_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
+                          int z0, int z1, int out_z0, cudaStream_t st) {
+  using K = TileClass<CLS>;
   const SmallFastTables* T = device_table<SmallFastTables>(small_fast_build_tables);
   if (!T) return fail(RB_ERR_CUDA, "could not build the table block on the device");
   const long long total = (long long)(z1 - z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
+  int grid = 0;
+  RB_CUDA(resident_grid(tiles_fast_kernel<CLS, K::NT, K::MINB, OutT>, K::NT, 0, total, grid));
+  tiles_fast_kernel<CLS, K::NT, K::MINB, OutT><<<grid, K::NT, 0, st>>>(l8, centers, P, T, out, fstride, z0, z1, out_z0);
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+
+// ------------------------------------------------------------------------------------ the entry
+template <typename OutT>
+static int fast_run(int cls, const uint8_t* l8, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
+                    int z0, int z1, int out_z0, cudaStream_t st) {
+  switch (cls) {
+    case C_GLCM: return glcm_fast_run(l8, centers, P, out, fstride, z0, z1, out_z0, st);
+    case C_GLRLM: return glrlm_fast_run(l8, centers, P, out, fstride, z0, z1, out_z0, st);
+    case C_GLSZM: return tiles_fast_run<C_GLSZM>(l8, centers, P, out, fstride, z0, z1, out_z0, st);
+    case C_GLDM: return tiles_fast_run<C_GLDM>(l8, centers, P, out, fstride, z0, z1, out_z0, st);
+    default: return tiles_fast_run<C_NGTDM>(l8, centers, P, out, fstride, z0, z1, out_z0, st);
+  }
+}
+
+// the fast kernels of class cls, for settings voxel_fast_path (host_common.hpp) accepts: `out` holds float maps when
+// out_f32, else double
+int voxel_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
+                      long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
   const uint8_t* l8 = (const uint8_t*)lev;
-  if (out_f32) return small_fast_run(cls, T, l8, centers, P, (float*)out, fstride, z0, z1, out_z0, st);
-  return small_fast_run(cls, T, l8, centers, P, (double*)out, fstride, z0, z1, out_z0, st);
+  if (out_f32) return fast_run(cls, l8, centers, P, (float*)out, fstride, z0, z1, out_z0, st);
+  return fast_run(cls, l8, centers, P, (double*)out, fstride, z0, z1, out_z0, st);
 }
 
 }  // namespace rb

@@ -98,17 +98,11 @@ def voxel_features(cls: str, lev: torch.Tensor, settings, *, centers=None, z0=0,
     if out is None:
         out = torch.empty((nf, z1 - z0, Y, X), dtype=dtype, device=lev.device)
         out_z0 = z0
-    f32 = out_is_f32(out)
+    out_is_f32(out)                          # TypeError for any other map type, before any launch
     assert out.shape[0] == nf and out.shape[2:] == (Y, X) and out.stride()[1:] == (Y * X, X, 1)
     if out_z0 is None:
         out_z0 = z0
-    if cls == "glcm" and alive is None:
-        alive = glcm_alive_angles(lev, settings, centers)
-    if status is None:
-        status = torch.zeros(1, dtype=torch.int32, device=lev.device)
-    check(lib().rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(z0), int(z1),
-                                      C.byref(settings), ptr(alive), ptr(out), f32, out.stride(0), int(out_z0), ptr(status),
-                                      stream()), cls)
+    texture_launch(cls, lev, settings, centers=centers, alive=alive, status=status)(z0, z1, out, out_z0)
     return out
 
 
@@ -276,8 +270,9 @@ def _runs(idx):
 
 
 def texture_launch(cls: str, lev: torch.Tensor, settings, *, centers=None, alive=None, status=None):
-    """the `launch(za, zb, buf)` of maps_to_host for the fused kernel of one texture class: planes [za,zb) of `lev` into
-    `buf` [F, >= zb-za, Y, X] (plane za at buf[:, 0], float64 or float32 maps as buf's dtype) on the current stream"""
+    """the `launch(za, zb, buf, out_z0=za)` of maps_to_host for the fused kernel of one texture class: planes [za,zb) of
+    `lev` into `buf` [F, ..., Y, X] (plane z at buf[:, z - out_z0], float64 or float32 maps as buf's dtype) on the current
+    stream"""
     cid = CLASS_ID[cls]
     Z, Y, X = lev.shape
     if cls == "glcm" and alive is None:
@@ -285,10 +280,11 @@ def texture_launch(cls: str, lev: torch.Tensor, settings, *, centers=None, alive
     if status is None:
         status = torch.zeros(1, dtype=torch.int32, device=lev.device)
 
-    def launch(za, zb, buf):
+    def launch(za, zb, buf, out_z0=None):
         check(lib().rb_voxel_features_dev(cid, ptr(lev), level_bytes(lev), ptr(centers), Z, Y, X, int(za), int(zb),
-                                          C.byref(settings), ptr(alive), ptr(buf), out_is_f32(buf), buf.stride(0), int(za),
-                                          ptr(status), torch.cuda.current_stream(lev.device).cuda_stream), cls)
+                                          C.byref(settings), ptr(alive), ptr(buf), out_is_f32(buf), buf.stride(0),
+                                          int(za if out_z0 is None else out_z0), ptr(status),
+                                          torch.cuda.current_stream(lev.device).cuda_stream), cls)
     return launch
 
 

@@ -45,30 +45,6 @@ extern "C" int emul_voxel_features(int cls, const uint16_t* lev, const uint8_t* 
   return status;
 }
 
-// GLCM fast path (r=1, 13 angles, symmetric, unweighted, 8-bit levels) on the host
-extern "C" int emul_glcm_fast(const uint16_t* lev, int Z, int Y, int X, const VoxSettings* s, const uint32_t* alive,
-                              double* out) {
-  VoxParams P;
-  int rc = fill_vox_params(C_GLCM, Z, Y, X, *s, P);
-  if (rc) return rc;
-  if (alive) for (int k = 0; k < (NW_MAX + 31) / 32; k++) P.alive[k] = alive[k];
-  if (P.na != 13 || P.rz != 1 || P.ry != 1 || P.rx != 1 || !P.symmetric || P.weighted || s->Ng > 255) return -5;
-  GlcmFastTables* T = new GlcmFastTables;
-  glcm_fast_build_tables(*T, s->Ng);
-  const long long nvox = (long long)Z * Y * X;
-  for (int z = 0; z < Z; z++) for (int y = 0; y < Y; y++) for (int x = 0; x < X; x++) {
-    long long i = ((long long)z * Y + y) * X + x;
-    if (!lev[i]) { for (int k = 0; k < GLCM_NF; k++) out[k * nvox + i] = P.init_value; continue; }
-    uint16_t w16[27]; uint8_t w[27]; uint32_t eq[27]; double f[GLCM_NF];
-    load_window<uint16_t>(lev, P, z, y, x, w16);
-    for (int k = 0; k < 27; k++) w[k] = (uint8_t)w16[k];
-    glcm_fast_voxel(w, 1, eq, 1, *T, P, f);
-    for (int k = 0; k < GLCM_NF; k++) out[k * nvox + i] = f[k];
-  }
-  delete T;
-  return 0;
-}
-
 #include "../../pyradiomics_b200/csrc/glrlm_fast.cuh"
 // MCC eigen-task of one 27-voxel window and angle slot through the dispatcher (dense register solve up to 12 levels,
 // register Lanczos above); cls < 0: derive it
@@ -92,51 +68,41 @@ extern "C" double emul_glcm_solve_window_cls(const uint8_t* w, int slot, int Ng,
   return r;
 }
 
-// GLRLM fast path (r=1, 13 angles, unweighted, 8-bit levels) on the host
-extern "C" int emul_glrlm_fast(const uint16_t* lev, int Z, int Y, int X, const VoxSettings* s, double* out) {
-  VoxParams P;
-  int rc = fill_vox_params(C_GLRLM, Z, Y, X, *s, P);
-  if (rc) return rc;
-  if (P.na != 13 || P.rz != 1 || P.ry != 1 || P.rx != 1 || P.weighted || s->Ng > 255) return -5;
-  GlrlmFastTables* T = new GlrlmFastTables;
-  glrlm_fast_build_tables(*T);
-  const long long nvox = (long long)Z * Y * X;
-  for (int z = 0; z < Z; z++) for (int y = 0; y < Y; y++) for (int x = 0; x < X; x++) {
-    long long i = ((long long)z * Y + y) * X + x;
-    if (!lev[i]) { for (int k = 0; k < GLRLM_NF; k++) out[k * nvox + i] = P.init_value; continue; }
-    uint16_t w16[27]; int wl[27]; double f[GLRLM_NF];
-    load_window<uint16_t>(lev, P, z, y, x, w16);
-    for (int k = 0; k < 27; k++) wl[k] = w16[k];
-    glrlm_fast_voxel(wl, *T, f);
-    for (int k = 0; k < GLRLM_NF; k++) out[k * nvox + i] = f[k];
-  }
-  delete T;
-  return 0;
-}
-
 #include "../../pyradiomics_b200/csrc/small_fast.cuh"
-// GLSZM / GLDM / NGTDM fast paths (r=1, 26-neighbourhood, 8-bit levels) on the host
-extern "C" int emul_small_fast(int cls, const uint16_t* lev, int Z, int Y, int X, const VoxSettings* s, double* out) {
+// The kernelRadius-1 fast path of class cls on the host: -5 when voxel_fast_path sends these settings to the generic
+// kernels, else every centre (non-zero level) through the class's per-voxel fast math.  alive: GLCM's alive angles
+// (NULL: all).
+extern "C" int emul_fast(int cls, const uint16_t* lev, int Z, int Y, int X, const VoxSettings* s, const uint32_t* alive,
+                         double* out) {
   VoxParams P;
   int rc = fill_vox_params(cls, Z, Y, X, *s, P);
   if (rc) return rc;
-  if (P.na != 26 || P.rz != 1 || P.ry != 1 || P.rx != 1 || s->Ng > 255) return -5;
-  SmallFastTables* T = new SmallFastTables;
-  small_fast_build_tables(*T);
+  if (alive) for (int k = 0; k < (NW_MAX + 31) / 32; k++) P.alive[k] = alive[k];
+  if (!voxel_fast_path(cls, s->Ng <= 255 ? 1 : 2, P)) return -5;     // the level width rb_level_bytes picks
+  GlcmFastTables* TC = cls == C_GLCM ? new GlcmFastTables : nullptr;
+  GlrlmFastTables* TR = cls == C_GLRLM ? new GlrlmFastTables : nullptr;
+  SmallFastTables* TS = cls >= C_GLSZM ? new SmallFastTables : nullptr;
+  if (TC) glcm_fast_build_tables(*TC, s->Ng);
+  if (TR) glrlm_fast_build_tables(*TR);
+  if (TS) small_fast_build_tables(*TS);
   const int nf = kNumFeatures[cls];
   const long long nvox = (long long)Z * Y * X;
   for (int z = 0; z < Z; z++) for (int y = 0; y < Y; y++) for (int x = 0; x < X; x++) {
     long long i = ((long long)z * Y + y) * X + x;
     if (!lev[i]) { for (int k = 0; k < nf; k++) out[k * nvox + i] = P.init_value; continue; }
-    uint16_t w16[27]; int wl[27]; double f[16];
+    uint16_t w16[27]; uint8_t w8[27]; uint32_t eq[27]; int wl[27]; double f[32];
     load_window<uint16_t>(lev, P, z, y, x, w16);
-    for (int k = 0; k < 27; k++) wl[k] = w16[k];
-    if (cls == C_GLSZM) glszm_fast_voxel(wl, *T, f);
-    else if (cls == C_GLDM) gldm_fast_voxel(wl, P.alpha, *T, f);
-    else ngtdm_fast_voxel(wl, *T, f);
+    for (int k = 0; k < 27; k++) { w8[k] = (uint8_t)w16[k]; wl[k] = w16[k]; }
+    switch (cls) {
+      case C_GLCM: glcm_fast_voxel(w8, 1, eq, 1, *TC, P, f); break;
+      case C_GLRLM: glrlm_fast_voxel(wl, *TR, f); break;
+      case C_GLSZM: glszm_fast_voxel(wl, *TS, f); break;
+      case C_GLDM: gldm_fast_voxel(wl, P.alpha, *TS, f); break;
+      case C_NGTDM: ngtdm_fast_voxel(wl, *TS, f); break;
+    }
     for (int k = 0; k < nf; k++) out[k * nvox + i] = f[k];
   }
-  delete T;
+  delete TC; delete TR; delete TS;
   return 0;
 }
 

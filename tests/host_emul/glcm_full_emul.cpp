@@ -10,7 +10,7 @@ using namespace rb;
 
 static int params(const VoxSettings* s, VoxParams& P) {
   if (fill_vox_params(C_GLCM, 3, 3, 3, *s, P)) return -1;
-  if (P.na != 13 || P.rz != 1 || P.ry != 1 || P.rx != 1 || !P.symmetric || P.weighted || s->Ng > 255) return -5;
+  if (!voxel_fast_path(C_GLCM, 1, P)) return -5;
   return 0;
 }
 

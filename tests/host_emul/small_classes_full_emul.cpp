@@ -16,7 +16,7 @@ extern "C" int emul_small_class_window(int cls, const uint8_t* w27, int body, co
   if (cls != C_GLSZM && cls != C_GLDM) return -1;
   VoxParams P;
   if (fill_vox_params(cls, 3, 3, 3, *s, P)) return -1;
-  if (P.na != 26 || P.rz != 1 || P.ry != 1 || P.rx != 1 || s->Ng > 255) return -5;
+  if (!voxel_fast_path(cls, 1, P)) return -5;
   int wl[27];
   bool full = true;
   for (int p = 0; p < 27; p++) { wl[p] = w27[p]; full &= w27[p] != 0; }

@@ -135,7 +135,7 @@ static void emu_launch(int nblocks, int nthreads, F body) {
   }
 }
 
-// The whole fused GLCM path of glcm_fast_launch on the CPU: phase A (256-thread blocks, per-angle barriers, queue
+// The whole fused GLCM path of glcm_fast_run on the CPU: phase A (256-thread blocks, per-angle barriers, queue
 // reservation by atomics), the three solve kernels, the finish kernel; planes [0, Z) in chunks of `zchunk`.
 // out: [24][Z][Y][X] float64.  Returns the total number of eigen-tasks.
 extern "C" long long emul_glcm_pipeline(const uint8_t* lev, int Z, int Y, int X, int Ng, int zchunk, double* out) {
@@ -158,7 +158,7 @@ extern "C" long long emul_glcm_pipeline(const uint8_t* lev, int Z, int Y, int X,
     GlcmTask* qp = q.data(); double* rp = res.data(); unsigned* cp = &count;
     emu_launch(3, 256, [=]() { glcm_fast_kernel<1, 256>(lev, nullptr, P, T, out, fstride, za, zb, 0, qp, cp); });
     for (unsigned k = 0; k < count; k++) res[k] = -12345.0;
-    // one launch per size group of the n <= 8 and Lanczos kinds and one for the whole n <= 12 kind: glcm_fast_launch
+    // one launch per size group of the n <= 8 and Lanczos kinds and one for the whole n <= 12 kind: glcm_fast_run
     // splits the dense kinds the other way round, so between them both paths of `only` run for both dense kinds
     for (int g = 4; g <= 8; g += 2) emu_launch(2, 128, [=]() { glcm_fast_solve_kernel<0>(lev, P, T, qp, cp, rp, g); });
     emu_launch(2, 128, [=]() { glcm_fast_solve_kernel<1>(lev, P, T, qp, cp, rp, 0); });

@@ -95,7 +95,7 @@ def test_planted_corpus_reaches_every_task_class():
 
 
 def _emulated_kernel_math_within_gpu_bounds(emul, Ng, path):
-    """the fast paths' math (emul_glcm_fast / emul_glrlm_fast / emul_small_fast) or the generic kernels' math
+    """the fast paths' math (emul_fast) or the generic kernels' math
     (emul_voxel_features) on a planted corpus against the window oracle, at the bounds of
     tests/test_fast_voxel_windows_gpu.py (helpers.window_bound, helpers.compare_window_maps)"""
     wins, _ = ng_corpus(planted_corpus(1500, seed=1), Ng, 400, np.random.default_rng(Ng))
@@ -113,12 +113,8 @@ def _emulated_kernel_math_within_gpu_bounds(emul, Ng, path):
             out = np.zeros((len(FAST_NAMES[cname]), Zs, Ys, Xs))
             if path == "generic":
                 rc = emul.emul_voxel_features(cid, p(lev), None, Zs, Ys, Xs, C.byref(s), p(alive), p(out))
-            elif cname == "glcm":
-                rc = emul.emul_glcm_fast(p(lev), Zs, Ys, Xs, C.byref(s), p(alive), p(out))
-            elif cname == "glrlm":
-                rc = emul.emul_glrlm_fast(p(lev), Zs, Ys, Xs, C.byref(s), p(out))
             else:
-                rc = emul.emul_small_fast(cid, p(lev), Zs, Ys, Xs, C.byref(s), p(out))
+                rc = emul.emul_fast(cid, p(lev), Zs, Ys, Xs, C.byref(s), p(alive), p(out))
             assert rc == 0
             compare_window_maps(out[(slice(None),) + tuple(cen.T)], refs, cname, a, f"Ng={Ng}/{path}/gldm_a={a}",
                                 path == "generic")

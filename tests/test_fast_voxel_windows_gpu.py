@@ -130,7 +130,7 @@ def _launch_rules(shape, sms):
     Z, Y, X = shape
     plane = Y * X
     total = Z * plane
-    zchunk = min(max((48 << 20) // (plane * 13), 1), Z)                 # glcm_fast_launch: max_entries / (plane * GF_NA)
+    zchunk = min(max((48 << 20) // (plane * 13), 1), Z)                 # glcm_fast_run: max_entries / (plane * GF_NA)
     chunks = [min(zchunk, Z - z) for z in range(0, Z, zchunk)]
 
     def grid_for(n, block, per_sm):                                     # common.cuh

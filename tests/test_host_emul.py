@@ -126,7 +126,7 @@ def test_glcm_fast_math_equals_generic_math_on_host(emul, kind):
     Zs, Ys, Xs = shape
     fast = np.zeros((24, Zs, Ys, Xs))
     gen = np.zeros((24, Zs, Ys, Xs))
-    assert emul.emul_glcm_fast(lev.ctypes.data_as(C.c_void_p), Zs, Ys, Xs, C.byref(s), None, fast.ctypes.data_as(C.c_void_p)) == 0
+    assert emul.emul_fast(0, lev.ctypes.data_as(C.c_void_p), Zs, Ys, Xs, C.byref(s), None, fast.ctypes.data_as(C.c_void_p)) == 0
     assert emul.emul_voxel_features(0, lev.ctypes.data_as(C.c_void_p), None, Zs, Ys, Xs, C.byref(s), None, gen.ctypes.data_as(C.c_void_p)) == 0
     for k, f in enumerate(NAMES["glcm"]):
         atol = 1e-6 if f in ("Imc2", "Imc1") else 1e-9
@@ -249,10 +249,7 @@ def test_glrlm_glszm_gldm_ngtdm_fast_math_equals_generic_math_on_host(emul, kind
             continue
         nf = len(NAMES[cname])
         fast, gen = np.zeros((nf, Zs, Ys, Xs)), np.zeros((nf, Zs, Ys, Xs))
-        if cname == "glrlm":
-            assert emul.emul_glrlm_fast(p(lev), Zs, Ys, Xs, C.byref(s), p(fast)) == 0
-        else:
-            assert emul.emul_small_fast(cid, p(lev), Zs, Ys, Xs, C.byref(s), p(fast)) == 0
+        assert emul.emul_fast(cid, p(lev), Zs, Ys, Xs, C.byref(s), None, p(fast)) == 0
         assert emul.emul_voxel_features(cid, p(lev), None, Zs, Ys, Xs, C.byref(s), None, p(gen)) == 0
         for k, f in enumerate(NAMES[cname]):
             assert np.allclose(fast[k], gen[k], rtol=1e-10, atol=1e-12, equal_nan=True), (cname, f, np.nanmax(np.abs(fast[k] - gen[k])))

@@ -49,8 +49,8 @@ def test_emulated_solve_kernels_process_every_task_once(kind, n):
 @pytest.mark.parametrize("kind,n", [("smooth", 12), ("uniform", 14)])
 def test_emulated_glcm_pipeline_equals_per_voxel_math(kind, n):
     """phase A kernel (per-angle barriers, atomic queue reservation, non-centre voxels) -> three solve kernels -> finish
-    kernel, in plane chunks like glcm_fast_launch, against the single-thread composition of the same math
-    (emul_glcm_fast, itself pinned on the reference's voxel-mode maps in test_host_emul.py)"""
+    kernel, in plane chunks like glcm_fast_run, against the single-thread composition of the same math
+    (emul_fast, itself pinned on the reference's voxel-mode maps in test_host_emul.py)"""
     from pyradiomics_b200 import _lib
     pipe = _solve_lib()
     pipe.emul_glcm_pipeline.restype = C.c_longlong
@@ -70,6 +70,6 @@ def test_emulated_glcm_pipeline_equals_per_voxel_math(kind, n):
     ref = np.zeros((24, n, n, n))
     s = _lib.make_settings(32, 32)
     lev16 = lev.astype(np.uint16)
-    assert emul.emul_glcm_fast(p(lev16), n, n, n, C.byref(s), None, p(ref)) == 0
+    assert emul.emul_fast(0, p(lev16), n, n, n, C.byref(s), None, p(ref)) == 0
     for k, name in enumerate(_lib.feature_names("glcm")):
         assert np.array_equal(out[k], ref[k], equal_nan=True), name
