@@ -97,14 +97,16 @@ int rb_pack_levels_dev(const int32_t *image_dev, const uint8_t *mask_dev, long l
  * Feature f of voxel (z,y,x) goes to
  *     out[f * out_feature_stride + ((z - out_z0) * Y + y) * X + x]
  * as float64 (out_is_f32 == 0, the reference's map dtype, base.py:205-209) or float32 (out_is_f32 != 0; every path:
- * fast, generic, every kernelRadius <= 3, weighted / asymmetric GLCM, force2D, 16-bit levels).  out_feature_stride and
+ * fast, generic, wide, weighted / asymmetric GLCM, force2D, 16-bit levels).  out_feature_stride and
  * out_z0 count elements of that type.  Features are computed in float64 either way and a float32 map holds each value
  * rounded to nearest once (NaN stays NaN), so it equals the float64 map converted to float32 bit for bit.
  * Angles that are empty for every voxel of the ROI are "deleted" like in the reference
  * (glcm.py:187-196); rb_glcm_alive_angles_dev computes that set (32-bit words, bit a = angle a,
  * RB_ALIVE_WORDS words, zero-initialised by the caller) and alive_dev may be NULL to keep all.
+ * Windows of up to 343 positions run one thread per centre, 344 to 3375 (kernelRadius 4 to 7 in 3-D) one block per
+ * centre with the same results; a larger window returns RB_ERR_UNSUPPORTED.
  * status_dev: bit 0 = MCC eigen-problem larger than the in-kernel solver (value set to NaN),
- *             bit 1 = weighted GLCM entry overflow. */
+ *             bit 1 = weighted GLCM entry overflow (or, on a window of 344+ positions, more levels than Ng allows). */
 #define RB_ALIVE_WORDS 6
 int rb_glcm_alive_angles_dev(const void *levels_dev, int level_bytes, const uint8_t *centers_dev,
                              int Z, int Y, int X, const rb_voxel_settings *settings,

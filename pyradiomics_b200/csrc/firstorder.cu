@@ -6,10 +6,15 @@
 //                            (voxel_tiles.cuh).  A centre whose 27 window voxels are all in the volume, in the kernel
 //                            mask, non-zero in level and not NaN runs firstorder_full_body; every other centre is drained
 //                            through the generic gather + firstorder_voxel<27>.  Both give the same bits.
+//   firstorder_wide_kernel   windows of 344 to 3375 positions (kernelRadius 4 to 7): one block per centre, the window
+//                            in shared memory, a stable rank sort by the block (insertion sort on one thread when the
+//                            window holds a NaN), block_compact_levels' classes.  The same bits as firstorder_voxel.
 #include "common.cuh"
 #include "firstorder.cuh"
+#include "host_common.hpp"
 #include "pixel.cuh"
 #include "voxel_tiles.cuh"
+#include "wide_window.cuh"
 
 namespace rb {
 
@@ -147,6 +152,90 @@ firstorder_tiles_kernel(const void* __restrict__ img, const uint8_t* __restrict_
     });
 }
 
+constexpr int FO_WIDE_NT = 128;
+// shared memory of a wide window of wn positions: intensities by position and sorted, level scratch, levels, membership
+static int fo_wide_smem(int wn) { return wn * (8 + 8 + 4 + 4 + 4 + 2 + 2 + 1); }
+
+__global__ void __launch_bounds__(FO_WIDE_NT)
+firstorder_wide_kernel(const void* __restrict__ img, const uint8_t* __restrict__ mask, const uint8_t* __restrict__ centers,
+                       const void* __restrict__ lev, const __grid_constant__ FoParams P, double* __restrict__ out,
+                       long long fstride) {
+  extern __shared__ __align__(8) uint8_t smem[];
+  const int wn = (2 * P.rz + 1) * (2 * P.ry + 1) * (2 * P.rx + 1), tid = threadIdx.x;
+  double* xw = (double*)smem;            // intensity at each window position (members only)
+  double* xs = xw + wn;                  // the members' intensities in ascending order
+  int* fq = (int*)(xs + wn);
+  int* val = fq + wn;
+  int* cnt = val + wn;
+  uint16_t* w = (uint16_t*)(cnt + wn);
+  uint16_t* lidx = w + wn;
+  uint8_t* in = (uint8_t*)(lidx + wn);   // in the volume and in the kernel mask
+  __shared__ double s_f[FIRSTORDER_NF];
+  __shared__ int s_n, s_nl, s_N, s_nan;
+  const long long plane = (long long)P.Y * P.X;
+  const long long total = (long long)(P.z1 - P.z0) * plane;
+  for (long long t = blockIdx.x; t < total; t += gridDim.x) {         // block-uniform
+    const ChunkVoxel v = chunk_voxel(P, plane, P.z0, P.out_z0, t);
+    if (!firstorder_center(mask, centers, v)) {
+      if (tid < FIRSTORDER_NF) out[tid * fstride + v.oi] = P.init_value;
+      continue;
+    }
+    if (tid == 0) { s_n = 0; s_N = 0; s_nan = 0; }
+    __syncthreads();
+    int nloc = 0, Nloc = 0;
+    bool nan = false;
+    for (int p = tid; p < wn; p += FO_WIDE_NT) {        // firstorder_generic's gather, by position
+      const WindowOffset o(p, P.rz, P.ry, P.rx);
+      const int zz = v.z + o.dz, yy = v.y + o.dy, xx = v.x + o.dx;
+      bool m = zz >= 0 && zz < P.Z && yy >= 0 && yy < P.Y && xx >= 0 && xx < P.X;
+      const long long j = m ? (long long)zz * P.sz + (long long)yy * P.sy + xx : 0;
+      if (m && mask && !mask[j]) m = false;
+      in[p] = m;
+      w[p] = 0;
+      cnt[p] = 0;
+      if (m) {
+        xw[p] = load_f64(img, P.dtype, j);
+        nan |= xw[p] != xw[p];
+        w[p] = P.level_bytes == 1 ? (uint16_t)((const uint8_t*)lev)[j] : ((const uint16_t*)lev)[j];
+        nloc++;
+        Nloc += w[p] != 0;
+      }
+    }
+    if (nloc) atomicAdd(&s_n, nloc);
+    if (Nloc) atomicAdd(&s_N, Nloc);
+    if (nan) s_nan = 1;
+    __syncthreads();
+    const int n = s_n;
+    if (!s_nan) {
+      // stable rank: #{members before j with x <= x_j} + #{members after j with x < x_j}, the insertion sort's position
+      for (int jp = tid; jp < wn; jp += FO_WIDE_NT) {
+        if (!in[jp]) continue;
+        const double xj = xw[jp];
+        int r = 0;
+        for (int i = 0; i < jp; i++) r += in[i] && xw[i] <= xj;
+        for (int i = jp + 1; i < wn; i++) r += in[i] && xw[i] < xj;
+        xs[r] = xj;
+      }
+    } else if (tid == 0) {
+      int k = 0;
+      for (int p = 0; p < wn; p++) if (in[p]) xs[k++] = xw[p];
+      fo_insertion_sort(xs, n);
+    }
+    const int nl = block_compact_levels(w, wn, val, lidx, fq, s_nl);
+    for (int p = tid; p < wn; p += FO_WIDE_NT)
+      if (lidx[p] != NOLEV) atomicAdd(&cnt[lidx[p]], 1);
+    __syncthreads();
+    if (tid == 0) {
+      double ent, uni;
+      fo_level_classes(cnt, nl, s_N, ent, uni);
+      firstorder_sorted(xs, n, ent, uni, P.shift, P.voxel_volume, s_f);
+    }
+    __syncthreads();
+    if (tid < FIRSTORDER_NF) out[tid * fstride + v.oi] = s_f[tid];
+    __syncthreads();
+  }
+}
+
 static FoParams fo_params(int dtype, int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift,
                           double voxel_volume, double init_value, int z0, int z1, int out_z0) {
   return FoParams{Z, Y, X, (long long)Y * X, X, rz, ry, rx, z0, z1, out_z0, dtype, level_bytes, shift, voxel_volume,
@@ -178,6 +267,23 @@ int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uin
   else if (wcap <= 125) firstorder_kernel<125><<<grid, 128, 0, st>>>(img, mask, centers, lev, P, out, fstride);
   else if (wcap <= 343) firstorder_kernel<343><<<grid, 128, 0, st>>>(img, mask, centers, lev, P, out, fstride);
   else return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
+  RB_LAUNCH_CHECK();
+  return RB_OK;
+}
+
+int firstorder_wide_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
+                           int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
+                           double init_value, double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
+  const FoParams P = fo_params(dtype, level_bytes, Z, Y, X, rz, ry, rx, shift, voxel_volume, init_value, z0, z1, out_z0);
+  const long long total = (long long)(z1 - z0) * Y * X;
+  if (total <= 0) return RB_OK;
+  const int smem = fo_wide_smem((2 * rz + 1) * (2 * ry + 1) * (2 * rx + 1));
+  RB_CUDA(set_max_dynamic_smem(firstorder_wide_kernel, fo_wide_smem(WIDE_WCAP_MAX)));
+  int per_sm = 0;
+  RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, firstorder_wide_kernel, FO_WIDE_NT, smem));
+  long long grid = (long long)sm_count() * (per_sm > 0 ? per_sm : 1);
+  if (grid > total) grid = total;
+  firstorder_wide_kernel<<<(int)grid, FO_WIDE_NT, smem, st>>>(img, mask, centers, lev, P, out, fstride);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }

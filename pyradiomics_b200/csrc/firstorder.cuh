@@ -66,25 +66,36 @@ RB_HD void firstorder_sorted(const XS& x, int n, double ent, double uni, double 
   out[F_Variance] = m2;
 }
 
-// x: the n window intensities (unsorted, destroyed: sorted in place); w: the window's levels (0 = not
-// in the kernel), wn entries
-template <int WCAP>
-RB_HD void firstorder_voxel(double* x, int n, const uint16_t* w, int wn, double shift, double voxel_volume, double* out) {
-  for (int i = 1; i < n; i++) {              // insertion sort (n <= 343, typically 27): stable
+// insertion sort of x[0..n-1] in place: stable, and with NaN the order every body of the window must reproduce
+RB_HD void fo_insertion_sort(double* x, int n) {
+  for (int i = 1; i < n; i++) {
     const double v = x[i];
     int j = i - 1;
     while (j >= 0 && x[j] > v) { x[j + 1] = x[j]; j--; }
     x[j + 1] = v;
   }
+}
+
+// Entropy / Uniformity of the nl level classes cnt[] (N window voxels with a level), in class order
+RB_HD void fo_level_classes(const int* cnt, int nl, int N, double& ent, double& uni) {
+  const double invN = 1.0 / (N ? N : 1);
+  ent = 0; uni = 0;
+  for (int k = 0; k < nl; k++) fo_level_class(cnt[k], invN, ent, uni);
+}
+
+// x: the n window intensities (unsorted, destroyed: sorted in place); w: the window's levels (0 = not
+// in the kernel), wn entries
+template <int WCAP>
+RB_HD void firstorder_voxel(double* x, int n, const uint16_t* w, int wn, double shift, double voxel_volume, double* out) {
+  fo_insertion_sort(x, n);                   // n <= 343, typically 27
   // level histogram of the window, classes in order of first occurrence
   int val[WCAP]; uint16_t lidx[WCAP]; int cnt[WCAP];
   const int nl = compact_levels<WCAP>(w, wn, val, lidx);
   for (int k = 0; k < nl; k++) cnt[k] = 0;
   int N = 0;
   for (int p = 0; p < wn; p++) if (lidx[p] != NOLEV) { cnt[lidx[p]]++; N++; }
-  const double invN = 1.0 / (N ? N : 1);
-  double ent = 0, uni = 0;
-  for (int k = 0; k < nl; k++) fo_level_class(cnt[k], invN, ent, uni);
+  double ent, uni;
+  fo_level_classes(cnt, nl, N, ent, uni);
   firstorder_sorted(x, n, ent, uni, shift, voxel_volume, out);
 }
 

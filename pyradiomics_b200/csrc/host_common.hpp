@@ -118,6 +118,18 @@ inline int fill_vox_params(int cls, int Z, int Y, int X, const VoxSettings& s, V
 
 inline int window_capacity(const VoxParams& P) { return (2 * P.rz + 1) * (2 * P.ry + 1) * (2 * P.rx + 1); }
 
+// Which kernel a window of `cap` positions runs on, texture and first order alike (after the r = 1 fast paths below):
+// the thread-per-centre generic kernels up to 7^3 = 343 positions, the block-per-centre wide kernels (voxel_wide.cu,
+// firstorder.cu) up to 15^3 = 3375 (kernelRadius 4 to 7 in 3-D; larger force2D / 2-D windows), nothing beyond.
+// force_wide (B200_RADIOMICS_FORCE_WIDE=1, for tests) sends the generic kernels' windows to the wide kernels too.
+// The host emulation (tests/host_emul) runs the generic path, so it stops at WP_WIDE.
+constexpr int GENERIC_WCAP_MAX = 343, WIDE_WCAP_MAX = 3375;
+enum WindowPath { WP_GENERIC, WP_WIDE, WP_UNSUPPORTED };
+inline WindowPath window_path(int cap, bool force_wide) {
+  if (cap > WIDE_WCAP_MAX) return WP_UNSUPPORTED;
+  return cap > GENERIC_WCAP_MAX || force_wide ? WP_WIDE : WP_GENERIC;
+}
+
 // Whether texture class cls runs its kernelRadius-1 fast kernel (voxel_fast_launch) rather than the generic one: 8-bit
 // levels and a 3x3x3 window, plus the angle set and weighting the class's fast body is written for.  The host
 // emulation takes the same decision.

@@ -18,6 +18,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #ifdef __CUDACC__
 #define RB_HD __host__ __device__ __forceinline__
 #define RB_HDN __host__ __device__ __noinline__
@@ -123,6 +125,21 @@ struct Entries {
   RB_HD void add(uint32_t k, W v) {
     for (int e = 0; e < n; e++) if (key[e] == k) { w[e] += v; return; }
     if (n < CAP) { key[n] = k; w[n] = v; n++; } else overflow = true;
+  }
+};
+
+// the same list on caller storage (the wide kernel's per-block workspace), capacity cap
+template <typename W>
+struct EntryList {
+  uint32_t* key;
+  W* w;
+  int cap;
+  int n;
+  bool overflow;
+  RB_HD void clear() { n = 0; overflow = false; }
+  RB_HD void add(uint32_t k, W v) {
+    for (int e = 0; e < n; e++) if (key[e] == k) { w[e] += v; return; }
+    if (n < cap) { key[n] = k; w[n] = v; n++; } else overflow = true;
   }
 };
 
@@ -371,16 +388,39 @@ static RB_HDN double sym_second_largest_abs(double* A, int n, int ld, double* d,
   return fmax(fabs(top2), fabs(bot));
 }
 
+// Workspace arrays of glcm_angle_features on the wide kernel: px, py, ridx, cidx of the window's level count, parent of
+// twice that, the |i-j| / i+j lists, and the dense solve's NJCAP^2 matrix and two NJCAP vectors
+struct GlcmScratch {
+  double *px, *py;
+  EntryList<double> D, Sm;
+  uint16_t *ridx, *cidx, *parent;
+  double *A, *dd, *ee;
+};
+// The entry list of glcm_angle_features<0, ...>: an EntryList on the workspace that also carries the workspace of the
+// rest of the function
+template <typename W>
+struct Entries<0, W> : EntryList<W> {
+  GlcmScratch* ws;
+};
+
+// a function's local array T[N], or a pointer to the workspace
+template <bool LOCAL, typename T, int N>
+using ScratchArr = std::conditional_t<LOCAL, T[N], T*>;
+
 // --------------------------------------------------------------------------------------------
 // GLCM: 24 features of ONE normalised matrix given as merged ordered entries (li<<16|lj, weight).
 // Returns false if the matrix is empty (sum 0 -> the reference's NaN angle).
+// Storage: for ECAP > 0 (the generic kernel) the per-level arrays, the |i-j| / i+j lists and the dense solve's matrix are
+// local arrays sized by the template arguments.  ECAP = 0 (the wide kernel, voxel_wide.cu) takes E as an Entries<0, W>
+// and them from E.ws, its workspace (NCAP unused).
 template <int ECAP, int NCAP, int NJCAP, typename W>
 RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val, const VoxParams& P,
                                 double* f, int* status) {
   double S = 0;
   for (int e = 0; e < E.n; e++) S += (double)E.w[e];
   if (S == 0) return false;
-  double px[NCAP], py[NCAP];
+  ScratchArr<(ECAP > 0), double, NCAP> px, py;
+  if constexpr (!(ECAP > 0)) { px = E.ws->px; py = E.ws->py; }
   for (int k = 0; k < n; k++) { px[k] = 0; py[k] = 0; }
   double ux = 0, uy = 0;
   for (int e = 0; e < E.n; e++) {
@@ -391,7 +431,8 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
   }
   // difference / sum histograms (merged by k)
   constexpr int KCAP = ECAP < 1024 ? ECAP : 1024;
-  Entries<KCAP, double> D, Sm;
+  std::conditional_t<(ECAP > 0), Entries<KCAP, double>, EntryList<double>> D, Sm;
+  if constexpr (!(ECAP > 0)) { D = E.ws->D; Sm = E.ws->Sm; }
   D.clear(); Sm.clear();
   double ac = 0, cp = 0, cs = 0, ct = 0, con = 0, sxx = 0, syy = 0, sxy = 0, da = 0, idm = 0, idmn = 0,
          id = 0, idn = 0, inv = 0, ene = 0, maxp = 0, hxy = 0, hxy1 = 0, sa = 0;
@@ -457,14 +498,16 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
   // values of M; every connected component of the bipartite (row level, column level) graph
   // contributes one singular value 1, so >=2 components -> lambda2 = 1 without an eigen-solve.
   if (P.n_roi_levels < 2) { f[G_MCC] = 1.0; return true; }
-  uint16_t ridx[NCAP], cidx[NCAP];
+  ScratchArr<(ECAP > 0), uint16_t, NCAP> ridx, cidx;
+  if constexpr (!(ECAP > 0)) { ridx = E.ws->ridx; cidx = E.ws->cidx; }
   int nr = 0, nc = 0;
   for (int k = 0; k < n; k++) { ridx[k] = px[k] > 0 ? (uint16_t)nr++ : NOLEV; cidx[k] = py[k] > 0 ? (uint16_t)nc++ : NOLEV; }
   // one row or one column level (an asymmetric GLCM may have one and not the other): M has rank 1, Q's eigenvalues are
   // {1, 0, ...}, the second largest is 0 -- before the capacity rule, which only a solve needs
   if (nr < 2 || nc < 2) { f[G_MCC] = 0.0; return true; }
   {
-    uint16_t parent[2 * NCAP];
+    ScratchArr<(ECAP > 0), uint16_t, 2 * NCAP> parent;
+    if constexpr (!(ECAP > 0)) { parent = E.ws->parent; }
     for (int k = 0; k < nr + nc; k++) parent[k] = (uint16_t)k;
     for (int e = 0; e < E.n; e++) {
       int a = ridx[E.key[e] >> 16], b = nr + cidx[E.key[e] & 0xFFFF];
@@ -478,8 +521,9 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
   }
   // capacity: M is nr x nc (nr == nc for a symmetric GLCM) and must fit the NJCAP x NJCAP local array
   if (nr > NJCAP || nc > NJCAP) { f[G_MCC] = NAN; if (status) *status |= 1; return true; }
-  double A[NJCAP * NJCAP];
-  double dd[NJCAP], ee[NJCAP];
+  ScratchArr<(ECAP > 0), double, NJCAP * NJCAP> A;
+  ScratchArr<(ECAP > 0), double, NJCAP> dd, ee;
+  if constexpr (!(ECAP > 0)) { A = E.ws->A; dd = E.ws->dd; ee = E.ws->ee; }
   if (P.symmetric) {
     for (int k = 0; k < nr * nr; k++) A[k] = 0;
     // symmetric P (px = py): M = P / sqrt(px_i px_j + eps) is itself symmetric, its singular values are the |eigenvalues|
@@ -504,6 +548,27 @@ RB_HDN bool glcm_angle_features(const Entries<ECAP, W>& E, int n, const int* val
   }
   f[G_MCC] = second_singular_value(A, m, nn, nn, dd, ee);
   return true;
+}
+
+// angle a's co-occurrences of the window (local levels lidx) into E, weight v each; a symmetrical GLCM adds the
+// mirror pair right after its pair.  The wide kernel's; glcm_voxel keeps its own copy of this loop, because calling
+// this from it changes the generic kernel's SASS.
+template <typename EL, typename V>
+RB_HD void glcm_angle_entries(const uint16_t* lidx, const WinGeom& G, const VoxParams& P, int a, V v, EL& E) {
+  const int az = P.ang[a][0], ay = P.ang[a][1], ax = P.ang[a][2];
+  for (int z = 0; z < G.wz; z++) for (int y = 0; y < G.wy; y++) for (int x = 0; x < G.wx; x++) {
+    if (!G.inside(z + az, y + ay, x + ax)) continue;
+    uint16_t li = lidx[G.idx(z, y, x)], lj = lidx[G.idx(z + az, y + ay, x + ax)];
+    if (li == NOLEV || lj == NOLEV) continue;
+    E.add(((uint32_t)li << 16) | lj, v);
+    if (P.symmetric) E.add(((uint32_t)lj << 16) | li, v);
+  }
+}
+
+// the per-voxel mean over angles: angle features f (NF of them) join the sums where they are not NaN
+template <int NF>
+RB_HD void angle_mean_add(const double* f, double* sum, int* cnt) {
+  for (int k = 0; k < NF; k++) if (f[k] == f[k]) { sum[k] += f[k]; cnt[k]++; }
 }
 
 // all 24 GLCM feature values of one centre voxel
@@ -561,13 +626,13 @@ RB_HD void glcm_voxel(const uint16_t* w, const VoxParams& P, double* out, int* s
 
 // --------------------------------------------------------------------------------------------
 // GLRLM
-template <int ECAP, int NCAP, typename W>
-RB_HDN bool glrlm_angle_features(const Entries<ECAP, W>& E, int n, const int* val, double* f) {
-  constexpr int RLCAP = 8;
+// 16 features of ONE run-length matrix given as merged ordered entries (li<<16|rl-1, count), on caller storage: pr of
+// RLCAP (> the window's longest line), pg of n.  Returns false if the matrix is empty.
+template <int RLCAP, typename EL>
+RB_HD bool glrlm_angle_features_on(const EL& E, int n, const int* val, double* f, double* pr, double* pg) {
   double Nr = 0;
   for (int e = 0; e < E.n; e++) Nr += (double)E.w[e];
   if (Nr == 0) return false;
-  double pr[RLCAP], pg[NCAP];
   for (int k = 0; k < RLCAP; k++) pr[k] = 0;
   for (int k = 0; k < n; k++) pg[k] = 0;
   double re = 0, srlgle = 0, srhgle = 0, lrlgle = 0, lrhgle = 0;
@@ -604,6 +669,38 @@ RB_HDN bool glrlm_angle_features(const Entries<ECAP, W>& E, int n, const int* va
   return true;
 }
 
+template <int ECAP, int NCAP, typename W>
+RB_HDN bool glrlm_angle_features(const Entries<ECAP, W>& E, int n, const int* val, double* f) {
+  constexpr int RLCAP = 8;
+  double pr[RLCAP], pg[NCAP];
+  return glrlm_angle_features_on<RLCAP>(E, n, val, f, pr, pg);
+}
+
+// angle a's runs along every line of the window into E (li<<16 | rl-1, 1 each); returns whether some line of the angle
+// holds more than one ROI voxel
+template <typename EL>
+RB_HD bool glrlm_angle_runs(const uint16_t* lidx, const WinGeom& G, const VoxParams& P, int a, EL& E) {
+  const int az = P.ang[a][0], ay = P.ang[a][1], ax = P.ang[a][2];
+  bool multi = false;
+  for (int z = 0; z < G.wz; z++) for (int y = 0; y < G.wy; y++) for (int x = 0; x < G.wx; x++) {
+    if (G.inside(z - az, y - ay, x - ax)) continue;  // not a line start
+    int cz = z, cy = y, cx = x, gl = -1, rl = 0, elements = 0;
+    while (G.inside(cz, cy, cx)) {
+      uint16_t l = lidx[G.idx(cz, cy, cx)];
+      if (l != NOLEV) {
+        elements++;
+        if (gl < 0) { gl = l; rl = 0; }
+        else if (l == gl) rl++;
+        else { E.add(((uint32_t)gl << 16) | (uint32_t)rl, 1); gl = l; rl = 0; }
+      } else if (gl >= 0) { E.add(((uint32_t)gl << 16) | (uint32_t)rl, 1); gl = -1; rl = 0; }
+      cz += az; cy += ay; cx += ax;
+    }
+    if (gl >= 0) E.add(((uint32_t)gl << 16) | (uint32_t)rl, 1);
+    if (elements > 1) multi = true;
+  }
+  return multi;
+}
+
 template <int WCAP, bool WEIGHTED>
 RB_HD void glrlm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
   const WinGeom G(P);
@@ -613,31 +710,14 @@ RB_HD void glrlm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
   for (int k = 0; k < GLRLM_NF; k++) { sum[k] = 0; cnt[k] = 0; }
   Entries<WCAP, double> EW; EW.clear();
   for (int a = 0; a < P.na; a++) {
-    const int az = P.ang[a][0], ay = P.ang[a][1], ax = P.ang[a][2];
     Entries<WCAP, int> E; E.clear();
-    bool multi = false;
-    for (int z = 0; z < G.wz; z++) for (int y = 0; y < G.wy; y++) for (int x = 0; x < G.wx; x++) {
-      if (G.inside(z - az, y - ay, x - ax)) continue;  // not a line start
-      int cz = z, cy = y, cx = x, gl = -1, rl = 0, elements = 0;
-      while (G.inside(cz, cy, cx)) {
-        uint16_t l = lidx[G.idx(cz, cy, cx)];
-        if (l != NOLEV) {
-          elements++;
-          if (gl < 0) { gl = l; rl = 0; }
-          else if (l == gl) rl++;
-          else { E.add(((uint32_t)gl << 16) | (uint32_t)rl, 1); gl = l; rl = 0; }
-        } else if (gl >= 0) { E.add(((uint32_t)gl << 16) | (uint32_t)rl, 1); gl = -1; rl = 0; }
-        cz += az; cy += ay; cx += ax;
-      }
-      if (gl >= 0) E.add(((uint32_t)gl << 16) | (uint32_t)rl, 1);
-      if (elements > 1) multi = true;
-    }
+    const bool multi = glrlm_angle_runs(lidx, G, P, a, E);
     if (!multi) continue;  // cmatrices.c:524-534: the angle's (only) run-length-1 column is zeroed
     if (WEIGHTED) {
       for (int e = 0; e < E.n; e++) EW.add(E.key[e], P.wgt[a] * E.w[e]);
     } else {
       if (!glrlm_angle_features<WCAP, WCAP, int>(E, n, val, f)) continue;
-      for (int k = 0; k < GLRLM_NF; k++) if (f[k] == f[k]) { sum[k] += f[k]; cnt[k]++; }
+      angle_mean_add<GLRLM_NF>(f, sum, cnt);
     }
   }
   if (WEIGHTED) {
@@ -650,12 +730,13 @@ RB_HD void glrlm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
 
 // --------------------------------------------------------------------------------------------
 // "level x size" feature block shared by GLSZM (size = zone size) and GLDM (size = dep + 1)
-template <int ECAP, int NCAP, int JCAP>
-RB_HDN void size_matrix_features(const Entries<ECAP, int>& E, int n, const int* val, double* f) {
+// on caller storage: pj of jcap + 1 (jcap >= the largest size), pg of n
+template <typename EL>
+RB_HD void size_matrix_features_on(const EL& E, int n, const int* val, double* f, int jcap, double* pj, double* pg) {
+  const int JCAP = jcap;
   double Nz = 0;
   for (int e = 0; e < E.n; e++) Nz += E.w[e];
   double NzDiv = Nz == 0 ? 1.0 : Nz;
-  double pj[JCAP + 1], pg[NCAP];
   int jmax = 0;
   for (int k = 0; k <= JCAP; k++) pj[k] = 0;
   for (int k = 0; k < n; k++) pg[k] = 0;
@@ -686,13 +767,16 @@ RB_HDN void size_matrix_features(const Entries<ECAP, int>& E, int n, const int* 
   f[S_Percentage] = NzDiv / (np_ == 0 ? 1.0 : np_); f[S_SizeVar] = sv;
 }
 
-template <int WCAP>
-RB_HD void glszm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
-  const WinGeom G(P);
-  int val[WCAP]; uint16_t lidx[WCAP];
-  const int n = compact_levels<WCAP>(w, G.n, val, lidx);
-  Entries<WCAP, int> E; E.clear();
-  uint16_t stack[WCAP];
+template <int ECAP, int NCAP, int JCAP>
+RB_HDN void size_matrix_features(const Entries<ECAP, int>& E, int n, const int* val, double* f) {
+  double pj[JCAP + 1], pg[NCAP];
+  size_matrix_features_on(E, n, val, f, JCAP, pj, pg);
+}
+
+// the window's zones (li<<16 | size, 1 each) into E by flood fill from each unvisited voxel in scan order, so zones
+// come in order of their lowest position; lidx is consumed (NOLEV after), stack holds up to the window's size
+template <typename EL>
+RB_HD void glszm_zones(uint16_t* lidx, const WinGeom& G, const VoxParams& P, uint16_t* stack, EL& E) {
   for (int s = 0; s < G.n; s++) {
     uint16_t gl = lidx[s];
     if (gl == NOLEV) continue;
@@ -711,6 +795,36 @@ RB_HD void glszm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
     }
     E.add(((uint32_t)gl << 16) | (uint32_t)region, 1);
   }
+}
+
+// every ROI voxel's (li<<16 | dependence + 1) into E, in scan order
+template <typename EL>
+RB_HD void gldm_entries(const uint16_t* lidx, const int* val, const WinGeom& G, const VoxParams& P, EL& E) {
+  for (int z = 0; z < G.wz; z++) for (int y = 0; y < G.wy; y++) for (int x = 0; x < G.wx; x++) {
+    uint16_t li = lidx[G.idx(z, y, x)];
+    if (li == NOLEV) continue;
+    int dep = 0;
+    for (int a = 0; a < P.na; a++) {
+      int z2 = z + P.ang[a][0], y2 = y + P.ang[a][1], x2 = x + P.ang[a][2];
+      if (!G.inside(z2, y2, x2)) continue;
+      uint16_t lj = lidx[G.idx(z2, y2, x2)];
+      if (lj == NOLEV) continue;
+      int d = val[li] - val[lj];
+      if (d < 0) d = -d;
+      if (d <= P.alpha) dep++;
+    }
+    E.add(((uint32_t)li << 16) | (uint32_t)(dep + 1), 1);
+  }
+}
+
+template <int WCAP>
+RB_HD void glszm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
+  const WinGeom G(P);
+  int val[WCAP]; uint16_t lidx[WCAP];
+  const int n = compact_levels<WCAP>(w, G.n, val, lidx);
+  Entries<WCAP, int> E; E.clear();
+  uint16_t stack[WCAP];
+  glszm_zones(lidx, G, P, stack, E);
   double f[SIZE_NF];
   size_matrix_features<WCAP, WCAP, WCAP>(E, n, val, f);
   for (int k = 0; k < GLSZM_NF; k++) out[k] = f[k];
@@ -730,33 +844,17 @@ RB_HD void gldm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
   int val[WCAP]; uint16_t lidx[WCAP];
   const int n = compact_levels<WCAP>(w, G.n, val, lidx);
   Entries<WCAP, int> E; E.clear();
-  for (int z = 0; z < G.wz; z++) for (int y = 0; y < G.wy; y++) for (int x = 0; x < G.wx; x++) {
-    uint16_t li = lidx[G.idx(z, y, x)];
-    if (li == NOLEV) continue;
-    int dep = 0;
-    for (int a = 0; a < P.na; a++) {
-      int z2 = z + P.ang[a][0], y2 = y + P.ang[a][1], x2 = x + P.ang[a][2];
-      if (!G.inside(z2, y2, x2)) continue;
-      uint16_t lj = lidx[G.idx(z2, y2, x2)];
-      if (lj == NOLEV) continue;
-      int d = val[li] - val[lj];
-      if (d < 0) d = -d;
-      if (d <= P.alpha) dep++;
-    }
-    E.add(((uint32_t)li << 16) | (uint32_t)(dep + 1), 1);
-  }
+  gldm_entries(lidx, val, G, P, E);
   double f[SIZE_NF];
   size_matrix_features<WCAP, WCAP, NA_MAX + 1>(E, n, val, f);
   gldm_from_size(f, out);
 }
 
 // --------------------------------------------------------------------------------------------
-template <int WCAP>
-RB_HD void ngtdm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
-  const WinGeom G(P);
-  int val[WCAP]; uint16_t lidx[WCAP];
-  const int n = compact_levels<WCAP>(w, G.n, val, lidx);
-  double cnt[WCAP], s[WCAP];
+// NGTDM of the window on caller storage cnt, s (n each): per-level counts and |differences| summed in scan order, then
+// the five features
+RB_HD void ngtdm_window(const uint16_t* lidx, const int* val, int n, const WinGeom& G, const VoxParams& P, double* cnt,
+                        double* s, double* out) {
   for (int k = 0; k < n; k++) { cnt[k] = 0; s[k] = 0; }
   for (int z = 0; z < G.wz; z++) for (int y = 0; y < G.wy; y++) for (int x = 0; x < G.wx; x++) {
     uint16_t li = lidx[G.idx(z, y, x)];
@@ -793,6 +891,15 @@ RB_HD void ngtdm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
   out[N_Busyness] = busy_den != 0 ? ps / busy_den : 0.0;
   out[N_Complexity] = cpx / Nvp;
   out[N_Strength] = ssum != 0 ? str / ssum : 0.0;
+}
+
+template <int WCAP>
+RB_HD void ngtdm_voxel(const uint16_t* w, const VoxParams& P, double* out) {
+  const WinGeom G(P);
+  int val[WCAP]; uint16_t lidx[WCAP];
+  const int n = compact_levels<WCAP>(w, G.n, val, lidx);
+  double cnt[WCAP], s[WCAP];
+  ngtdm_window(lidx, val, n, G, P, cnt, s, out);
 }
 
 }  // namespace rb
