@@ -76,6 +76,7 @@ __device__ __forceinline__ void lanczos_group(const uint8_t* __restrict__ lev, c
                                               const uint16_t* order, unsigned base, int begin, int end, double* scratch) {
   for (int b0 = begin; b0 < end; b0 += 128) {
     const int i = b0 + (int)threadIdx.x;
+    if (b0 + (int)(threadIdx.x & ~31u) >= end) break;   // a warp with no task left (the solver holds no barrier)
     const bool live = i < end;
     const unsigned k = base + order[live ? i : begin];
     const GlcmTask e = queue[k];
@@ -99,17 +100,23 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
   if (threadIdx.x == 0) glcm_solve_tables_from(*Tg, T);
   __syncthreads();
   const unsigned n = *qcount;
-  // Tiles of 4096 consecutive tasks are counting-sorted by size class in shared memory, so the lanes of a warp run
+  // Tiles of up to 4096 consecutive tasks are counting-sorted by size class in shared memory, so the lanes of a warp run
   // solves of the same size (otherwise a third of the lanes stay active).  The sort is STABLE and atomic-free (per-thread
-  // counts, one serial scan per class), so a task's position is the same in every run.
+  // counts, one serial scan per class), so a task's position is the same in every run.  The Lanczos kind cuts the queue
+  // into a whole number of tiles per block, all of one size (+-1), so no launch ends on a partial wave of tiles; the dense
+  // kinds, whose block-uniform rounds cost the same however few tasks they hold, keep full tiles.  A task's result does
+  // not depend on its tile.
   constexpr int TILE = 4096;
   constexpr int LO = SolveKind<KIND>::lo, KC = SolveKind<KIND>::hi - SolveKind<KIND>::lo + 1;
   __shared__ uint16_t order[TILE];
   __shared__ int bucket[GF_NCLS];                 // end position of each class of this kind in `order`
   __shared__ uint16_t cnt[KC][128];               // [class][thread]: count, then exclusive prefix over the threads
-  const unsigned ntiles = (n + TILE - 1) / TILE;
+  const unsigned long long per_wave = (unsigned long long)gridDim.x * TILE;
+  const unsigned ntiles = KIND == 2 ? gridDim.x * (unsigned)((n + per_wave - 1) / per_wave) : (n + TILE - 1) / TILE;
   for (unsigned tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const unsigned base = tile * TILE;
+    const unsigned base = KIND == 2 ? (unsigned)((unsigned long long)n * tile / ntiles) : tile * TILE;
+    const unsigned tend = KIND == 2 ? (unsigned)((unsigned long long)n * (tile + 1) / ntiles)   // tend - base <= TILE
+                                    : (n - base < (unsigned)TILE ? n : base + TILE);
 #pragma unroll
     for (int c = 0; c < KC; c++) cnt[c][threadIdx.x] = 0;
     if (threadIdx.x < GF_NCLS) bucket[threadIdx.x] = 0;
@@ -117,7 +124,7 @@ glcm_fast_solve_kernel(const uint8_t* __restrict__ lev, const __grid_constant__ 
 #pragma unroll
     for (int j = 0; j < TILE / 128; j++) {
       const unsigned k = base + j * 128 + threadIdx.x;
-      mycls[j] = k < n ? queue[k].cls : GF_NCLS;
+      mycls[j] = k < tend ? queue[k].cls : GF_NCLS;
       const int c = (int)mycls[j] - LO;
       if (c >= 0 && c < KC) cnt[c][threadIdx.x]++;
     }

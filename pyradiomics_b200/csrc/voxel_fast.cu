@@ -69,11 +69,14 @@ static int glcm_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxPar
   if (P.sy != P.X || P.sz != plane) return fail(RB_ERR_ARG, "GLCM fast path expects a contiguous level volume");
   const int sms = sm_count();
   // chunk of planes whose worst-case queue (13 eigen-tasks per voxel) stays <= 48 Mi entries
-  // (768 MB of tasks + 384 MB of results)
+  // (768 MB of tasks + 384 MB of results); the planes are spread evenly over the chunks, so the last one is not a
+  // small remainder that leaves most of the GPU idle
   const long long max_entries = 48ll << 20;
   int zchunk = (int)(max_entries / (plane * GF_NA));
   if (zchunk < 1) zchunk = 1;
   if (zchunk > z1 - z0) zchunk = z1 - z0;
+  const int nchunks = (z1 - z0 + zchunk - 1) / zchunk;
+  zchunk = (z1 - z0 + nchunks - 1) / nchunks;
   // float maps: phase A keeps the partial MCC of the voxels with eigen-tasks in float64 (zchunk planes), so the finished
   // MCC is rounded to float once
   constexpr bool f64 = std::is_same<OutT, double>::value;
