@@ -147,7 +147,8 @@ int rb_voxel_features_host(int cls, const int32_t *image, const uint8_t *mask, i
  *        glrlm [nvox][Ng][Nr][Na]        Na = unidirectional distance-1 angles
  *        gldm  [nvox][Ng][2*Na+1]        Na = BIdirectional angles of `distances` (_cmatrices.c:790)
  *        ngtdm [nvox][Ng][3]             columns n_i, s_i, i
- *      Use rb_generate_angles first to learn Na; `angles` (may be NULL) receives Na x nd ints. */
+ *      Use rb_generate_angles first to learn Na; `angles` (may be NULL) receives Na x nd ints.
+ *      A GLRLM run longer than Nr, in either mode, gives RB_ERR_LEVEL_RANGE. */
 int rb_calculate_glcm(const int32_t *image, const uint8_t *mask, const int *size, int nd,
                       const int *distances, int ndist, int Ng, int force2D, int force2Ddimension,
                       int kernelRadius, const int *voxels, int nvox, double *glcm, int *angles);

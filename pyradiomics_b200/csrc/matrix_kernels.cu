@@ -38,11 +38,13 @@ __device__ __forceinline__ void batch_window(const T* __restrict__ lev, const Ba
   load_window<T>(lev, P, voxels[v], voxels[G.nvox + v], voxels[2 * G.nvox + v], w);
 }
 
-// MODE 0 glcm, 1 gldm, 2 ngtdm, 3 glrlm
+// MODE 0 glcm, 1 gldm, 2 ngtdm, 3 glrlm.  A GLRLM run longer than Nr sets bit 1 of *status and is not counted: its
+// flat index would fall in the next gray level's row, or past the voxel's matrix at the top level.
 template <typename T, int WCAP, int MODE>
 __global__ void __launch_bounds__(128)
 batch_matrix_kernel(const T* __restrict__ lev, BatchGeom G, const int* __restrict__ voxels,
-                    const __grid_constant__ AngleSet A, int Ng, int Nr, int alpha, double* __restrict__ out) {
+                    const __grid_constant__ AngleSet A, int Ng, int Nr, int alpha, double* __restrict__ out,
+                    int* __restrict__ status) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= G.nvox) return;
   uint16_t w[WCAP];
@@ -84,8 +86,13 @@ batch_matrix_kernel(const T* __restrict__ lev, BatchGeom G, const int* __restric
     }
   } else {
     double* o = out + (size_t)v * Ng * Nr * A.na;
+    bool too_long = false;
     for (int a = 0; a < A.na; a++) {
       const int az = A.a[a][0], ay = A.a[a][1], ax = A.a[a][2];
+      const auto count = [&](int gl, int rl) {
+        if (rl < Nr) o[((size_t)(gl - 1) * Nr + rl) * A.na + a] += 1.0;
+        else too_long = true;
+      };
       bool multi = false;
       for (int z = 0; z < W.wz; z++) for (int y = 0; y < W.wy; y++) for (int x = 0; x < W.wx; x++) {
         if (W.inside(z - az, y - ay, x - ax)) continue;
@@ -96,15 +103,16 @@ batch_matrix_kernel(const T* __restrict__ lev, BatchGeom G, const int* __restric
             elements++;
             if (!gl) { gl = g; rl = 0; }
             else if (g == gl) rl++;
-            else { o[((size_t)(gl - 1) * Nr + rl) * A.na + a] += 1.0; gl = g; rl = 0; }
-          } else if (gl) { o[((size_t)(gl - 1) * Nr + rl) * A.na + a] += 1.0; gl = 0; rl = 0; }
+            else { count(gl, rl); gl = g; rl = 0; }
+          } else if (gl) { count(gl, rl); gl = 0; rl = 0; }
           cz += az; cy += ay; cx += ax;
         }
-        if (gl) o[((size_t)(gl - 1) * Nr + rl) * A.na + a] += 1.0;
+        if (gl) count(gl, rl);
         if (elements > 1) multi = true;
       }
       if (!multi) for (int g = 0; g < Ng; g++) o[((size_t)g * Nr) * A.na + a] = 0.0;
     }
+    if (too_long) atomicOr(status, 2);
   }
 }
 
@@ -219,6 +227,7 @@ static int check_status(const Prepared& R, const char* what) {
   int st = 0;
   RB_CUDA(cudaMemcpy(&st, R.status.p, sizeof st, cudaMemcpyDeviceToHost));
   if (st & 1) return fail(RB_ERR_LEVEL_RANGE, "Calculation of %s Failed: gray level outside 1..Ng inside the mask", what);
+  if (st & 2) return fail(RB_ERR_LEVEL_RANGE, "Calculation of %s Failed: run longer than Nr", what);
   return RB_OK;
 }
 
@@ -237,9 +246,10 @@ static int launch_batch(const Prepared& R, const BatchGeom& G, int Ng, int Nr, i
   const int grid = (G.nvox + 127) / 128;
   const T* lev = R.lev.as<const T>();
   const int* vox = R.vox.as<const int>();
-  if (cap <= 27) batch_matrix_kernel<T, 27, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out);
-  else if (cap <= 125) batch_matrix_kernel<T, 125, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out);
-  else if (cap <= 343) batch_matrix_kernel<T, 343, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out);
+  int* st = R.status.as<int>();
+  if (cap <= 27) batch_matrix_kernel<T, 27, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out, st);
+  else if (cap <= 125) batch_matrix_kernel<T, 125, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out, st);
+  else if (cap <= 343) batch_matrix_kernel<T, 343, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out, st);
   else return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
   RB_LAUNCH_CHECK();
   return RB_OK;

@@ -66,6 +66,15 @@ if "matrix" in fams:
         cmatrices.calculate_gldm(lev, m, [1], 32, 0, False, -1, 1, vox)
         cmatrices.calculate_ngtdm(lev, m, [1], 32, False, -1, 1, vox)
         print("matrix ok", float(P.sum()), flush=True)
+    # voxel batches at kernelRadius 3 (the 343-position window) with 16-bit levels: GLCM lists 16 voxels (150 MB)
+    lev16 = lev + 268
+    vox = np.array(np.where(mask_rag))[:, ::23].astype(np.int32)
+    cmatrices.calculate_glcm(lev16, mask_rag, [1], 300, False, -1, 3, vox[:, :16])
+    cmatrices.calculate_glrlm(lev16, mask_rag, 300, 7, False, -1, 3, vox)
+    cmatrices.calculate_glszm(lev16, mask_rag, 300, 343, False, -1, 3, vox)
+    cmatrices.calculate_gldm(lev16, mask_rag, [1], 300, 1, False, -1, 3, vox)
+    cmatrices.calculate_ngtdm(lev16, mask_rag, [1], 300, False, -1, 3, vox)
+    print("matrix r3 16-bit ok", flush=True)
     # a row pitch that is a multiple of 16 bytes: the fused tile kernel stages its boxes by TMA (else cooperative loads)
     lt, mt = np.ascontiguousarray(lev[:, :, :N16]), np.ascontiguousarray(mask_rag[:, :, :N16])
     for tma in ("1", "0"):
