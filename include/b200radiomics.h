@@ -63,11 +63,18 @@ const char *rb_last_error(void);
 const char *rb_version(void);
 int rb_device_count(void);          /* >= 0, or RB_ERR_CUDA                                   */
 int rb_num_features(int cls);       /* 24 / 16 / 16 / 14 / 5                                  */
-/* The fused GLCM path keeps one eigen-task queue per (device, stream) it ran on (grown on demand, up to 1.15 GB) so that
- * repeated calls do not reallocate; this synchronises the current device and frees its queues.  Threading contract of
- * the library: calls on DIFFERENT streams may run from different host threads (each stream owns its queue; the cache map
- * is mutex-protected); two host threads must not issue GLCM calls on the SAME stream at once, nor call this function while
- * another thread has a call in flight on this device. */
+/* The fused GLCM path keeps one eigen-task queue per (device, stream) it ran on (grown on demand, up to 1.15 GB), and the
+ * kernels for windows of 344+ positions one workspace per (device, stream), so that repeated calls do not reallocate;
+ * this frees those of the current device.  It waits for the calls that are enqueueing on them, synchronises the device,
+ * then frees; a later call allocates again.
+ * Threading contract of the library:
+ *   - every `*_dev` voxel entry point (rb_pack_levels_dev, rb_glcm_alive_angles_dev, rb_voxel_features_dev,
+ *     rb_firstorder_voxel_dev, rb_memcpy2d_async, rb_maps_to_f32_dev) issues its launches, memsets and copies on the
+ *     given stream only;
+ *   - concurrent calls are safe from any number of host threads, on the same stream or on different ones: a call holds
+ *     its stream's queue or workspace from taking it until its last launch on it is enqueued, so calls on one stream
+ *     enqueue one after the other and run in that order;
+ *   - rb_release_device_caches may be called at any time, from any thread. */
 int rb_release_device_caches(void);
 /* name of feature `idx` of class `cls` (the reference's get<Name>FeatureValue names, in the
  * alphabetical order in which the reference enumerates them, radiomics/base.py:163-179). */

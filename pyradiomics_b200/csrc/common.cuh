@@ -31,6 +31,9 @@ namespace rb {
 
 // A table block built on the host by build(T&) from zeroed memory and copied to the current device once per
 // (device, key); it stays for the life of the process.  nullptr if it could not be allocated or copied.
+// The copy has landed before the pointer is handed out: a plain cudaMemcpy from pageable memory may return while its
+// DMA is still in flight, ordered only with the legacy default stream, and the caller launches on its own (possibly
+// non-blocking) stream.  So it runs on a private stream that is synchronised, which stalls no other stream.
 template <typename T, typename Build>
 const T* device_table(Build build, int key = 0) {
   static std::mutex mu;
@@ -44,7 +47,12 @@ const T* device_table(Build build, int key = 0) {
   build(*h);
   T* d = nullptr;
   if (cudaMalloc(&d, sizeof(T)) != cudaSuccess) return nullptr;
-  if (cudaMemcpy(d, h.get(), sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(d); return nullptr; }
+  cudaStream_t s = nullptr;
+  if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) { cudaFree(d); return nullptr; }
+  const bool ok = cudaMemcpyAsync(d, h.get(), sizeof(T), cudaMemcpyHostToDevice, s) == cudaSuccess &&
+                  cudaStreamSynchronize(s) == cudaSuccess;
+  cudaStreamDestroy(s);
+  if (!ok) { cudaFree(d); return nullptr; }
   return cache[{dev, key}] = d;
 }
 

@@ -4,6 +4,7 @@
 // Every kernel and launch function takes the map type (double or float, store_map in voxel_tiles.cuh).
 #include <map>
 #include <mutex>
+#include <vector>
 
 #include "common.cuh"
 #define RB_GLCM_BLOCK_SYNC 1   // phase A is called by all threads of a block, uniformly
@@ -16,34 +17,49 @@
 namespace rb {
 
 // per (device, stream) task queue, grown on demand; float maps add the float64 partial-MCC plane of a chunk (mcc,
-// mcc_cap doubles)
+// mcc_cap doubles).  `mu` is held from taking the queue until the last launch that uses it is enqueued, so two host
+// threads on one stream enqueue their chunk sequences one after the other, and a growth or a release never frees a
+// buffer a call is still about to launch on.  Entries are never erased (a std::map node does not move), so a pointer to
+// one stays valid after g_queue_mu is dropped.
 struct GlcmQueue {
   GlcmTask* q = nullptr; double* res = nullptr; unsigned* count = nullptr; size_t cap = 0;
   double* mcc = nullptr; size_t mcc_cap = 0;
+  std::mutex mu;
 };
-static std::mutex g_queue_mu;
+static std::mutex g_queue_mu;   // the map only
 static std::map<std::pair<int, cudaStream_t>, GlcmQueue> g_queue_cache;
-// rb_release_device_caches: give the eigen-task queues of the current device back (up to 1.15 GB per stream that ran GLCM)
+// rb_release_device_caches: give the eigen-task queues of the current device back (up to 1.15 GB per stream that ran
+// GLCM).  Every queue's lock is taken first, so no call is between taking a queue and its last launch; the device
+// synchronisation then waits for the launches already enqueued.
 int glcm_release_queues() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return RB_ERR_CUDA;
+  std::vector<std::unique_lock<std::mutex>> held;
+  std::vector<GlcmQueue*> mine;
+  {
+    std::lock_guard<std::mutex> lk(g_queue_mu);
+    for (auto& kv : g_queue_cache)
+      if (kv.first.first == dev) mine.push_back(&kv.second);
+  }
+  for (GlcmQueue* Q : mine) held.emplace_back(Q->mu);
   cudaDeviceSynchronize();
-  std::lock_guard<std::mutex> lk(g_queue_mu);
-  for (auto it = g_queue_cache.begin(); it != g_queue_cache.end();) {
-    if (it->first.first == dev) {
-      cudaFree(it->second.q); cudaFree(it->second.res); cudaFree(it->second.count); cudaFree(it->second.mcc);
-      it = g_queue_cache.erase(it);
-    } else ++it;
+  for (GlcmQueue* Q : mine) {
+    cudaFree(Q->q); cudaFree(Q->res); cudaFree(Q->count); cudaFree(Q->mcc);
+    Q->q = nullptr; Q->res = nullptr; Q->count = nullptr; Q->mcc = nullptr; Q->cap = Q->mcc_cap = 0;
   }
   return RB_OK;
 }
-static GlcmQueue* glcm_queue(cudaStream_t st, size_t need, size_t mcc_need) {
-  std::mutex& mu = g_queue_mu;
-  auto& cache = g_queue_cache;
+// the queue of (current device, st), grown to `need` tasks and `mcc_need` partial-MCC doubles, with its lock held in lk
+static GlcmQueue* glcm_queue(cudaStream_t st, size_t need, size_t mcc_need, std::unique_lock<std::mutex>& lk) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  std::lock_guard<std::mutex> lk(mu);
-  GlcmQueue& Q = cache[{dev, st}];
+  GlcmQueue* entry;
+  {
+    std::lock_guard<std::mutex> mlk(g_queue_mu);
+    entry = &g_queue_cache[{dev, st}];
+  }
+  lk = std::unique_lock<std::mutex>(entry->mu);
+  GlcmQueue& Q = *entry;
   if (!Q.count && cudaMalloc(&Q.count, sizeof(unsigned)) != cudaSuccess) return nullptr;
   if (Q.cap < need) {
     if (Q.q) { cudaStreamSynchronize(st); cudaFree(Q.q); cudaFree(Q.res); Q.q = nullptr; Q.res = nullptr; Q.cap = 0; }
@@ -80,7 +96,8 @@ static int glcm_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxPar
   // float maps: phase A keeps the partial MCC of the voxels with eigen-tasks in float64 (zchunk planes), so the finished
   // MCC is rounded to float once
   constexpr bool f64 = std::is_same<OutT, double>::value;
-  GlcmQueue* Q = glcm_queue(st, (size_t)zchunk * plane * GF_NA, f64 ? 0 : (size_t)zchunk * plane);
+  std::unique_lock<std::mutex> qlk;      // held until the last chunk's finish kernel is enqueued
+  GlcmQueue* Q = glcm_queue(st, (size_t)zchunk * plane * GF_NA, f64 ? 0 : (size_t)zchunk * plane, qlk);
   if (!Q) return fail(RB_ERR_NOMEM, "could not allocate the GLCM eigen-task queue");
   // phase A: one CTA per SM (register-bound).  512 threads at 128 registers (a hundred spilled words per thread, L1-
   // resident) put 16 warps on an SM instead of the 8 of a 256-thread / 236-register build, which hides more of the

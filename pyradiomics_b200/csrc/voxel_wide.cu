@@ -11,6 +11,7 @@
 // (B200_RADIOMICS_FORCE_WIDE=1 sends windows <= 343 here to show it).
 #include <map>
 #include <mutex>
+#include <vector>
 
 #include "common.cuh"
 #include "host_common.hpp"
@@ -282,32 +283,49 @@ static WideLayout wide_layout(int cls, const VoxParams& P) {
   return L;
 }
 
-// per (device, stream) workspace, grown on demand
-static std::mutex g_ws_mu;
-static std::map<std::pair<int, cudaStream_t>, std::pair<void*, size_t>> g_ws_cache;
+// per (device, stream) workspace, grown on demand.  `mu` is held from taking the workspace until the kernel that uses it
+// is enqueued (voxel_fast.cu's GlcmQueue does the same): a second host thread on the stream cannot free it under a call
+// that has not launched yet, and its own launch follows the first in stream order.  Entries are never erased.
+struct WideWorkspace {
+  void* p = nullptr;
+  size_t bytes = 0;
+  std::mutex mu;
+};
+static std::mutex g_ws_mu;   // the map only
+static std::map<std::pair<int, cudaStream_t>, WideWorkspace> g_ws_cache;
 
 int wide_release_workspace() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return RB_ERR_CUDA;
-  cudaDeviceSynchronize();
-  std::lock_guard<std::mutex> lk(g_ws_mu);
-  for (auto it = g_ws_cache.begin(); it != g_ws_cache.end();) {
-    if (it->first.first == dev) { cudaFree(it->second.first); it = g_ws_cache.erase(it); } else ++it;
+  std::vector<std::unique_lock<std::mutex>> held;
+  std::vector<WideWorkspace*> mine;
+  {
+    std::lock_guard<std::mutex> lk(g_ws_mu);
+    for (auto& kv : g_ws_cache)
+      if (kv.first.first == dev) mine.push_back(&kv.second);
   }
+  for (WideWorkspace* W : mine) held.emplace_back(W->mu);
+  cudaDeviceSynchronize();
+  for (WideWorkspace* W : mine) { cudaFree(W->p); W->p = nullptr; W->bytes = 0; }
   return RB_OK;
 }
 
-static uint8_t* wide_workspace(cudaStream_t st, size_t need) {
+// the workspace of (current device, st), at least `need` bytes, with its lock held in lk
+static uint8_t* wide_workspace(cudaStream_t st, size_t need, std::unique_lock<std::mutex>& lk) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  std::lock_guard<std::mutex> lk(g_ws_mu);
-  auto& W = g_ws_cache[{dev, st}];
-  if (W.second < need) {
-    if (W.first) { cudaStreamSynchronize(st); cudaFree(W.first); W.first = nullptr; W.second = 0; }
-    if (cudaMalloc(&W.first, need) != cudaSuccess) { W.first = nullptr; return nullptr; }
-    W.second = need;
+  WideWorkspace* W;
+  {
+    std::lock_guard<std::mutex> mlk(g_ws_mu);
+    W = &g_ws_cache[{dev, st}];
   }
-  return (uint8_t*)W.first;
+  lk = std::unique_lock<std::mutex>(W->mu);
+  if (W->bytes < need) {
+    if (W->p) { cudaStreamSynchronize(st); cudaFree(W->p); W->p = nullptr; W->bytes = 0; }
+    if (cudaMalloc(&W->p, need) != cudaSuccess) { W->p = nullptr; return nullptr; }
+    W->bytes = need;
+  }
+  return (uint8_t*)W->p;
 }
 
 // one resident wave of blocks (the occupancy at this window's shared memory), at most one block per centre, and no
@@ -335,7 +353,8 @@ static int wide_run(int cls, const T* lev, const uint8_t* centers, const VoxPara
   auto launch = [&](auto kernel) -> int {
     int grid = 0;
     if (int rc = wide_grid(kernel, smem, total, L.block_bytes, grid)) return rc;
-    uint8_t* ws = wide_workspace(st, (size_t)grid * L.block_bytes);
+    std::unique_lock<std::mutex> wlk;    // held until the kernel is enqueued
+    uint8_t* ws = wide_workspace(st, (size_t)grid * L.block_bytes, wlk);
     if (!ws) return fail(RB_ERR_NOMEM, "could not allocate the wide voxel kernel's workspace (%lld bytes)",
                          (long long)grid * L.block_bytes);
     kernel<<<grid, WIDE_NT, smem, st>>>(lev, centers, P, L, ws, out, fstride, z0, z1, out_z0, status);

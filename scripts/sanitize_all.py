@@ -16,7 +16,8 @@ from pyradiomics_b200 import _lib, cmatrices, cshape, featureclasses as FC, imag
 args = [a for a in sys.argv[1:]]
 N = int(args.pop(0)) if args and args[0].isdigit() else 20
 N16 = N - N % 16 if N >= 16 else N
-fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d", "imagetypes", "preprocess"]
+fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d", "imagetypes", "preprocess",
+                "streams"]
 rng = np.random.default_rng(0)
 
 
@@ -155,4 +156,36 @@ if "preprocess" in fams:
             kept.append(int((I.as_array(out) != 0).sum()))
     torch.cuda.synchronize()
     print("preprocess ok", kept, flush=True)
+if "streams" in fams:
+    # the per-stream locks of the GLCM queue and the wide workspace: two host threads on the default stream, each a
+    # GLCM call and a wide (kernelRadius 5) call, the second thread's wide call on more levels (a larger workspace)
+    import threading
+    n = min(N, 12)
+    alive = np.full(_lib.ALIVE_WORDS, 0xFFFFFFFF, np.uint32)
+    cen = torch.zeros((n, n, n), dtype=torch.uint8, device="cuda")
+    cen[::4, ::4, ::4] = 1
+
+    def packed(lv):
+        lv = np.ascontiguousarray(lv[:n, :n, :n])
+        levd, _ = voxel.pack_levels(torch.as_tensor(lv).cuda(), torch.ones(lv.shape, dtype=torch.uint8, device="cuda"),
+                                    int(lv.max()))
+        return levd, _lib.make_settings(int(lv.max()), 32), _lib.make_settings(int(lv.max()), 32, kernelRadius=5)
+    # (8-bit levels of the GLCM call, levels of the wide call): thread 1's wide call has 16-bit levels
+    jobs = [(packed(vols["smooth"]), packed(vols["smooth"])), (packed(vols["uniform"]), packed(vols["smooth"] + 268))]
+    barrier = threading.Barrier(2)
+    res = [None, None]
+
+    def work(k):
+        (l1, s1, _), (l5, _, s5) = jobs[k]
+        barrier.wait()
+        res[k] = (voxel.voxel_features("glcm", l1, s1, alive=alive),
+                  voxel.voxel_features("glcm", l5, s5, centers=cen, alive=alive))
+    ts = [threading.Thread(target=work, args=(k,)) for k in range(2)]
+    for t in ts:
+        t.start()
+    for t in ts:
+        t.join()
+    torch.cuda.synchronize()
+    _lib.lib().rb_release_device_caches()
+    print("streams ok", [float(r[0][0].sum().item()) for r in res], flush=True)
 print("sanitize_all done")
