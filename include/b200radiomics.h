@@ -290,6 +290,14 @@ int rb_lbp3d_dev(const void *img_dev, int img_dtype, int sample_dtype, const uin
 enum { RB_LBP2D_DEFAULT = 0, RB_LBP2D_ROR = 1, RB_LBP2D_UNIFORM = 2, RB_LBP2D_NRI_UNIFORM = 3, RB_LBP2D_VAR = 4 };
 int rb_lbp2d_dev(const void *img_dev, int dtype, int Z, int Y, int X, int axis, int P, const double *rp_host,
                  const double *cp_host, int method, double *out_dev, void *stream);
+/* rb_lbp2d_cast_dev: the same codes stored in the image's own pixel type, as the reference's per-slice assignment
+ *   im_arr[idx, ...] = local_binary_pattern(...) stores them (NumPy's unsafe float64 -> image_type cast): out_dev has the
+ *   input's rb_dtype (`image_type`) and layout, and no float64 volume is made.  The cast (csrc/lbp2d.cuh, numpy_cast):
+ *   float64 unchanged; float32 rounded to nearest (+-inf beyond its range); int32 trunc(v) if it fits, else INT32_MIN (NaN
+ *   and +-inf too); int16 / uint16 / uint8 the low bits of that int32; int64 trunc(v) if it fits, else INT64_MIN.
+ *   Argument checks as rb_lbp2d_dev. */
+int rb_lbp2d_cast_dev(const void *img_dev, int image_type, int Z, int Y, int X, int axis, int P, const double *rp_host,
+                      const double *cp_host, int method, void *out_dev, void *stream);
 
 /* ---- per-voxel image types (reference radiomics/imageoperations.py:973-1073, getSquareImage, getSquareRootImage,
  *      getLogarithmImage, getExponentialImage).  out_dev[i] = f(x), x = img_dev[i] as float64, for i < nvoxels:

@@ -95,6 +95,7 @@ PROTOTYPES = {
     "rb_resample_dev": (_i, [_p, _i, _p, _p, _i, _p, _p, _p, _i, _d, _p]),
     "rb_lbp3d_dev": (_i, [_p, _i, _i, _p, _i, _i, _i, _p, _i, _p, _i, _p, _p, _p]),
     "rb_lbp2d_dev": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p]),
+    "rb_lbp2d_cast_dev": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p, _i, _p, _p]),
     "rb_pointwise_image_dev": (_i, [_p, _i, _ll, _i, _d, _p, _p]),
     "rb_gradient_magnitude_dev": (_i, [_p, _i, _i, _i, _i, _p, _p, _p]),
     "rb_roi_moments_dev": (_i, [_p, _i, _p, _ll, _i, _p, _p, _p]),

@@ -97,7 +97,7 @@ int resample_launch(const void* src, int src_dt, const int* in_size, void* dst, 
 int lbp3d_launch(const void* img, int img_dt, int sample_dt, const uint8_t* roi, int Z, int Y, int X, const double* vertices,
                  int nv, const double* harmonics, int levels, double* coeff_scratch, double* out, cudaStream_t st);
 int lbp2d_launch(const void* img, int dt, int Z, int Y, int X, int axis, int P, const double* rp, const double* cp, int method,
-                 double* out, cudaStream_t st);
+                 int out_dt, void* out, cudaStream_t st);
 
 int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
                       int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
@@ -415,7 +415,12 @@ int rb_lbp3d_dev(const void* img_dev, int img_dtype, int sample_dtype, const uin
 int rb_lbp2d_dev(const void* img_dev, int dtype, int Z, int Y, int X, int axis, int P, const double* rp_host,
                  const double* cp_host, int method, double* out_dev, void* stream) {
   if (int rc = check_dtypes({dtype})) return rc;
-  return lbp2d_launch(img_dev, dtype, Z, Y, X, axis, P, rp_host, cp_host, method, out_dev, (cudaStream_t)stream);
+  return lbp2d_launch(img_dev, dtype, Z, Y, X, axis, P, rp_host, cp_host, method, RB_DT_FLOAT64, out_dev, (cudaStream_t)stream);
+}
+int rb_lbp2d_cast_dev(const void* img_dev, int image_type, int Z, int Y, int X, int axis, int P, const double* rp_host,
+                      const double* cp_host, int method, void* out_dev, void* stream) {
+  if (int rc = check_dtypes({image_type})) return rc;
+  return lbp2d_launch(img_dev, image_type, Z, Y, X, axis, P, rp_host, cp_host, method, image_type, out_dev, (cudaStream_t)stream);
 }
 
 int rb_swt3d_dev(const double* in_dev, int Z, int Y, int X, const double* dec_lo, const double* dec_hi, int flen,

@@ -963,25 +963,42 @@ def _lbp2d_params(samples, radius, method):
     return P, code, rp, cp
 
 
-def lbp2d_device(img_t: torch.Tensor, axis=0, samples=8, radius=1, method="uniform"):
+def _lbp2d_axis(axis):
+    """force2Ddimension as rb_lbp2d_dev's axis 0..2 (swapaxes' negative axes), or ValueError"""
+    if isinstance(axis, (int, np.integer)) and -3 <= axis <= 2:
+        return int(axis) % 3
+    raise ValueError(f"LBP 2D: force2Ddimension {axis!r} (0, 1 or 2)")
+
+
+# what rb_lbp2d_dev / rb_lbp2d_cast_dev read: the device path's pixel types and torch.uint16, which the kernels read as
+# uint16 (a uint16 NumPy image that _to_device uploads arrives as int32 and is read, and cast, as int32)
+_LBP2D_SOURCE_CODE = {**TORCH_DTYPE_CODE, torch.uint16: DTYPE_CODE[np.dtype(np.uint16)]}
+
+
+def lbp2d_device(img_t: torch.Tensor, axis=0, samples=8, radius=1, method="uniform", out_dtype=None):
     """2-D LBP (skimage.feature.local_binary_pattern(slice, P=samples, R=radius, method=method)) of every slice of a CUDA
     volume (Z,Y,X) cut along `axis` as getLBP2DImage cuts it (swapaxes(0, axis): axis 0 -> (y, x) slices, 1 -> (z, x),
-    2 -> (y, z)), or of a CUDA plane (Y,X) -> float64 CUDA tensor of the input's shape (rb_lbp2d_dev).  No cast to the
-    image's dtype: getLBP2DImage does that on the host, as the reference does."""
+    2 -> (y, z)), or of a CUDA plane (Y,X) -> CUDA tensor of the input's shape.  `out_dtype` None (default): float64, no
+    cast (rb_lbp2d_dev; getLBP2DImage casts on the host, as the reference does).  `out_dtype` = img_t's dtype: a volume's
+    codes are stored in that dtype by the kernel with the reference's NumPy cast (rb_lbp2d_cast_dev), what getLBP2DImage
+    returns; a plane stays float64, as the reference's 2-D branch leaves it."""
     P, code, rp, cp = _lbp2d_params(samples, radius, method)
-    src = _checked_source(img_t)
+    src = img_t.contiguous()
+    if src.dtype not in _LBP2D_SOURCE_CODE:
+        raise ValueError(f"unsupported pixel type {src.dtype}")
+    if out_dtype is not None and out_dtype != src.dtype:
+        raise ValueError(f"LBP 2D: out_dtype {out_dtype} is neither None (float64) nor the image's {src.dtype}")
     if src.dim() not in (2, 3):
         raise ValueError(f"LBP 2D: 2-D or 3-D image expected, got {src.dim()}-D")
-    if src.dim() == 2:
-        axis = 0
-    elif isinstance(axis, (int, np.integer)) and -3 <= axis <= 2:
-        axis = int(axis) % 3                                    # swapaxes' negative axes
-    else:
-        raise ValueError(f"LBP 2D: force2Ddimension {axis!r} (0, 1 or 2)")
+    axis = 0 if src.dim() == 2 else _lbp2d_axis(axis)
     Z, Y, X = (1,) * (3 - src.dim()) + tuple(src.shape)
-    out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
-    check(lib().rb_lbp2d_dev(ptr(src), TORCH_DTYPE_CODE[src.dtype], Z, Y, X, int(axis), P, ptr(rp), ptr(cp), code, ptr(out),
-                             stream()), "lbp2d")
+    dt = _LBP2D_SOURCE_CODE[src.dtype]
+    if out_dtype is None or src.dim() == 2:
+        out = torch.empty(src.shape, dtype=torch.float64, device=src.device)
+        check(lib().rb_lbp2d_dev(ptr(src), dt, Z, Y, X, axis, P, ptr(rp), ptr(cp), code, ptr(out), stream()), "lbp2d")
+    else:
+        out = torch.empty(src.shape, dtype=src.dtype, device=src.device)
+        check(lib().rb_lbp2d_cast_dev(ptr(src), dt, Z, Y, X, axis, P, ptr(rp), ptr(cp), code, ptr(out), stream()), "lbp2d")
     return out
 
 

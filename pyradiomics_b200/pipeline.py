@@ -2,7 +2,7 @@
 
 * ``voxel_suite_with_filters`` -- Original + wavelet (8 sub-bands) + LoG (one per sigma) derived
   images (+ the square / squareroot / logarithm / exponential / gradient and 3-D LBP images on
-  request) -> per-image gray-level discretisation -> the five fused voxel-based texture kernels and,
+  request, and the 2-D LBP image in the image's own dtype) -> per-image gray-level discretisation -> the five fused voxel-based texture kernels and,
   on request, the first-order kernel on the image's own intensities, everything on one GPU without host round trips (what ``RadiomicsFeatureExtractor.execute(...,
   voxelBased=True)`` does image type by image type, reference radiomics/featureextractor.py:371-392).
 * ``segment_suite_with_filters`` -- the segment-based counterpart: shape of the ROI, then first order and the five
@@ -26,16 +26,39 @@ from ._lib import CLASSES
 IMAGE_TYPES = ("square", "squareroot", "logarithm", "exponential", "gradient")
 
 
+def _lbp2d_args(lbp2d):
+    """(axis, samples, radius, method) of an `lbp2d` settings dict with getLBP2DImage's defaults; ValueError / KeyError
+    for settings the kernel refuses, so that they raise before anything is launched"""
+    samples, radius = lbp2d.get("lbp2DSamples", 8), lbp2d.get("lbp2DRadius", 1)
+    method = lbp2d.get("lbp2DMethod", "uniform")
+    IO._lbp2d_params(samples, radius, method)
+    return IO._lbp2d_axis(lbp2d.get("force2Ddimension", 0)), samples, radius, method
+
+
+def _suite_lbp2d(lbp2d, settings):
+    """a suite's `lbp2d` dict, its force2D / force2Ddimension taken from the suite's settings where it has none, checked"""
+    if lbp2d is None:
+        return None
+    lbp2d = {"force2D": settings.get("force2D", False), "force2Ddimension": settings.get("force2Ddimension", 0), **lbp2d}
+    _lbp2d_args(lbp2d)
+    return lbp2d
+
+
 def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1", sigmas=(1.0, 2.0, 3.0),
-                   original=True, lbp3d=None, mask=None, image_types=(), gradient_use_spacing=True):
+                   original=True, lbp3d=None, mask=None, image_types=(), gradient_use_spacing=True, lbp2d=None):
     """yields (name, CUDA tensor) like the reference's imageType generators.  `image_types`: names out of IMAGE_TYPES,
     yielded after LoG in the caller's order as float64 images (one max|x| reduction serves every per-voxel type;
-    `gradient_use_spacing` is getGradientImage's gradientUseSpacing).  `lbp3d`: a settings dict (lbp3DLevels,
+    `gradient_use_spacing` is getGradientImage's gradientUseSpacing).  `lbp2d`: a settings dict (lbp2DRadius,
+    lbp2DSamples, lbp2DMethod, force2D, force2Ddimension; {} = getLBP2DImage's defaults) adds the 2-D LBP image
+    'lbp-2D' after those: the slices are cut along force2Ddimension (default 0) and the codes stored in x's dtype with
+    the reference's NumPy cast (imageoperations.lbp2d_device(out_dtype=x.dtype)), getLBP2DImage's warning logged when
+    force2D is off; its settings are checked before the first image is yielded.  `lbp3d`: a settings dict (lbp3DLevels,
     lbp3DIcosphereRadius, lbp3DIcosphereSubdivision; {} = the defaults) adds the 3-D LBP level maps and kurtosis map of
-    the ROI `mask` (non-zero voxels) after those, as getLBP3DImage names them; None (default) leaves them out."""
+    the ROI `mask` (non-zero voxels) after those, as getLBP3DImage names them; None (default) leaves either out."""
     unknown = [t for t in image_types if t not in IMAGE_TYPES]
     if unknown:
         raise ValueError(f"unknown image types {unknown} (known: {IMAGE_TYPES})")
+    lbp2d_args = _lbp2d_args(lbp2d) if lbp2d is not None else None
     if original:
         yield "original", x
     if wavelet:
@@ -56,6 +79,10 @@ def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1"
         if max_abs is None:
             max_abs = IO.image_max_abs(x)
         yield t, IO.pointwise_image_device(x, t, max_abs)
+    if lbp2d is not None:
+        if not lbp2d.get("force2D", False):
+            IO.logger.warning("Calculating Local Binary Pattern in 2D, but extracting features in 3D. Use with caution!")
+        yield "lbp-2D", IO.lbp2d_device(x, *lbp2d_args, out_dtype=x.dtype)
     if lbp3d is not None:
         if mask is None:
             raise ValueError("the LBP 3-D images need the ROI mask")
@@ -69,10 +96,11 @@ def derived_images(x: torch.Tensor, spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1"
 
 def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CLASSES, spacing_zyx=(1.0, 1.0, 1.0),
                              wavelet="coif1", sigmas=(1.0, 2.0, 3.0), consume=None, lbp3d=None, image_types=(),
-                             gradient_use_spacing=True, normalize=None, resegment=None, map_dtype=torch.float64, **kw):
+                             gradient_use_spacing=True, normalize=None, resegment=None, map_dtype=torch.float64, lbp2d=None,
+                             **kw):
     """image: CUDA tensor (Z,Y,X) of raw intensities, mask: CUDA uint8/bool.  For every derived
-    image (`image_types`, `gradient_use_spacing`, `lbp3d`: see derived_images): bin (binWidth/binCount in kw) -> pack ->
-    fused kernels.
+    image (`image_types`, `gradient_use_spacing`, `lbp2d`, `lbp3d`: see derived_images; force2D / force2Ddimension
+    missing from `lbp2d` come from kw): bin (binWidth/binCount in kw) -> pack -> fused kernels.
     `normalize` (a dict with normalizeScale, removeOutliers; {} = the defaults) normalises the whole image first and every
     derived image comes from the normalised one; `resegment` (a dict with resegmentRange, resegmentMode) then resegments
     the mask against that image, and binning, the texture kernels and the LBP 3-D ROI use the resegmented mask -- the
@@ -89,6 +117,7 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
     if unknown:
         raise ValueError(f"unknown voxel classes {unknown} (known: {CLASSES + ('firstorder',)})")
     fo_kw = {k: kw[k] for k in ("kernelRadius", "force2D", "force2Ddimension", "voxelArrayShift", "initValue") if k in kw}
+    lbp2d = _suite_lbp2d(lbp2d, kw)
     if normalize is not None:
         image = IO.normalize_image_device(image, normalize.get("normalizeScale", 1), normalize.get("removeOutliers"))
     msk = (mask != 0).to(torch.uint8).contiguous()
@@ -98,7 +127,7 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
     outs = {}
     info = []
     for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=msk, image_types=image_types,
-                                    gradient_use_spacing=gradient_use_spacing):
+                                    gradient_use_spacing=gradient_use_spacing, lbp2d=lbp2d):
         img = img.contiguous()
         _, _, lev, levels, Ng = voxel.discretize(img, msk, **kw)
         nlev = len(levels)
@@ -120,11 +149,12 @@ def voxel_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=CL
 def segment_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=("firstorder",) + CLASSES, shape=True,
                                spacing_zyx=(1.0, 1.0, 1.0), wavelet="coif1", sigmas=(1.0, 2.0, 3.0), image_types=(),
                                lbp3d=None, gradient_use_spacing=True, normalize=None, resegment=None,
-                               resegment_shape=False, label=1, **settings):
+                               resegment_shape=False, label=1, lbp2d=None, **settings):
     """Segment-based extraction over every image type on one GPU.  image: CUDA tensor (Z,Y,X) of raw intensities,
     mask: CUDA label map; the ROI is ``mask == label``.  `normalize` / `resegment` as in voxel_suite_with_filters (first
     normalisation, then resegmentation of the ROI against the normalised image, then the filters of derived_images, with
-    `wavelet`, `sigmas`, `image_types`, `gradient_use_spacing` and `lbp3d` as there).  `classes`: "firstorder" and names
+    `wavelet`, `sigmas`, `image_types`, `gradient_use_spacing`, `lbp2d` and `lbp3d` as there; force2D /
+    force2Ddimension missing from `lbp2d` come from `settings`).  `classes`: "firstorder" and names
     out of CLASSES, in the order their features are wanted; binning, distances, symmetricalGLCM, weightingNorm, gldm_a,
     force2D, force2Ddimension and voxelArrayShift come from `settings`.
     Returns an ordered dict keyed like RadiomicsFeatureExtractor.execute() without the diagnostics: first
@@ -137,6 +167,7 @@ def segment_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=
     unknown = [c for c in classes if c not in CLASSES and c != "firstorder"]
     if unknown:
         raise ValueError(f"unknown segment classes {unknown} (known: {('firstorder',) + CLASSES})")
+    lbp2d = _suite_lbp2d(lbp2d, settings)
     if normalize is not None:
         image = IO.normalize_image_device(image, normalize.get("normalizeScale", 1), normalize.get("removeOutliers"))
     roi = (mask == label).to(torch.uint8).contiguous()
@@ -154,7 +185,7 @@ def segment_suite_with_filters(image: torch.Tensor, mask: torch.Tensor, classes=
     fo_names = FC.RadiomicsFirstOrder.getFeatureNames()
     fo_enabled = {n: True for n, deprecated in fo_names.items() if not deprecated}      # what enableAllFeatures enables
     for name, img in derived_images(image, spacing_zyx, wavelet, sigmas, lbp3d=lbp3d, mask=roi, image_types=image_types,
-                                    gradient_use_spacing=gradient_use_spacing):
+                                    gradient_use_spacing=gradient_use_spacing, lbp2d=lbp2d):
         img = img.contiguous()
         dev = FC.DeviceImage(img, roi, 1, True, settings)
         for c in classes:

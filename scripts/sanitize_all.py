@@ -1,6 +1,6 @@
 """compute-sanitizer target: ONE small invocation of every kernel family of the library (fused voxel fast
 paths, the generic voxel kernel, the cMatrices builders in segment and voxel-batch mode, discretisation,
-wavelet, LoG, shape, first-order, 3-D LBP, the square / squareroot / logarithm / exponential / gradient
+wavelet, LoG, shape, first-order, 3-D LBP, the 2-D LBP stored in the image's dtype, the square / squareroot / logarithm / exponential / gradient
 image types, normalisation and resegmentation).  Run as
     compute-sanitizer --tool memcheck|racecheck|initcheck|synccheck python scripts/sanitize_all.py [N] [family ...]
 The families are independent so a slow tool can be pointed at one of them."""
@@ -16,8 +16,8 @@ from pyradiomics_b200 import _lib, cmatrices, cshape, featureclasses as FC, imag
 args = [a for a in sys.argv[1:]]
 N = int(args.pop(0)) if args and args[0].isdigit() else 20
 N16 = N - N % 16 if N >= 16 else N
-fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d", "imagetypes", "preprocess",
-                "streams"]
+fams = args or ["fast", "generic", "matrix", "filters", "shape", "firstorder", "lbp3d", "lbp2d_cast", "imagetypes",
+                "preprocess", "streams"]
 rng = np.random.default_rng(0)
 
 
@@ -136,6 +136,14 @@ if "lbp3d" in fams:
         names = [n for _, n, _ in IO.getLBP3DImage(raw, mask_rag.astype(np.uint8), **kw)]
     torch.cuda.synchronize()
     print("lbp3d ok", names, flush=True)
+if "lbp2d_cast" in fams:
+    # rb_lbp2d_cast_dev once per method: uint8 (the codes wrap), int16 along x, float32 with P 24 R 3
+    raw = ((vols["smooth"] - 1) * 25 + 3).astype(np.int16)
+    for k, method in enumerate(IO.LBP2D_METHODS):
+        img = torch.from_numpy([raw.astype(np.uint8), raw, raw.astype(np.float32) / 7][k % 3]).cuda()
+        out = IO.lbp2d_device(img, k % 3, 24 if k % 3 == 2 else 9, 3 if k % 3 == 2 else 1, method, out_dtype=img.dtype)
+    torch.cuda.synchronize()
+    print("lbp2d_cast ok", out.dtype, flush=True)
 if "imagetypes" in fams:
     raw = ((vols["smooth"] - 1) * 25 - 300).astype(np.int16)
     names = []
