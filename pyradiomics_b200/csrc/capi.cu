@@ -5,7 +5,6 @@
 #include <vector>
 
 #include "common.cuh"
-#include "host_common.hpp"
 #include "pixel.cuh"
 
 namespace rb {
@@ -24,32 +23,24 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
-// the voxel kernels' launch functions: `out` holds float maps when out_f32, else double
-int voxel_features_generic(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P,
-                           void* out, bool out_f32, long long fstride, int z0, int z1, int out_z0, int* status,
-                           cudaStream_t st);
 int glcm_alive_angles(const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P, uint32_t* alive,
                       cudaStream_t st);
 int pack_levels(const int32_t* image, const uint8_t* mask, long long n, int Ng, void* lev, uint32_t* presence,
                 int* status, cudaStream_t st);
-int glcm_release_queues();
-int voxel_features_wide(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P, void* out,
-                        bool out_f32, long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st);
-int wide_release_workspace();
-int voxel_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
-                      long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
 
-// B200_RADIOMICS_FORCE_GENERIC=1 routes everything through the generic kernels (used by the
-// tests to cross-check the fast paths on the GPU)
-static bool force_generic() {
-  const char* e = getenv("B200_RADIOMICS_FORCE_GENERIC");
+static bool env_flag(const char* name) {
+  const char* e = getenv(name);
   return e && e[0] == '1';
 }
-// B200_RADIOMICS_FORCE_WIDE=1 sends every window, fast-path ones included, to the wide kernels (window_path): the tests
-// compare them with the generic kernels bit for bit
-static bool force_wide() {
-  const char* e = getenv("B200_RADIOMICS_FORCE_WIDE");
-  return e && e[0] == '1';
+// window_path with the two test overrides read from the environment: B200_RADIOMICS_FORCE_GENERIC=1 declines the fast
+// kernels (the tests cross-check them against the generic ones), B200_RADIOMICS_FORCE_WIDE=1 sends every window to the
+// wide kernels (the tests compare them with the generic and fast kernels bit for bit)
+static WindowPath voxel_window_path(bool fast_fits, int positions) {
+  return window_path(positions, env_flag("B200_RADIOMICS_FORCE_WIDE"), fast_fits, env_flag("B200_RADIOMICS_FORCE_GENERIC"));
+}
+static int unsupported_window(int positions) {
+  return fail(RB_ERR_UNSUPPORTED, "a kernel window of %d positions is outside the implemented envelope (at most %d: "
+              "kernelRadius <= 7 in 3-D)", positions, WIDE_WCAP_MAX);
 }
 
 int calculate_matrix_host(int mode, const int32_t* image, const uint8_t* mask, const int* size, int nd,
@@ -99,15 +90,6 @@ int lbp3d_launch(const void* img, int img_dt, int sample_dt, const uint8_t* roi,
 int lbp2d_launch(const void* img, int dt, int Z, int Y, int X, int axis, int P, const double* rp, const double* cp, int method,
                  int out_dt, void* out, cudaStream_t st);
 
-int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
-                      int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
-                      double init_value, double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
-int firstorder_wide_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
-                           int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
-                           double init_value, double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
-int firstorder_fast_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
-                           int Z, int Y, int X, double shift, double voxel_volume, double init_value, double* out,
-                           long long fstride, int z0, int z1, int out_z0, cudaStream_t st);
 int firstorder_segment(const void* img, int dtype, const uint8_t* roi, const void* lev, int level_bytes, long long n,
                        double shift, double voxel_volume, double* out18_host, cudaStream_t st);
 static const char* kFirstOrderNames[] = {"10Percentile", "90Percentile", "Energy", "Entropy", "InterquartileRange", "Kurtosis",
@@ -166,9 +148,7 @@ int rb_device_count(void) {
 }
 
 int rb_release_device_caches(void) {
-  const int rc = glcm_release_queues();
-  const int rc2 = wide_release_workspace();
-  return rc ? rc : rc2;
+  return release_stream_scratch();
 }
 
 int rb_num_features(int cls) { return (cls < 0 || cls > 4) ? RB_ERR_ARG : kNumFeatures[cls]; }
@@ -209,23 +189,15 @@ int rb_voxel_features_dev(int cls, const void* levels_dev, int level_bytes, cons
                           void* stream) {
   if (cls < 0 || cls > 4) return fail(RB_ERR_ARG, "unknown texture class %d", cls);
   if (z0 < 0 || z1 > Z || z0 > z1) return fail(RB_ERR_ARG, "bad z range");
-  VoxParams P;
-  if (fill_vox_params(cls, Z, Y, X, *settings, P)) return fail(RB_ERR_ARG, "bad voxel settings");
-  if (alive_host && cls == C_GLCM) memcpy(P.alive, alive_host, sizeof P.alive);
-  const bool f32 = out_is_f32 != 0, wide = force_wide();
-  if (!force_generic() && !wide && voxel_fast_path(cls, level_bytes, P))
-    return voxel_fast_launch(cls, levels_dev, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1, out_z0,
-                             (cudaStream_t)stream);
-  switch (window_path(window_capacity(P), wide)) {
-    case WP_GENERIC:
-      return voxel_features_generic(cls, levels_dev, level_bytes, centers_dev, P, out_dev, f32, out_feature_stride, z0,
-                                    z1, out_z0, status_dev, (cudaStream_t)stream);
-    case WP_WIDE:
-      return voxel_features_wide(cls, levels_dev, level_bytes, centers_dev, P, out_dev, f32, out_feature_stride, z0, z1,
-                                 out_z0, status_dev, (cudaStream_t)stream);
-    default:
-      return fail(RB_ERR_UNSUPPORTED, "a kernel window of %d positions is outside the implemented envelope (at most %d: "
-                  "kernelRadius <= 7 in 3-D)", window_capacity(P), WIDE_WCAP_MAX);
+  VoxLaunch A = {cls, levels_dev, level_bytes, centers_dev, {}, out_dev, out_is_f32 != 0, out_feature_stride, z0, z1,
+                 out_z0, status_dev, (cudaStream_t)stream};
+  if (fill_vox_params(cls, Z, Y, X, *settings, A.P)) return fail(RB_ERR_ARG, "bad voxel settings");
+  if (alive_host && cls == C_GLCM) memcpy(A.P.alive, alive_host, sizeof A.P.alive);
+  switch (voxel_window_path(voxel_fast_path(cls, level_bytes, A.P), window_capacity(A.P))) {
+    case WP_FAST: return voxel_fast_launch(A);
+    case WP_GENERIC: return voxel_features_generic(A);
+    case WP_WIDE: return voxel_features_wide(A);
+    default: return unsupported_window(window_capacity(A.P));
   }
 }
 
@@ -496,23 +468,16 @@ int rb_firstorder_voxel_dev(const void* image_dev, int dtype, const uint8_t* mas
   if (int rc = check_dtypes({dtype})) return rc;
   if (level_bytes != 1 && level_bytes != 2) return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
   if (rz < 0 || ry < 0 || rx < 0 || z0 < 0 || z1 > Z || z0 > z1) return fail(RB_ERR_ARG, "bad window / z range");
-  const bool wide = force_wide();
-  if (!force_generic() && !wide && firstorder_fast_path(level_bytes, rz, ry, rx))
-    return firstorder_fast_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, Z, Y, X, voxelArrayShift,
-                                  voxel_volume, initValue, out_dev, out_feature_stride, z0, z1, out_z0, (cudaStream_t)stream);
-  const int cap = (2 * rz + 1) * (2 * ry + 1) * (2 * rx + 1);
-  switch (window_path(cap, wide)) {
-    case WP_GENERIC:
-      return firstorder_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, level_bytes, Z, Y, X, rz, ry, rx,
-                               voxelArrayShift, voxel_volume, initValue, out_dev, out_feature_stride, z0, z1, out_z0,
-                               (cudaStream_t)stream);
-    case WP_WIDE:
-      return firstorder_wide_launch(image_dev, dtype, mask_dev, centers_dev, levels_dev, level_bytes, Z, Y, X, rz, ry, rx,
-                                    voxelArrayShift, voxel_volume, initValue, out_dev, out_feature_stride, z0, z1, out_z0,
-                                    (cudaStream_t)stream);
-    default:
-      return fail(RB_ERR_UNSUPPORTED, "a kernel window of %d positions is outside the implemented envelope (at most %d: "
-                  "kernelRadius <= 7 in 3-D)", cap, WIDE_WCAP_MAX);
+  const FoLaunch A = {image_dev, mask_dev, centers_dev, levels_dev,
+                      {Z, Y, X, (long long)Y * X, X, rz, ry, rx, z0, z1, out_z0, dtype, level_bytes, voxelArrayShift,
+                       voxel_volume, initValue},
+                      out_dev, out_feature_stride, (cudaStream_t)stream};
+  const int positions = (2 * rz + 1) * (2 * ry + 1) * (2 * rx + 1);
+  switch (voxel_window_path(firstorder_fast_path(level_bytes, rz, ry, rx), positions)) {
+    case WP_FAST: return firstorder_fast_launch(A);
+    case WP_GENERIC: return firstorder_launch(A);
+    case WP_WIDE: return firstorder_wide_launch(A);
+    default: return unsupported_window(positions);
   }
 }
 

@@ -1,5 +1,6 @@
-// Shared host-side plumbing of libb200radiomics: error state, CUDA call checking, temporary device buffers and the
-// per-device launch state (table blocks, SM count, occupancy, kernel attributes).
+// Shared host-side plumbing of libb200radiomics: error state, CUDA call checking, temporary device buffers, the
+// per-device launch state (table blocks, SM count, occupancy, kernel attributes) and the voxel-map kernels' dispatch
+// (runtime values to template arguments, launch argument blocks, per-stream scratch).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdio.h>
@@ -8,9 +9,12 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <utility>
+#include <vector>
 
 #include "../../include/b200radiomics.h"
+#include "host_common.hpp"
 
 namespace rb {
 std::string& last_error_ref();
@@ -145,6 +149,125 @@ cudaError_t set_max_dynamic_smem(K* kernel, int bytes) {
     set = true;
   }
   return cudaSuccess;
+}
+
+// ---- voxel-map dispatch: each helper calls f with the type tag of a runtime value and returns f's result
+// packed levels: uint8_t or uint16_t
+template <typename F>
+int with_level_type(int level_bytes, F&& f) {
+  if (level_bytes == 1) return f(uint8_t{});
+  if (level_bytes == 2) return f(uint16_t{});
+  return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
+}
+// feature maps: float or double
+template <typename F>
+int with_map_type(bool out_f32, F&& f) {
+  return out_f32 ? f(float{}) : f(double{});
+}
+// the generic kernels' window class (window_class): std::integral_constant<int, 27 / 125 / 343>
+template <typename F>
+int with_window_class(int positions, F&& f) {
+  switch (window_class(positions)) {
+    case 27: return f(std::integral_constant<int, 27>{});
+    case 125: return f(std::integral_constant<int, 125>{});
+    case GENERIC_WCAP_MAX: return f(std::integral_constant<int, GENERIC_WCAP_MAX>{});
+    default: return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
+  }
+}
+
+// The arguments of a texture-class launch (voxel_fast_launch, voxel_features_generic, voxel_features_wide): the packed
+// levels, the centres (NULL: every non-zero level), the maps (`out` holds float maps when out_f32, else double;
+// feature k of chunk plane z at out + k * fstride + (z - out_z0) * Y * X), the chunk's planes [z0, z1), the word the
+// kernels OR their status bits into and the stream every launch runs on.
+struct VoxLaunch {
+  int cls;
+  const void* lev; int level_bytes; const uint8_t* centers; VoxParams P;
+  void* out; bool out_f32; long long fstride;
+  int z0, z1, out_z0;
+  int* status; cudaStream_t st;
+};
+int voxel_fast_launch(const VoxLaunch& A);
+int voxel_features_generic(const VoxLaunch& A);
+int voxel_features_wide(const VoxLaunch& A);
+
+// The first-order kernels' parameter block (passed to them by value)
+struct FoParams {
+  int Z, Y, X;
+  long long sz, sy;    // element strides of the (contiguous) image, mask and level volumes
+  int rz, ry, rx, z0, z1, out_z0, dtype, level_bytes;
+  double shift, voxel_volume, init_value;
+};
+// The arguments of a first-order launch (firstorder_fast_launch, firstorder_launch, firstorder_wide_launch)
+struct FoLaunch {
+  const void* img; const uint8_t* mask; const uint8_t* centers; const void* lev;
+  FoParams P;
+  double* out; long long fstride;
+  cudaStream_t st;
+};
+int firstorder_fast_launch(const FoLaunch& A);
+int firstorder_launch(const FoLaunch& A);
+int firstorder_wide_launch(const FoLaunch& A);
+
+// ---- per-(device, stream) scratch of the voxel kernels, grown on demand: GLCM's eigen-task queue (tasks, results,
+// count, float maps' partial-MCC plane) and the wide kernels' workspace.  A call holds its entry's mutex from taking the
+// entry until its last launch on these buffers is enqueued: two host threads on one stream enqueue one after the other
+// (in stream order), and a growth or a release never frees a buffer a call is still about to launch on.  Calls on other
+// streams never wait for it.  Entries are emptied, never erased (a std::map node does not move), so a pointer to one
+// stays valid after the map's own mutex is dropped.
+struct ScratchBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+  template <typename U> U* as() const { return (U*)p; }
+};
+struct StreamScratch {
+  std::mutex mu;
+  cudaStream_t st = 0;
+  ScratchBuf tasks, results, count, mcc, wide;
+  // b holds at least `bytes`: a smaller buffer is freed once the stream has finished with it, then a new one allocated;
+  // false, with b empty, if that allocation fails
+  bool grow(ScratchBuf& b, size_t bytes) {
+    if (b.bytes >= bytes) return true;
+    if (b.p) { cudaStreamSynchronize(st); cudaFree(b.p); b.p = nullptr; b.bytes = 0; }
+    if (cudaMalloc(&b.p, bytes) != cudaSuccess) { b.p = nullptr; return false; }
+    b.bytes = bytes;
+    return true;
+  }
+};
+inline std::mutex g_scratch_mu;   // the map only
+inline std::map<std::pair<int, cudaStream_t>, StreamScratch> g_scratch;
+
+// the scratch of (current device, st) with its mutex held in lk; nullptr if the device cannot be read
+inline StreamScratch* stream_scratch(cudaStream_t st, std::unique_lock<std::mutex>& lk) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  StreamScratch* S;
+  {
+    std::lock_guard<std::mutex> mlk(g_scratch_mu);
+    S = &g_scratch[{dev, st}];
+  }
+  lk = std::unique_lock<std::mutex>(S->mu);
+  S->st = st;
+  return S;
+}
+
+// rb_release_device_caches: free the current device's scratch (up to 1.15 GB of GLCM queue per stream that ran GLCM,
+// up to 1 GiB of wide workspace).  Every entry's mutex is taken first, so no call is between taking its entry and its
+// last launch; the device synchronisation then waits for the launches already enqueued.
+inline int release_stream_scratch() {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return RB_ERR_CUDA;
+  std::vector<StreamScratch*> mine;
+  {
+    std::lock_guard<std::mutex> lk(g_scratch_mu);
+    for (auto& kv : g_scratch)
+      if (kv.first.first == dev) mine.push_back(&kv.second);
+  }
+  std::vector<std::unique_lock<std::mutex>> held;
+  for (StreamScratch* S : mine) held.emplace_back(S->mu);
+  cudaDeviceSynchronize();
+  for (StreamScratch* S : mine)
+    for (ScratchBuf* b : {&S->tasks, &S->results, &S->count, &S->mcc, &S->wide}) { cudaFree(b->p); *b = ScratchBuf(); }
+  return RB_OK;
 }
 
 }  // namespace rb

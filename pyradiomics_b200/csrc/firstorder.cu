@@ -11,19 +11,11 @@
 //                            window holds a NaN), block_compact_levels' classes.  The same bits as firstorder_voxel.
 #include "common.cuh"
 #include "firstorder.cuh"
-#include "host_common.hpp"
 #include "pixel.cuh"
 #include "voxel_tiles.cuh"
 #include "wide_window.cuh"
 
 namespace rb {
-
-struct FoParams {
-  int Z, Y, X;
-  long long sz, sy;    // element strides of the (contiguous) image, mask and level volumes
-  int rz, ry, rx, z0, z1, out_z0, dtype, level_bytes;
-  double shift, voxel_volume, init_value;
-};
 
 // the generic window of centre (z, y, x): the intensities of the in-volume, in-mask voxels and every position's level
 // (0 = not in the kernel), then firstorder_voxel<WCAP>
@@ -236,54 +228,40 @@ firstorder_wide_kernel(const void* __restrict__ img, const uint8_t* __restrict__
   }
 }
 
-static FoParams fo_params(int dtype, int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift,
-                          double voxel_volume, double init_value, int z0, int z1, int out_z0) {
-  return FoParams{Z, Y, X, (long long)Y * X, X, rz, ry, rx, z0, z1, out_z0, dtype, level_bytes, shift, voxel_volume,
-                  init_value};
-}
-
-int firstorder_fast_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
-                           int Z, int Y, int X, double shift, double voxel_volume, double init_value, double* out,
-                           long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
-  const FoParams P = fo_params(dtype, 1, Z, Y, X, 1, 1, 1, shift, voxel_volume, init_value, z0, z1, out_z0);
-  const long long total = (long long)(z1 - z0) * Y * X;
+int firstorder_fast_launch(const FoLaunch& A) {
+  const long long total = (long long)(A.P.z1 - A.P.z0) * A.P.Y * A.P.X;
   if (total <= 0) return RB_OK;
   int grid = 0;
   RB_CUDA(resident_grid(firstorder_tiles_kernel<FO_NT>, FO_NT, 0, total, grid));
-  firstorder_tiles_kernel<FO_NT><<<grid, FO_NT, 0, st>>>(img, mask, centers, (const uint8_t*)lev, P, out, fstride);
+  firstorder_tiles_kernel<FO_NT><<<grid, FO_NT, 0, A.st>>>(A.img, A.mask, A.centers, (const uint8_t*)A.lev, A.P, A.out,
+                                                           A.fstride);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }
 
-int firstorder_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
-                      int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
-                      double init_value, double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
-  const FoParams P = fo_params(dtype, level_bytes, Z, Y, X, rz, ry, rx, shift, voxel_volume, init_value, z0, z1, out_z0);
-  const long long total = (long long)(z1 - z0) * Y * X;
+int firstorder_launch(const FoLaunch& A) {
+  const FoParams& P = A.P;
+  const long long total = (long long)(P.z1 - P.z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
-  const int grid = grid_for(total, 128, 32);
-  const int wcap = (2 * rz + 1) * (2 * ry + 1) * (2 * rx + 1);
-  if (wcap <= 27) firstorder_kernel<27><<<grid, 128, 0, st>>>(img, mask, centers, lev, P, out, fstride);
-  else if (wcap <= 125) firstorder_kernel<125><<<grid, 128, 0, st>>>(img, mask, centers, lev, P, out, fstride);
-  else if (wcap <= 343) firstorder_kernel<343><<<grid, 128, 0, st>>>(img, mask, centers, lev, P, out, fstride);
-  else return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
-  RB_LAUNCH_CHECK();
-  return RB_OK;
+  return with_window_class((2 * P.rz + 1) * (2 * P.ry + 1) * (2 * P.rx + 1), [&](auto wcap) -> int {
+    firstorder_kernel<decltype(wcap)::value><<<grid_for(total, 128, 32), 128, 0, A.st>>>(A.img, A.mask, A.centers, A.lev,
+                                                                                          P, A.out, A.fstride);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+  });
 }
 
-int firstorder_wide_launch(const void* img, int dtype, const uint8_t* mask, const uint8_t* centers, const void* lev,
-                           int level_bytes, int Z, int Y, int X, int rz, int ry, int rx, double shift, double voxel_volume,
-                           double init_value, double* out, long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
-  const FoParams P = fo_params(dtype, level_bytes, Z, Y, X, rz, ry, rx, shift, voxel_volume, init_value, z0, z1, out_z0);
-  const long long total = (long long)(z1 - z0) * Y * X;
+int firstorder_wide_launch(const FoLaunch& A) {
+  const FoParams& P = A.P;
+  const long long total = (long long)(P.z1 - P.z0) * P.Y * P.X;
   if (total <= 0) return RB_OK;
-  const int smem = fo_wide_smem((2 * rz + 1) * (2 * ry + 1) * (2 * rx + 1));
+  const int smem = fo_wide_smem((2 * P.rz + 1) * (2 * P.ry + 1) * (2 * P.rx + 1));
   RB_CUDA(set_max_dynamic_smem(firstorder_wide_kernel, fo_wide_smem(WIDE_WCAP_MAX)));
   int per_sm = 0;
   RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, firstorder_wide_kernel, FO_WIDE_NT, smem));
   long long grid = (long long)sm_count() * (per_sm > 0 ? per_sm : 1);
   if (grid > total) grid = total;
-  firstorder_wide_kernel<<<(int)grid, FO_WIDE_NT, smem, st>>>(img, mask, centers, lev, P, out, fstride);
+  firstorder_wide_kernel<<<(int)grid, FO_WIDE_NT, smem, A.st>>>(A.img, A.mask, A.centers, A.lev, P, A.out, A.fstride);
   RB_LAUNCH_CHECK();
   return RB_OK;
 }

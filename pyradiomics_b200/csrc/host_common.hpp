@@ -1,5 +1,5 @@
 // Host-side helpers shared by the C-ABI (capi.cu) and the test-only host emulation:
-// neighbour-offset ("angle") enumeration, the per-launch parameter block and the rule that picks the fast voxel kernels.
+// neighbour-offset ("angle") enumeration, the per-launch parameter block and the rule that picks each voxel kernel.
 #pragma once
 #include <math.h>
 #include <string.h>
@@ -118,16 +118,26 @@ inline int fill_vox_params(int cls, int Z, int Y, int X, const VoxSettings& s, V
 
 inline int window_capacity(const VoxParams& P) { return (2 * P.rz + 1) * (2 * P.ry + 1) * (2 * P.rx + 1); }
 
-// Which kernel a window of `cap` positions runs on, texture and first order alike (after the r = 1 fast paths below):
-// the thread-per-centre generic kernels up to 7^3 = 343 positions, the block-per-centre wide kernels (voxel_wide.cu,
-// firstorder.cu) up to 15^3 = 3375 (kernelRadius 4 to 7 in 3-D; larger force2D / 2-D windows), nothing beyond.
-// force_wide (B200_RADIOMICS_FORCE_WIDE=1, for tests) sends the generic kernels' windows to the wide kernels too.
-// The host emulation (tests/host_emul) runs the generic path, so it stops at WP_WIDE.
+// The generic kernels' window classes: a window of `positions` runs in the 27-, 125- or 343-position instantiation
+// (kernelRadius 1, 2, 3 in 3-D), and its entry lists are sized by that class; the wide kernels size theirs for
+// WIDE_WCAP_MAX above 343 positions.
 constexpr int GENERIC_WCAP_MAX = 343, WIDE_WCAP_MAX = 3375;
-enum WindowPath { WP_GENERIC, WP_WIDE, WP_UNSUPPORTED };
-inline WindowPath window_path(int cap, bool force_wide) {
-  if (cap > WIDE_WCAP_MAX) return WP_UNSUPPORTED;
-  return cap > GENERIC_WCAP_MAX || force_wide ? WP_WIDE : WP_GENERIC;
+constexpr int window_class(int positions) {
+  return positions <= 27 ? 27 : positions <= 125 ? 125 : positions <= GENERIC_WCAP_MAX ? GENERIC_WCAP_MAX : WIDE_WCAP_MAX;
+}
+
+// Which kernel a voxel-map launch runs on, texture and first order alike: the r = 1 fast kernel when it fits
+// (fast_fits: voxel_fast_path / firstorder_fast_path below), else the thread-per-centre generic kernels up to 7^3 = 343
+// positions, the block-per-centre wide kernels (voxel_wide.cu, firstorder.cu) up to 15^3 = 3375 (kernelRadius 4 to 7 in
+// 3-D; larger force2D / 2-D windows), nothing beyond.  Two overrides, for tests: force_wide
+// (B200_RADIOMICS_FORCE_WIDE=1) sends every window, fast and generic ones included, to the wide kernels; force_generic
+// (B200_RADIOMICS_FORCE_GENERIC=1) declines the fast kernel.  The host emulation (tests/host_emul) returns the values
+// as they are, and runs the generic path, so it stops at WP_WIDE.
+enum WindowPath { WP_GENERIC, WP_WIDE, WP_UNSUPPORTED, WP_FAST };
+inline WindowPath window_path(int positions, bool force_wide, bool fast_fits = false, bool force_generic = false) {
+  if (fast_fits && !force_generic && !force_wide) return WP_FAST;
+  if (positions > WIDE_WCAP_MAX) return WP_UNSUPPORTED;
+  return positions > GENERIC_WCAP_MAX || force_wide ? WP_WIDE : WP_GENERIC;
 }
 
 // Whether texture class cls runs its kernelRadius-1 fast kernel (voxel_fast_launch) rather than the generic one: 8-bit

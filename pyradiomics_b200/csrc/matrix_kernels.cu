@@ -7,7 +7,6 @@
 //                  voxel-based features never materialise these (see voxel_kernels.cu / voxel_fast.cu).
 // GLSZM is two-phase in both modes: phase one leaves its zones in a GlszmHandle, glszm_fill turns them into the matrix.
 #include "common.cuh"
-#include "host_common.hpp"
 #include "vox_features.cuh"
 
 namespace rb {
@@ -240,19 +239,17 @@ static BatchGeom batch_geom(const Prepared& R, int kernelRadius, int nvox) {
   return G;
 }
 
-template <typename T, int MODE>
+template <int MODE>
 static int launch_batch(const Prepared& R, const BatchGeom& G, int Ng, int Nr, int alpha, double* out) {
-  const int cap = (2 * G.rz + 1) * (2 * G.ry + 1) * (2 * G.rx + 1);
-  const int grid = (G.nvox + 127) / 128;
-  const T* lev = R.lev.as<const T>();
-  const int* vox = R.vox.as<const int>();
-  int* st = R.status.as<int>();
-  if (cap <= 27) batch_matrix_kernel<T, 27, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out, st);
-  else if (cap <= 125) batch_matrix_kernel<T, 125, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out, st);
-  else if (cap <= 343) batch_matrix_kernel<T, 343, MODE><<<grid, 128>>>(lev, G, vox, R.G.A, Ng, Nr, alpha, out, st);
-  else return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
-  RB_LAUNCH_CHECK();
-  return RB_OK;
+  return with_level_type(R.lb, [&](auto lt) -> int {
+    return with_window_class((2 * G.rz + 1) * (2 * G.ry + 1) * (2 * G.rx + 1), [&](auto wcap) -> int {
+      using T = decltype(lt);
+      batch_matrix_kernel<T, decltype(wcap)::value, MODE><<<(G.nvox + 127) / 128, 128>>>(
+          R.lev.as<const T>(), G, R.vox.as<const int>(), R.G.A, Ng, Nr, alpha, out, R.status.as<int>());
+      RB_LAUNCH_CHECK();
+      return RB_OK;
+    });
+  });
 }
 
 // one driver for GLCM (mode 0) / GLDM (1) / NGTDM (2) / GLRLM (3) from host image + mask
@@ -282,9 +279,8 @@ int calculate_matrix_host(int mode, const int32_t* image, const uint8_t* mask, c
   RB_CUDA(cudaMemsetAsync(dout.p, 0, sizeof(double) * per * nvox, 0));
   double* out = dout.as<double>();
   BatchGeom G = batch_geom(R, kernelRadius, nvox);
-#define RB_B(MODE) (R.lb == 1 ? launch_batch<uint8_t, MODE>(R, G, Ng, Nr, alpha, out) : launch_batch<uint16_t, MODE>(R, G, Ng, Nr, alpha, out))
-  rc = mode == 0 ? RB_B(0) : mode == 1 ? RB_B(1) : mode == 2 ? RB_B(2) : RB_B(3);
-#undef RB_B
+  rc = mode == 0 ? launch_batch<0>(R, G, Ng, Nr, alpha, out) : mode == 1 ? launch_batch<1>(R, G, Ng, Nr, alpha, out)
+     : mode == 2 ? launch_batch<2>(R, G, Ng, Nr, alpha, out) : launch_batch<3>(R, G, Ng, Nr, alpha, out);
   if (rc) return rc;
   rc = check_status(R, names[mode]);
   if (rc) return rc;
@@ -305,23 +301,24 @@ int glszm_zones_host(const int32_t* image, const uint8_t* mask, const int* size,
   if (rc) return rc;
   if (!voxels) return segment_glszm(R.lev.p, R.lb, size, nd, Ng, force2D, force2Ddimension, max_region_out, handle_out, 0);
   BatchGeom G = batch_geom(R, kernelRadius, nvox);
-  const int cap = (2 * G.rz + 1) * (2 * G.ry + 1) * (2 * G.rx + 1);
-  const int wcap = cap <= 27 ? 27 : cap <= 125 ? 125 : 343;
-  if (cap > 343) return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
   std::unique_ptr<GlszmHandle> H(new GlszmHandle);   // handed to the caller only on success
-  H->batch = true; H->nvox = nvox; H->wcap = wcap;
-  RB_CUDA(H->zones.alloc(sizeof(int) * 2 * (size_t)wcap * nvox));
-  RB_CUDA(H->nz.alloc(sizeof(int) * (size_t)nvox));
   DevBuf mx;
-  RB_CUDA(mx.alloc(4));
-  RB_CUDA(cudaMemsetAsync(mx.p, 0, 4, 0));
-  const int grid = (nvox + 127) / 128;
-  const int* vox = R.vox.as<const int>();
-#define RB_Z(T, W) batch_glszm_zones_kernel<T, W><<<grid, 128>>>(R.lev.as<const T>(), G, vox, R.G.A, H->zones.as<int>(), H->nz.as<int>(), mx.as<unsigned>())
-  if (R.lb == 1) { if (wcap == 27) RB_Z(uint8_t, 27); else if (wcap == 125) RB_Z(uint8_t, 125); else RB_Z(uint8_t, 343); }
-  else { if (wcap == 27) RB_Z(uint16_t, 27); else if (wcap == 125) RB_Z(uint16_t, 125); else RB_Z(uint16_t, 343); }
-#undef RB_Z
-  RB_LAUNCH_CHECK();
+  rc = with_window_class((2 * G.rz + 1) * (2 * G.ry + 1) * (2 * G.rx + 1), [&](auto wcap) -> int {
+    constexpr int WCAP = decltype(wcap)::value;
+    H->batch = true; H->nvox = nvox; H->wcap = WCAP;
+    RB_CUDA(H->zones.alloc(sizeof(int) * 2 * (size_t)WCAP * nvox));
+    RB_CUDA(H->nz.alloc(sizeof(int) * (size_t)nvox));
+    RB_CUDA(mx.alloc(4));
+    RB_CUDA(cudaMemsetAsync(mx.p, 0, 4, 0));
+    return with_level_type(R.lb, [&](auto lt) -> int {
+      using T = decltype(lt);
+      batch_glszm_zones_kernel<T, WCAP><<<(nvox + 127) / 128, 128>>>(R.lev.as<const T>(), G, R.vox.as<const int>(), R.G.A,
+                                                                      H->zones.as<int>(), H->nz.as<int>(), mx.as<unsigned>());
+      RB_LAUNCH_CHECK();
+      return RB_OK;
+    });
+  });
+  if (rc) return rc;
   unsigned max_region = 0;
   RB_CUDA(cudaMemcpy(&max_region, mx.p, 4, cudaMemcpyDeviceToHost));
   *max_region_out = (int)max_region;

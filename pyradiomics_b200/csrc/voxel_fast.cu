@@ -2,78 +2,14 @@
 // distances [1], 8-bit levels).  One thread per centre voxel, consecutive threads = consecutive
 // x so the 24 float64 map stores of a warp are 256-byte coalesced segments (128-byte for float32 maps).
 // Every kernel and launch function takes the map type (double or float, store_map in voxel_tiles.cuh).
-#include <map>
-#include <mutex>
-#include <vector>
-
 #include "common.cuh"
 #define RB_GLCM_BLOCK_SYNC 1   // phase A is called by all threads of a block, uniformly
 #include "glcm_fast.cuh"
 #include "glcm_kernels.cuh"
 #include "glrlm_fast.cuh"
 #include "small_fast.cuh"
-#include "host_common.hpp"
 
 namespace rb {
-
-// per (device, stream) task queue, grown on demand; float maps add the float64 partial-MCC plane of a chunk (mcc,
-// mcc_cap doubles).  `mu` is held from taking the queue until the last launch that uses it is enqueued, so two host
-// threads on one stream enqueue their chunk sequences one after the other, and a growth or a release never frees a
-// buffer a call is still about to launch on.  Entries are never erased (a std::map node does not move), so a pointer to
-// one stays valid after g_queue_mu is dropped.
-struct GlcmQueue {
-  GlcmTask* q = nullptr; double* res = nullptr; unsigned* count = nullptr; size_t cap = 0;
-  double* mcc = nullptr; size_t mcc_cap = 0;
-  std::mutex mu;
-};
-static std::mutex g_queue_mu;   // the map only
-static std::map<std::pair<int, cudaStream_t>, GlcmQueue> g_queue_cache;
-// rb_release_device_caches: give the eigen-task queues of the current device back (up to 1.15 GB per stream that ran
-// GLCM).  Every queue's lock is taken first, so no call is between taking a queue and its last launch; the device
-// synchronisation then waits for the launches already enqueued.
-int glcm_release_queues() {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return RB_ERR_CUDA;
-  std::vector<std::unique_lock<std::mutex>> held;
-  std::vector<GlcmQueue*> mine;
-  {
-    std::lock_guard<std::mutex> lk(g_queue_mu);
-    for (auto& kv : g_queue_cache)
-      if (kv.first.first == dev) mine.push_back(&kv.second);
-  }
-  for (GlcmQueue* Q : mine) held.emplace_back(Q->mu);
-  cudaDeviceSynchronize();
-  for (GlcmQueue* Q : mine) {
-    cudaFree(Q->q); cudaFree(Q->res); cudaFree(Q->count); cudaFree(Q->mcc);
-    Q->q = nullptr; Q->res = nullptr; Q->count = nullptr; Q->mcc = nullptr; Q->cap = Q->mcc_cap = 0;
-  }
-  return RB_OK;
-}
-// the queue of (current device, st), grown to `need` tasks and `mcc_need` partial-MCC doubles, with its lock held in lk
-static GlcmQueue* glcm_queue(cudaStream_t st, size_t need, size_t mcc_need, std::unique_lock<std::mutex>& lk) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  GlcmQueue* entry;
-  {
-    std::lock_guard<std::mutex> mlk(g_queue_mu);
-    entry = &g_queue_cache[{dev, st}];
-  }
-  lk = std::unique_lock<std::mutex>(entry->mu);
-  GlcmQueue& Q = *entry;
-  if (!Q.count && cudaMalloc(&Q.count, sizeof(unsigned)) != cudaSuccess) return nullptr;
-  if (Q.cap < need) {
-    if (Q.q) { cudaStreamSynchronize(st); cudaFree(Q.q); cudaFree(Q.res); Q.q = nullptr; Q.res = nullptr; Q.cap = 0; }
-    if (cudaMalloc(&Q.q, need * sizeof(GlcmTask)) != cudaSuccess) return nullptr;
-    if (cudaMalloc(&Q.res, need * sizeof(double)) != cudaSuccess) { cudaFree(Q.q); Q.q = nullptr; return nullptr; }
-    Q.cap = need;
-  }
-  if (Q.mcc_cap < mcc_need) {
-    if (Q.mcc) { cudaStreamSynchronize(st); cudaFree(Q.mcc); Q.mcc = nullptr; Q.mcc_cap = 0; }
-    if (cudaMalloc(&Q.mcc, mcc_need * sizeof(double)) != cudaSuccess) return nullptr;
-    Q.mcc_cap = mcc_need;
-  }
-  return &Q;
-}
 
 template <typename OutT>
 static int glcm_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
@@ -96,9 +32,15 @@ static int glcm_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxPar
   // float maps: phase A keeps the partial MCC of the voxels with eigen-tasks in float64 (zchunk planes), so the finished
   // MCC is rounded to float once
   constexpr bool f64 = std::is_same<OutT, double>::value;
-  std::unique_lock<std::mutex> qlk;      // held until the last chunk's finish kernel is enqueued
-  GlcmQueue* Q = glcm_queue(st, (size_t)zchunk * plane * GF_NA, f64 ? 0 : (size_t)zchunk * plane, qlk);
-  if (!Q) return fail(RB_ERR_NOMEM, "could not allocate the GLCM eigen-task queue");
+  const size_t ntasks = (size_t)zchunk * plane * GF_NA, nmcc = f64 ? 0 : (size_t)zchunk * plane;
+  std::unique_lock<std::mutex> lk;       // held until the last chunk's finish kernel is enqueued
+  StreamScratch* S = stream_scratch(st, lk);
+  if (!S || !S->grow(S->count, sizeof(unsigned)) || !S->grow(S->tasks, ntasks * sizeof(GlcmTask)) ||
+      !S->grow(S->results, ntasks * sizeof(double)) || !S->grow(S->mcc, nmcc * sizeof(double)))
+    return fail(RB_ERR_NOMEM, "could not allocate the GLCM eigen-task queue");
+  GlcmTask* q = S->tasks.as<GlcmTask>();
+  double *res = S->results.as<double>(), *mcc = S->mcc.as<double>();
+  unsigned* count = S->count.as<unsigned>();
   // phase A: one CTA per SM (register-bound).  512 threads at 128 registers (a hundred spilled words per thread, L1-
   // resident) put 16 warps on an SM instead of the 8 of a 256-thread / 236-register build, which hides more of the
   // latency of this issue-bound kernel.
@@ -109,22 +51,21 @@ static int glcm_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxPar
   RB_CUDA(set_max_dynamic_smem(glcm_fast_solve_kernel<2>, GF_LZ_SMEM_BYTES));
   for (int za = z0; za < z1; za += zchunk) {
     const int zb = za + zchunk < z1 ? za + zchunk : z1;
-    RB_CUDA(cudaMemsetAsync(Q->count, 0, sizeof(unsigned), st));
+    RB_CUDA(cudaMemsetAsync(count, 0, sizeof(unsigned), st));
     int grid = 0;
     RB_CUDA(resident_grid(glcm_fast_kernel<1, NT, OutT>, NT, smem, (long long)(zb - za) * plane, grid));
-    glcm_fast_kernel<1, NT, OutT><<<grid, NT, smem, st>>>(l8, centers, P, T, out, fstride, za, zb, out_z0, Q->q, Q->count,
-                                                         Q->mcc);
+    glcm_fast_kernel<1, NT, OutT><<<grid, NT, smem, st>>>(l8, centers, P, T, out, fstride, za, zb, out_z0, q, count, mcc);
     RB_LAUNCH_CHECK();
     // One launch per size group keeps ONE solver body in the instruction cache (the three Lanczos templates together are
     // 18.5 k SASS instructions, 296 KB, and on a smooth volume the blocks of an SM otherwise sit in different groups); the
     // dense n <= 8 solves stay a single launch, where the repeated tile sorts would cost more than they save.
-    glcm_fast_solve_kernel<0><<<sms * 8, 128, 0, st>>>(l8, P, T, Q->q, Q->count, Q->res, 0);
-    for (int g = 10; g <= 12; g += 2) glcm_fast_solve_kernel<1><<<sms * 8, 128, 0, st>>>(l8, P, T, Q->q, Q->count, Q->res, g);
+    glcm_fast_solve_kernel<0><<<sms * 8, 128, 0, st>>>(l8, P, T, q, count, res, 0);
+    for (int g = 10; g <= 12; g += 2) glcm_fast_solve_kernel<1><<<sms * 8, 128, 0, st>>>(l8, P, T, q, count, res, g);
     for (int g = 18; g >= 14; g -= 2)
-      glcm_fast_solve_kernel<2><<<sms * 2, 128, GF_LZ_SMEM_BYTES, st>>>(l8, P, T, Q->q, Q->count, Q->res, g);
+      glcm_fast_solve_kernel<2><<<sms * 2, 128, GF_LZ_SMEM_BYTES, st>>>(l8, P, T, q, count, res, g);
     RB_LAUNCH_CHECK();
-    glcm_fast_finish_kernel<OutT><<<sms * 8, 256, 0, st>>>(P, Q->q, Q->count, Q->res, out + (long long)G_MCC * fstride,
-                                                           out_z0, Q->mcc, za);
+    glcm_fast_finish_kernel<OutT><<<sms * 8, 256, 0, st>>>(P, q, count, res, out + (long long)G_MCC * fstride,
+                                                           out_z0, mcc, za);
     RB_LAUNCH_CHECK();
   }
   return RB_OK;
@@ -263,25 +204,20 @@ static int tiles_fast_run(const uint8_t* l8, const uint8_t* centers, const VoxPa
 }
 
 // ------------------------------------------------------------------------------------ the entry
-template <typename OutT>
-static int fast_run(int cls, const uint8_t* l8, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
-                    int z0, int z1, int out_z0, cudaStream_t st) {
-  switch (cls) {
-    case C_GLCM: return glcm_fast_run(l8, centers, P, out, fstride, z0, z1, out_z0, st);
-    case C_GLRLM: return glrlm_fast_run(l8, centers, P, out, fstride, z0, z1, out_z0, st);
-    case C_GLSZM: return tiles_fast_run<C_GLSZM>(l8, centers, P, out, fstride, z0, z1, out_z0, st);
-    case C_GLDM: return tiles_fast_run<C_GLDM>(l8, centers, P, out, fstride, z0, z1, out_z0, st);
-    default: return tiles_fast_run<C_NGTDM>(l8, centers, P, out, fstride, z0, z1, out_z0, st);
-  }
-}
-
-// the fast kernels of class cls, for settings voxel_fast_path (host_common.hpp) accepts: `out` holds float maps when
-// out_f32, else double
-int voxel_fast_launch(int cls, const void* lev, const uint8_t* centers, const VoxParams& P, void* out, bool out_f32,
-                      long long fstride, int z0, int z1, int out_z0, cudaStream_t st) {
-  const uint8_t* l8 = (const uint8_t*)lev;
-  if (out_f32) return fast_run(cls, l8, centers, P, (float*)out, fstride, z0, z1, out_z0, st);
-  return fast_run(cls, l8, centers, P, (double*)out, fstride, z0, z1, out_z0, st);
+// the fast kernels of class A.cls, for settings voxel_fast_path (host_common.hpp) accepts
+int voxel_fast_launch(const VoxLaunch& A) {
+  return with_map_type(A.out_f32, [&](auto ot) -> int {
+    using OutT = decltype(ot);
+    const uint8_t* l8 = (const uint8_t*)A.lev;
+    OutT* out = (OutT*)A.out;
+    switch (A.cls) {
+      case C_GLCM: return glcm_fast_run(l8, A.centers, A.P, out, A.fstride, A.z0, A.z1, A.out_z0, A.st);
+      case C_GLRLM: return glrlm_fast_run(l8, A.centers, A.P, out, A.fstride, A.z0, A.z1, A.out_z0, A.st);
+      case C_GLSZM: return tiles_fast_run<C_GLSZM>(l8, A.centers, A.P, out, A.fstride, A.z0, A.z1, A.out_z0, A.st);
+      case C_GLDM: return tiles_fast_run<C_GLDM>(l8, A.centers, A.P, out, A.fstride, A.z0, A.z1, A.out_z0, A.st);
+      default: return tiles_fast_run<C_NGTDM>(l8, A.centers, A.P, out, A.fstride, A.z0, A.z1, A.out_z0, A.st);
+    }
+  });
 }
 
 }  // namespace rb

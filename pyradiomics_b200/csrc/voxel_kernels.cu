@@ -4,7 +4,6 @@
 // any kernelRadius <= 3, distances subset {1,2,3}, force2D, asymmetric / weighted GLCM, uint8 or
 // uint16 levels, float64 or float32 maps (store_map).  The r=1 fast path lives in voxel_fast.cu.
 #include "common.cuh"
-#include "host_common.hpp"
 #include "vox_features.cuh"
 #include "voxel_tiles.cuh"
 
@@ -94,61 +93,47 @@ pack_levels_kernel(const int32_t* __restrict__ image, const uint8_t* __restrict_
   if (bad && status) atomicOr(status, 1);
 }
 
-template <typename T, int WCAP, typename OutT>
-static int launch_cls(int cls, bool weighted, const T* lev, const uint8_t* centers, const VoxParams& P, OutT* out,
-                      long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
-  const long long total = (long long)(z1 - z0) * P.Y * P.X;
-  if (total <= 0) return RB_OK;
-  const int grid = grid_for(total, 128, 64);
-#define RB_GO(CLS, WGT) voxel_features_kernel<T, WCAP, CLS, WGT, OutT><<<grid, 128, 0, st>>>(lev, centers, P, out, fstride, z0, z1, out_z0, status)
-  switch (cls) {
-    case C_GLCM: if (weighted) RB_GO(C_GLCM, true); else RB_GO(C_GLCM, false); break;
-    case C_GLRLM: if (weighted) RB_GO(C_GLRLM, true); else RB_GO(C_GLRLM, false); break;
-    case C_GLSZM: RB_GO(C_GLSZM, false); break;
-    case C_GLDM: RB_GO(C_GLDM, false); break;
-    case C_NGTDM: RB_GO(C_NGTDM, false); break;
-    default: return fail(RB_ERR_ARG, "unknown texture class %d", cls);
-  }
-#undef RB_GO
-  RB_LAUNCH_CHECK();
-  return RB_OK;
-}
-
-template <typename T, typename OutT>
-static int launch_generic(int cls, const T* lev, const uint8_t* centers, const VoxParams& P, OutT* out,
-                          long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
-  const int cap = window_capacity(P);
-  const bool wgt = P.weighted != 0;
-  if (cap <= 27) return launch_cls<T, 27, OutT>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  if (cap <= 125) return launch_cls<T, 125, OutT>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  if (cap <= 343) return launch_cls<T, 343, OutT>(cls, wgt, lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  return fail(RB_ERR_UNSUPPORTED, "kernelRadius > 3 is outside the implemented envelope");
-}
-
-template <typename OutT>
-static int generic_run(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P,
-                       OutT* out, long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
-  if (level_bytes == 1) return launch_generic(cls, (const uint8_t*)lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  if (level_bytes == 2) return launch_generic(cls, (const uint16_t*)lev, centers, P, out, fstride, z0, z1, out_z0, status, st);
-  return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
-}
-
-int voxel_features_generic(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P,
-                           void* out, bool out_f32, long long fstride, int z0, int z1, int out_z0, int* status,
-                           cudaStream_t st) {
-  if (out_f32) return generic_run(cls, lev, level_bytes, centers, P, (float*)out, fstride, z0, z1, out_z0, status, st);
-  return generic_run(cls, lev, level_bytes, centers, P, (double*)out, fstride, z0, z1, out_z0, status, st);
+int voxel_features_generic(const VoxLaunch& A) {
+  const long long total = (long long)(A.z1 - A.z0) * A.P.Y * A.P.X;
+  return with_level_type(A.level_bytes, [&](auto lt) -> int {
+    return with_window_class(window_capacity(A.P), [&](auto wcap) -> int {
+      return with_map_type(A.out_f32, [&](auto ot) -> int {
+        using T = decltype(lt);
+        using OutT = decltype(ot);
+        constexpr int WCAP = decltype(wcap)::value;
+        if (total <= 0) return RB_OK;
+        auto launch = [&](auto kernel) -> int {
+          kernel<<<grid_for(total, 128, 64), 128, 0, A.st>>>((const T*)A.lev, A.centers, A.P, (OutT*)A.out, A.fstride,
+                                                             A.z0, A.z1, A.out_z0, A.status);
+          RB_LAUNCH_CHECK();
+          return RB_OK;
+        };
+        const bool wgt = A.P.weighted != 0;
+        switch (A.cls) {
+          case C_GLCM: return wgt ? launch(voxel_features_kernel<T, WCAP, C_GLCM, true, OutT>)
+                                  : launch(voxel_features_kernel<T, WCAP, C_GLCM, false, OutT>);
+          case C_GLRLM: return wgt ? launch(voxel_features_kernel<T, WCAP, C_GLRLM, true, OutT>)
+                                   : launch(voxel_features_kernel<T, WCAP, C_GLRLM, false, OutT>);
+          case C_GLSZM: return launch(voxel_features_kernel<T, WCAP, C_GLSZM, false, OutT>);
+          case C_GLDM: return launch(voxel_features_kernel<T, WCAP, C_GLDM, false, OutT>);
+          case C_NGTDM: return launch(voxel_features_kernel<T, WCAP, C_NGTDM, false, OutT>);
+          default: return fail(RB_ERR_ARG, "unknown texture class %d", A.cls);
+        }
+      });
+    });
+  });
 }
 
 int glcm_alive_angles(const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P, uint32_t* alive,
                       cudaStream_t st) {
   const long long total = (long long)P.Z * P.Y * P.X;
   const int grid = grid_for(total, 256, 8);
-  if (level_bytes == 1) glcm_alive_kernel<uint8_t><<<grid, 256, 0, st>>>((const uint8_t*)lev, centers, P, alive);
-  else if (level_bytes == 2) glcm_alive_kernel<uint16_t><<<grid, 256, 0, st>>>((const uint16_t*)lev, centers, P, alive);
-  else return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
-  RB_LAUNCH_CHECK();
-  return RB_OK;
+  return with_level_type(level_bytes, [&](auto lt) -> int {
+    using T = decltype(lt);
+    glcm_alive_kernel<T><<<grid, 256, 0, st>>>((const T*)lev, centers, P, alive);
+    RB_LAUNCH_CHECK();
+    return RB_OK;
+  });
 }
 
 int pack_levels(const int32_t* image, const uint8_t* mask, long long n, int Ng, void* lev, uint32_t* presence,

@@ -9,12 +9,7 @@
 // Each entry list is built by the same Entries::add sequence as the generic kernel's, so its entries, their order and
 // every floating-point sum are the generic kernel's: the maps are bit-identical wherever both run
 // (B200_RADIOMICS_FORCE_WIDE=1 sends windows <= 343 here to show it).
-#include <map>
-#include <mutex>
-#include <vector>
-
 #include "common.cuh"
-#include "host_common.hpp"
 #include "vox_features.cuh"
 #include "voxel_tiles.cuh"
 #include "wide_window.cuh"
@@ -253,16 +248,13 @@ wide_voxel_kernel(const T* __restrict__ lev, const uint8_t* __restrict__ centers
   }
 }
 
-// the window capacity the generic kernel would give a window of wn positions (its semantic list limits follow it)
-static int generic_wcap(int wn) { return wn <= 27 ? 27 : wn <= 125 ? 125 : wn <= 343 ? 343 : WIDE_WCAP_MAX; }
-
 static WideLayout wide_layout(int cls, const VoxParams& P) {
   WideLayout L = {};
   L.cls = cls;
   L.wn = window_capacity(P);
   L.ncap = L.wn < P.Ng ? L.wn : P.Ng;
   const long long pairs = (long long)L.ncap * L.ncap;
-  const int wcap = generic_wcap(L.wn);
+  const int wcap = window_class(L.wn);            // the generic kernel's class: its semantic list limits follow it
   if (cls == C_GLCM && P.weighted) {
     L.ecap = wcap <= 27 ? wcap * wcap : 2048;                  // glcm_voxel's ECAP and KCAP: overflow is status bit 1
     L.kcap = L.ecap < 1024 ? L.ecap : 1024;
@@ -283,51 +275,6 @@ static WideLayout wide_layout(int cls, const VoxParams& P) {
   return L;
 }
 
-// per (device, stream) workspace, grown on demand.  `mu` is held from taking the workspace until the kernel that uses it
-// is enqueued (voxel_fast.cu's GlcmQueue does the same): a second host thread on the stream cannot free it under a call
-// that has not launched yet, and its own launch follows the first in stream order.  Entries are never erased.
-struct WideWorkspace {
-  void* p = nullptr;
-  size_t bytes = 0;
-  std::mutex mu;
-};
-static std::mutex g_ws_mu;   // the map only
-static std::map<std::pair<int, cudaStream_t>, WideWorkspace> g_ws_cache;
-
-int wide_release_workspace() {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return RB_ERR_CUDA;
-  std::vector<std::unique_lock<std::mutex>> held;
-  std::vector<WideWorkspace*> mine;
-  {
-    std::lock_guard<std::mutex> lk(g_ws_mu);
-    for (auto& kv : g_ws_cache)
-      if (kv.first.first == dev) mine.push_back(&kv.second);
-  }
-  for (WideWorkspace* W : mine) held.emplace_back(W->mu);
-  cudaDeviceSynchronize();
-  for (WideWorkspace* W : mine) { cudaFree(W->p); W->p = nullptr; W->bytes = 0; }
-  return RB_OK;
-}
-
-// the workspace of (current device, st), at least `need` bytes, with its lock held in lk
-static uint8_t* wide_workspace(cudaStream_t st, size_t need, std::unique_lock<std::mutex>& lk) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  WideWorkspace* W;
-  {
-    std::lock_guard<std::mutex> mlk(g_ws_mu);
-    W = &g_ws_cache[{dev, st}];
-  }
-  lk = std::unique_lock<std::mutex>(W->mu);
-  if (W->bytes < need) {
-    if (W->p) { cudaStreamSynchronize(st); cudaFree(W->p); W->p = nullptr; W->bytes = 0; }
-    if (cudaMalloc(&W->p, need) != cudaSuccess) { W->p = nullptr; return nullptr; }
-    W->bytes = need;
-  }
-  return (uint8_t*)W->p;
-}
-
 // one resident wave of blocks (the occupancy at this window's shared memory), at most one block per centre, and no
 // more than WIDE_WS_MAX bytes of workspace
 template <typename K>
@@ -342,44 +289,40 @@ static int wide_grid(K* kernel, int smem, long long total, long long block_bytes
   return RB_OK;
 }
 
-template <typename T, typename OutT>
-static int wide_run(int cls, const T* lev, const uint8_t* centers, const VoxParams& P, OutT* out, long long fstride,
-                    int z0, int z1, int out_z0, int* status, cudaStream_t st) {
-  const long long total = (long long)(z1 - z0) * P.Y * P.X;
-  if (total <= 0) return RB_OK;
-  const WideLayout L = wide_layout(cls, P);
-  const int smem = 12 * L.wn;
-  const bool wgt = P.weighted != 0;
-  auto launch = [&](auto kernel) -> int {
-    int grid = 0;
-    if (int rc = wide_grid(kernel, smem, total, L.block_bytes, grid)) return rc;
-    std::unique_lock<std::mutex> wlk;    // held until the kernel is enqueued
-    uint8_t* ws = wide_workspace(st, (size_t)grid * L.block_bytes, wlk);
-    if (!ws) return fail(RB_ERR_NOMEM, "could not allocate the wide voxel kernel's workspace (%lld bytes)",
-                         (long long)grid * L.block_bytes);
-    kernel<<<grid, WIDE_NT, smem, st>>>(lev, centers, P, L, ws, out, fstride, z0, z1, out_z0, status);
-    RB_LAUNCH_CHECK();
-    return RB_OK;
-  };
-  switch (cls) {
-    case C_GLCM: return wgt ? launch(wide_voxel_kernel<T, C_GLCM, true, OutT>) : launch(wide_voxel_kernel<T, C_GLCM, false, OutT>);
-    case C_GLRLM: return wgt ? launch(wide_voxel_kernel<T, C_GLRLM, true, OutT>) : launch(wide_voxel_kernel<T, C_GLRLM, false, OutT>);
-    case C_GLSZM: return launch(wide_voxel_kernel<T, C_GLSZM, false, OutT>);
-    case C_GLDM: return launch(wide_voxel_kernel<T, C_GLDM, false, OutT>);
-    case C_NGTDM: return launch(wide_voxel_kernel<T, C_NGTDM, false, OutT>);
-    default: return fail(RB_ERR_ARG, "unknown texture class %d", cls);
-  }
-}
-
-int voxel_features_wide(int cls, const void* lev, int level_bytes, const uint8_t* centers, const VoxParams& P, void* out,
-                        bool out_f32, long long fstride, int z0, int z1, int out_z0, int* status, cudaStream_t st) {
-  if (level_bytes != 1 && level_bytes != 2) return fail(RB_ERR_ARG, "level_bytes must be 1 or 2");
-  if (out_f32) {
-    if (level_bytes == 1) return wide_run(cls, (const uint8_t*)lev, centers, P, (float*)out, fstride, z0, z1, out_z0, status, st);
-    return wide_run(cls, (const uint16_t*)lev, centers, P, (float*)out, fstride, z0, z1, out_z0, status, st);
-  }
-  if (level_bytes == 1) return wide_run(cls, (const uint8_t*)lev, centers, P, (double*)out, fstride, z0, z1, out_z0, status, st);
-  return wide_run(cls, (const uint16_t*)lev, centers, P, (double*)out, fstride, z0, z1, out_z0, status, st);
+int voxel_features_wide(const VoxLaunch& A) {
+  const VoxParams& P = A.P;
+  const long long total = (long long)(A.z1 - A.z0) * P.Y * P.X;
+  return with_level_type(A.level_bytes, [&](auto lt) -> int {
+    return with_map_type(A.out_f32, [&](auto ot) -> int {
+      using T = decltype(lt);
+      using OutT = decltype(ot);
+      if (total <= 0) return RB_OK;
+      const WideLayout L = wide_layout(A.cls, P);
+      const int smem = 12 * L.wn;
+      auto launch = [&](auto kernel) -> int {
+        int grid = 0;
+        if (int rc = wide_grid(kernel, smem, total, L.block_bytes, grid)) return rc;
+        std::unique_lock<std::mutex> lk;    // held until the kernel is enqueued
+        StreamScratch* S = stream_scratch(A.st, lk);
+        if (!S || !S->grow(S->wide, (size_t)grid * L.block_bytes))
+          return fail(RB_ERR_NOMEM, "could not allocate the wide voxel kernel's workspace (%lld bytes)",
+                      (long long)grid * L.block_bytes);
+        kernel<<<grid, WIDE_NT, smem, A.st>>>((const T*)A.lev, A.centers, P, L, S->wide.as<uint8_t>(), (OutT*)A.out,
+                                              A.fstride, A.z0, A.z1, A.out_z0, A.status);
+        RB_LAUNCH_CHECK();
+        return RB_OK;
+      };
+      const bool wgt = P.weighted != 0;
+      switch (A.cls) {
+        case C_GLCM: return wgt ? launch(wide_voxel_kernel<T, C_GLCM, true, OutT>) : launch(wide_voxel_kernel<T, C_GLCM, false, OutT>);
+        case C_GLRLM: return wgt ? launch(wide_voxel_kernel<T, C_GLRLM, true, OutT>) : launch(wide_voxel_kernel<T, C_GLRLM, false, OutT>);
+        case C_GLSZM: return launch(wide_voxel_kernel<T, C_GLSZM, false, OutT>);
+        case C_GLDM: return launch(wide_voxel_kernel<T, C_GLDM, false, OutT>);
+        case C_NGTDM: return launch(wide_voxel_kernel<T, C_NGTDM, false, OutT>);
+        default: return fail(RB_ERR_ARG, "unknown texture class %d", A.cls);
+      }
+    });
+  });
 }
 
 }  // namespace rb

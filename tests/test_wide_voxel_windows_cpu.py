@@ -1,6 +1,6 @@
 """CPU side of tests/test_wide_voxel_windows_gpu.py: the window oracle (tests/helpers.py: WindowRun, box_features,
 box_mcc) equals the reference pipeline at kernelRadius 4, 5 and 7 on whole small volumes (faces, holes, a 2-D image,
-force2D); the rule that sends windows to the generic or the wide kernels, at its edges; and the oracle's cost per
+force2D); the rule that sends windows to the fast, generic or wide kernels, at its edges; and the oracle's cost per
 window at kernelRadius 7, which sizes the GPU file's corpora."""
 import ctypes as C
 import os
@@ -15,7 +15,7 @@ from helpers import FAST_NAMES, WindowRun, block_corpus, box_features, box_imc2_
 from pyradiomics_b200 import _lib
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-GENERIC, WIDE, UNSUPPORTED = 0, 1, 2
+GENERIC, WIDE, UNSUPPORTED, FAST = 0, 1, 2, 3
 
 
 @pytest.fixture(scope="module")
@@ -24,6 +24,7 @@ def emul(tmp_path_factory):
     subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-o", so, os.path.join(HERE, "host_emul", "window_path_emul.cpp")])
     lib = C.CDLL(so)
     lib.emul_window_path.argtypes = [C.c_int, C.c_int]
+    lib.emul_window_path_fast.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     lib.emul_window_positions.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     return lib
 
@@ -96,6 +97,19 @@ def test_window_path_rule(emul):
         assert emul.emul_window_path(cap, 0) == want, cap
     for cap, want in ((27, WIDE), (343, WIDE), (3375, WIDE), (3376, UNSUPPORTED)):
         assert emul.emul_window_path(cap, 1) == want, cap
+
+
+def test_window_path_fast_kernel_and_generic_override(emul):
+    """window_path with the r = 1 fast kernel fitting: the fast kernel, unless B200_RADIOMICS_FORCE_GENERIC (generic)
+    or B200_RADIOMICS_FORCE_WIDE (wide, also when both are set); the generic override leaves every other window's path
+    as the rule gives it"""
+    assert emul.emul_window_path_fast(27, 0, 1, 0) == FAST
+    assert emul.emul_window_path_fast(27, 0, 1, 1) == GENERIC
+    assert emul.emul_window_path_fast(27, 1, 1, 0) == WIDE
+    assert emul.emul_window_path_fast(27, 1, 1, 1) == WIDE
+    for cap in (27, 343, 344, 3375, 3376, 4913):
+        for wide in (0, 1):
+            assert emul.emul_window_path_fast(cap, wide, 0, 1) == emul.emul_window_path(cap, wide), (cap, wide)
 
 
 @pytest.mark.parametrize("kw,positions,path", [
